@@ -17,6 +17,7 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
     if (a->time_M < a->time_m) return B2_OK;
     std::lock_guard<std::mutex> api_lock(api_mutex());
     if (int rc0 = use_device(a->deviceid)) return rc0;
+    note_sweep_kernel("");
     const int so = a->space_order;
     int rc = B2_OK;
 

@@ -42,6 +42,11 @@ std::mutex &api_mutex();
 void timing_begin();
 void timing_end();
 
+// name of the sweep kernel variant launched (host-side only): read back with b2_last_sweep_kernel, so that a test
+// can tell which of the run-time selected variants ran. Set by the launchers next to timing_begin(); cleared at the
+// start of every b2_iso_forward / b2_tti_forward call.
+void note_sweep_kernel(const char *fmt, ...);
+
 inline void count_launch() { ++g_launches; }
 
 // SMs of the current device (cached on first use; the library serves one device per process);

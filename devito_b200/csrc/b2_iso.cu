@@ -783,6 +783,9 @@ template <int R> struct Tile2Of { static constexpr bool on = false; static const
 // into 255 registers per thread (9 warps would be allocated as 12: 168 registers, and the queues spill)
 template <> struct Tile2Of<6> { static constexpr bool on = true; static constexpr int TY = 28, TZ4 = 16; };
 
+// opt-in dynamic shared memory per block on sm_90 (227 KB)
+constexpr size_t kSmemPerBlockMax = 232448;
+
 
 static int env_int(const char *name, int dflt) {
     const char *v = getenv(name);
@@ -874,8 +877,18 @@ static int plan_tma(IsoPlan &p) {
     int rc;
     // so=12 on an H100: the one-row k_iso_tma (default 0) is faster than variant 4 of k_iso_tma2 (DESIGN §5b)
     p.v2 = Tile2Of<R>::on && p.n[1] >= 16 ? env_int("B2_ISO_V2", 0) : 0;
+    // only variants 1 and 4 exist: any other value would build the two-row tensor maps below and then launch the
+    // one-row kernel over them
+    if (p.v2 != 1 && p.v2 != 4) p.v2 = 0;
     if (p.v2) {
         using T2 = Tile2Of<R>;
+        // variant 4 with an array parameter rings three coefficient tiles: more shared memory than a block may have
+        constexpr size_t smem4 = IsoTma2Cfg<R, T2::TY, T2::TZ4, 0, 3>::SMEM;
+        if (p.v2 == 4 && p.param_kind != B2_PARAM_SCALAR && smem4 > kSmemPerBlockMax) {
+            set_error("iso: B2_ISO_V2=4 with an array-valued vp/m needs %zu bytes of shared memory per block (the "
+                      "device allows %zu); use B2_ISO_V2=0 (the default) or 1", smem4, kSmemPerBlockMax);
+            return B2_ERR_INVALID;
+        }
         if ((rc = make_tmap(&p.tm_uh, p.u, 4, dims4, 4 * T2::TZ4 + 2 * RZ, T2::TY + 2 * R))) return rc;
         // variant 4: u[t-1] and the coefficient tiles by TMA (28 x 64 tiles)
         if ((rc = make_tmap(&p.tm_uc, p.u, 4, dims4, 4 * T2::TZ4, T2::TY))) return rc;
@@ -948,20 +961,28 @@ static int launch_tma(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo
     using C = IsoTmaCfg<R, T::TY, T::TZ4, PK>;
     using C2 = IsoTma2Cfg<R, T2::TY, T2::TZ4>;
     auto kern = k_iso_tma<R, T::TY, T::TZ4, PK>;
-    static bool attr_set = false;
-    if (!attr_set) {
+    // the shared-memory size is opted into per kernel, before its first launch: a variant that cannot run (variant 4
+    // with an array parameter, refused by plan_tma) must not make the others fail
+    static bool attr_set[3] = {false, false, false};      // k_iso_tma, k_iso_tma2 variant 1, variant 4
+    const int v2 = T2::on ? p.v2 : 0;           // 4: TMA tile ring, 1: LDG prefetch (experiment), 0: k_iso_tma
+    if (v2 == 0 && !attr_set[0]) {
         B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM),
                 B2_ERR_LAUNCH);
-        if constexpr (T2::on) {
+        attr_set[0] = true;
+    }
+    if constexpr (T2::on) {
+        if (v2 == 1 && !attr_set[1]) {
             B2_CUDA(cudaFuncSetAttribute(k_iso_tma2<R, T2::TY, T2::TZ4, PK, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)C2::SMEM), B2_ERR_LAUNCH);
-            using C2t = IsoTma2Cfg<R, T2::TY, T2::TZ4, 0, (PK != B2_PARAM_SCALAR ? 3 : 2)>;
+            attr_set[1] = true;
+        }
+        using C2t = IsoTma2Cfg<R, T2::TY, T2::TZ4, 0, (PK != B2_PARAM_SCALAR ? 3 : 2)>;
+        if (v2 == 4 && !attr_set[2]) {
             B2_CUDA(cudaFuncSetAttribute(k_iso_tma2<R, T2::TY, T2::TZ4, PK, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)C2t::SMEM), B2_ERR_LAUNCH);
+            attr_set[2] = true;
         }
-        attr_set = true;
     }
-    const int v2 = T2::on ? p.v2 : 0;           // 4: TMA tile ring (default at so=12), 1: LDG prefetch (experiment)
     const int TYeff = v2 ? T2::TY : T::TY;
     IsoTK<R> k;
     k.u1 = p.u + (size_t)slot1 * p.slot_elems;
@@ -1025,6 +1046,7 @@ static int launch_tma(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo
     k.cA = p.coefA;
     k.cB = p.coefB;
     const unsigned grid = (unsigned)(k.ntz * k.nty * ntx);
+    const char *pk = PK == B2_PARAM_VP ? "vp" : (PK == B2_PARAM_M ? "m" : "scalar");
     timing_begin();
     bool launched = false;
     if constexpr (T2::on) {
@@ -1033,9 +1055,12 @@ static int launch_tma(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo
         if (v2 == 1) k_iso_tma2<R, T2::TY, T2::TZ4, PK, 2><<<grid, nth, C2::SMEM, stream()>>>(p.tm_uh, p.tm_uc, p.tm_damp, p.tm_par, k);
         if (v2 == 4) k_iso_tma2<R, T2::TY, T2::TZ4, PK, 0><<<grid, nth, C2t::SMEM, stream()>>>(p.tm_uh, p.tm_uc, p.tm_damp, p.tm_par, k);
         launched = v2 == 1 || v2 == 4;
+        if (launched) note_sweep_kernel("iso_tma2_v%d<%d,%s>", v2, R, pk);
     }
-    if (!launched)
+    if (!launched) {
         kern<<<grid, T::TY * T::TZ4 + 32, C::SMEM, stream()>>>(p.tm_uh, p.tm_uc, p.tm_damp, p.tm_par, k);
+        note_sweep_kernel("iso_tma<%d,%s>", R, pk);
+    }
     timing_end();
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
@@ -1153,6 +1178,7 @@ int iso_step(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo, int xco
     dim3 block(64, 4, 1);
     dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(xcount, 65535));
     timing_begin();
+    note_sweep_kernel("iso_generic");
     k_iso_generic<<<grid, block, 0, stream()>>>(k);
     timing_end();
     count_launch();

@@ -27,6 +27,15 @@ void set_error(const char *fmt, ...) {
     g_last_error = buf;
 }
 
+static char g_sweep_kernel[64] = "";
+
+void note_sweep_kernel(const char *fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(g_sweep_kernel, sizeof(g_sweep_kernel), fmt, ap);
+    va_end(ap);
+}
+
 static int g_bound_device = -1;
 
 int use_device(int dev) {
@@ -213,6 +222,8 @@ int b2_device_pci_bus_id(int deviceid, char *out, int len) {
 const char *b2_version(void) { return "b200stencil 0.1 (sm_90a)"; }
 
 unsigned long long b2_launch_count(void) { return g_launches; }
+
+const char *b2_last_sweep_kernel(void) { return g_sweep_kernel; }
 
 void b2_kernel_timing_enable(int on) { g_timing_on = on != 0; }
 

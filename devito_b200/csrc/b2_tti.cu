@@ -1221,6 +1221,7 @@ static int tti_launch_fused_arr(const TtiPlan &p, int slot0, int slotm, int slot
     for (int i = 0; i <= R; ++i) { k.w2x[i] = p.w2[0][i]; k.w2y[i] = p.w2[1][i]; k.w2z[i] = p.w2[2][i]; }
     for (int i = 0; i < R; ++i) { k.w1x[i] = p.w1[0][i]; k.w1y[i] = p.w1[1][i]; k.w1z[i] = p.w1[2][i]; }
     timing_begin();
+    note_sweep_kernel("tti_arr_ct%d<%d>", p.arr_ct == 2 ? 2 : (p.arr_ct == 1 ? 1 : 0), R);
     const unsigned nblk = (unsigned)(k.ntz * k.nty * ntx);
     if (p.arr_ct == 2)
         kern2<<<nblk, TY2 * 16 + 32, C2::SMEM, stream()>>>(p.tm_u, p.tm_v, p.tm_cx, p.tm_cy, p.tm_cz, k);
@@ -1297,6 +1298,8 @@ static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, i
         k.p_mdt2 = make_float2(k.m_dt2, k.m_dt2);
     }
     timing_begin();
+    if (ws) note_sweep_kernel("tti_ws<pf%d>", pf == 1 ? 1 : 2);
+    else note_sweep_kernel("tti_fused<%d>", R);
     if (ws)
         kern_ws<<<(unsigned)(k.ntz * k.nty * ntx), kTtiWsTY * 16 + 128, CW::SMEM, stream()>>>(p.tm_u, p.tm_v, k);
     else
@@ -1348,6 +1351,7 @@ int tti_step(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xco
     dim3 block(64, 4, 1);
     dim3 gridA((k.n2 + k.R + 63) / 64, (k.n1 + k.R + 3) / 4, (unsigned)std::min(xcount + k.R, 65535));
     timing_begin();
+    note_sweep_kernel("tti_two_pass");
     k_tti_gz<<<gridA, block, 0, stream()>>>(k);
     count_launch();
     dim3 gridB((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(xcount, 65535));

@@ -1,0 +1,113 @@
+"""Inputs of the kernel-variant matrix (tests/test_kernel_matrix.py on the GPU, tests/test_ref64.py on the CPU).
+
+Every case starts from white noise in all three time slots of the wavefields, halo included, a spatially varying
+damping field and, for array parameters, white-noise parameter fields. The grid is anisotropic and not a cube:
+spacing (10, 12.5, 8), shape (37, 45, 68) -- nx != ny != nz, ny a multiple of none of the sweep kernels' tile
+heights, nz a multiple of 4 but not of the 64-point z tiles. So an exchanged axis, stride or weight list, a wrong
+parameter sample, a skipped partial tile or a swapped time level changes the answer by far more than the tolerance
+(tests/test_ref64.py shows by how much). K = 4 steps: every slot rotation happens once, errors do not pile up.
+"""
+import numpy as np
+
+from oracle import oracle as O
+import ref64
+
+SHAPE = (37, 45, 68)
+SPACING = (10.0, 12.5, 8.0)
+K = 4                                   # time steps 1 .. K
+TOL = {'iso': 1e-5, 'tti': 1e-4}       # rel L-inf against float64 (BASELINE.json north star)
+TTI_SCALARS = dict(vp=2.0, epsilon=0.2, delta=0.1, theta=0.6, phi=0.35)
+SUBBOX = ((1, 2, 4), (SHAPE[0] - 3, SHAPE[1] - 4, SHAPE[2] - 9))   # reaches the halo in x and y, z_m % 4 == 0
+
+
+def _alloc(shape, so):
+    return tuple(n + 2 * so for n in shape)
+
+
+def iso_case(so, param, shape=SHAPE, box=None, seed=0):
+    """param: 'scalar' (vp = 2), 'vp' (vp array) or 'm' (squared-slowness array)."""
+    rng = np.random.default_rng(seed + 100 * so)
+    a = _alloc(shape, so)
+    u = rng.standard_normal((3,) + a).astype(np.float32)
+    damp = (0.1 * rng.uniform(0.0, 1.0, a)).astype(np.float32)
+    vp = rng.uniform(1.5, 2.5, a).astype(np.float32)
+    p = {'scalar': ('vp', np.float32(2.0)), 'vp': ('vp', vp), 'm': ('m', (1.0 / (vp * vp)).astype(np.float32))}[param]
+    lo, hi = box if box is not None else ((0, 0, 0), tuple(n - 1 for n in shape))
+    return dict(kind='iso', so=so, shape=shape, u=u, damp=damp, param=p, lo=tuple(lo), hi=tuple(hi),
+                dt=float(O.critical_dt(so, 3, min(SPACING), 2.5)))
+
+
+def tti_case(so, arrays, shape=SHAPE, seed=0):
+    """arrays: vp, epsilon, delta, theta, phi as white-noise fields (else the scalars TTI_SCALARS, phi != 0)."""
+    rng = np.random.default_rng(seed + 100 * so + 7)
+    a = _alloc(shape, so)
+    u = rng.standard_normal((3,) + a).astype(np.float32)
+    v = rng.standard_normal((3,) + a).astype(np.float32)
+    damp = (0.1 * rng.uniform(0.0, 1.0, a)).astype(np.float32)
+    if arrays:
+        rg = dict(vp=(1.5, 2.5), epsilon=(0.05, 0.3), delta=(0.02, 0.15), theta=(0.2, 1.2), phi=(-0.6, 0.9))
+        params = {n: rng.uniform(lo, hi, a).astype(np.float32) for n, (lo, hi) in rg.items()}
+    else:
+        params = {n: np.float32(x) for n, x in TTI_SCALARS.items()}
+    return dict(kind='tti', so=so, shape=shape, u=u, v=v, damp=damp, params=params, lo=(0, 0, 0),
+                hi=tuple(n - 1 for n in shape), dt=float(O.critical_dt(so, 3, min(SPACING), 2.5, eps_max=0.3)))
+
+
+def sparse_coordinates(shape=SHAPE, seed=3):
+    """Physical coordinates (origin 0) of points within one cell of every face, points outside the domain on both
+    sides of every axis (their supports reach into the halo, or miss the grid entirely), and two points in one
+    cell (their deposits meet in the same cells)."""
+    rng = np.random.default_rng(seed)
+    n = np.array(shape)
+    h = np.array(SPACING)
+    pts = []
+
+    def interior():
+        return rng.uniform(2.0, n - 3.0)
+
+    for d in range(3):
+        for where in (0.4, n[d] - 1 - 0.3, -1.6, n[d] - 1 + 1.3):   # inside near the faces, then just outside
+            p = interior()
+            p[d] = where
+            pts.append(p)
+    far = interior()
+    far[1] = -12.0                                                  # no support cell inside any halo
+    pts.append(far)
+    c = np.floor(interior())
+    pts.append(c + 0.27)
+    pts.append(c + np.array([0.81, 0.62, 0.55]))                    # same base cell as the point above
+    return (np.array(pts) * h).astype(np.float32)
+
+
+def sparse_tables(coords, interpolation, nt):
+    """Base cells and float64 weights (the host-side tabulation of the oracle) plus random traces."""
+    r = 1 if interpolation == 'linear' else 4
+    gp, ws = O.tabulate(coords, (0.0, 0.0, 0.0), SPACING, r, interpolation, dtype=np.float64)
+    rng = np.random.default_rng(11)
+    data = rng.standard_normal((nt, coords.shape[0])).astype(np.float32)
+    return dict(data=data, gp=gp, w=ws, r=r)
+
+
+def weights(kind, so):
+    """(float64 weights for the reference, float32 weights for the oracle) per axis."""
+    w64 = [ref64.fd2_weights(so, h) for h in SPACING]
+    w32 = [O.fd2_weights(so, h) for h in SPACING]
+    if kind == 'iso':
+        return w64, w32
+    w164 = [ref64.fd1_half_weights(so, h) for h in SPACING]
+    w132 = [O.fd1_half_weights(so, h) for h in SPACING]
+    return (w64, w164), (w32, w132)
+
+
+def reference(c, src=None, rec=None, mut=None):
+    """float64 run of a case: (fields..., traces)."""
+    so = c['so']
+    if c['kind'] == 'iso':
+        w64, _ = weights('iso', so)
+        u, tr = ref64.iso_forward(c['u'], so, w64, c['dt'], 1, K, damp=c['damp'], param=c['param'], lo=c['lo'],
+                                  hi=c['hi'], src=src, rec=rec, mut=mut)
+        return (u,), tr
+    (w2, w1), _ = weights('tti', so)
+    u, v, tr = ref64.tti_forward(c['u'], c['v'], so, w2, w1, c['dt'], 1, K, c['damp'], c['params'], lo=c['lo'],
+                                 hi=c['hi'], src=src, rec=rec, mut=mut)
+    return (u, v), tr

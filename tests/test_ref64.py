@@ -1,0 +1,125 @@
+"""The float64 reference (tests/ref64.py) against the float32 C oracle, and proof that the kernel-matrix inputs
+can fail a wrong kernel. CPU only.
+
+1. Pin: for every case of the GPU kernel matrix, ref64 and `oracle.iso_forward` / `oracle.tti_forward` (two
+   independent restatements, per-axis weights, update box) agree to rel L-inf 1e-5 (iso) / 1e-4 (TTI). TTI at
+   so=12 and so=16 has no golden fixture: this agreement is its pin.
+2. Sensitivity: every mutation of ref64.MUTATIONS that applies to a case moves the result by at least 100x the GPU
+   tolerance of that case. A kernel with that kind of bug therefore fails tests/test_kernel_matrix.py whatever
+   else it does. What float32 cannot resolve is not claimed: a mistake confined to the outermost tap at so=16
+   (w8/w0 ~ 1e-6) is below float32 resolution, and no mutation here is of that kind.
+"""
+import numpy as np
+import pytest
+
+from oracle import oracle as O
+from helpers import rel_linf
+import kernel_cases as KC
+import ref64
+
+ISO = [(so, p) for so in (4, 8, 12, 16) for p in ('scalar', 'vp', 'm')]
+TTI = [(so, arrays) for so in (4, 8, 12, 16) for arrays in (False, True)]
+
+
+def _iso_oracle(c, src=None, rec=None):
+    _, w32 = KC.weights('iso', c['so'])
+    kind, pv = c['param']
+    pk = 0 if np.ndim(pv) == 0 else (1 if kind == 'vp' else 2)
+    u = c['u'].copy()
+    O.iso_forward(u, c['so'], w32, c['dt'], 1, KC.K, damp=c['damp'], vp=float(pv) if pk == 0 else 1.0,
+                  param=pv if pk else None, param_kind=pk, lo=c['lo'], hi=c['hi'], src=src, rec=rec)
+    return (u,)
+
+
+def _tti_oracle(c):
+    _, (w2, w1) = KC.weights('tti', c['so'])
+    P = c['params']
+    arrays = {n: x for n, x in P.items() if np.ndim(x)}
+    sc = {n: (1.0 if n == 'vp' else 0.0) if np.ndim(x) else float(x) for n, x in P.items()}
+    u, v = c['u'].copy(), c['v'].copy()
+    O.tti_forward(u, v, c['so'], w2, w1, c['dt'], 1, KC.K, c['damp'], sc['vp'], sc['epsilon'], sc['delta'],
+                  sc['theta'], sc['phi'], lo=c['lo'], hi=c['hi'], arrays=arrays)
+    return (u, v)
+
+
+def _case_mutations(c):
+    arrays = (c['kind'] == 'iso' and np.ndim(c['param'][1]) > 0) or \
+             (c['kind'] == 'tti' and any(np.ndim(x) for x in c['params'].values()))
+    out = ['w_xy', 'w_yz', 'transpose_xy', 'halo_zero', 'tail_y', 'tail_z', 'swap_levels']
+    if arrays:
+        out += ['shift_x', 'shift_y', 'shift_z']
+        if c['kind'] == 'tti':
+            out.append('c_at_output')
+    return out
+
+
+def _distance(a, b):
+    return max(rel_linf(x, y) for x, y in zip(a, b))
+
+
+def _check(c, oracle_fields):
+    tol = KC.TOL[c['kind']]
+    ref, _ = KC.reference(c)
+    assert np.abs(ref[0]).max() > 0.5
+    err = _distance(oracle_fields, ref)
+    assert err < tol, f"oracle vs float64: {err:.2e}"
+    for mut in _case_mutations(c):
+        moved = _distance(KC.reference(c, mut=mut)[0], ref)
+        assert moved >= 100 * tol, f"mutation {mut!r} moves the result by only {moved:.2e}"
+
+
+@pytest.mark.parametrize('so,param', ISO)
+def test_iso_reference_matches_oracle_and_mutations_show(so, param):
+    c = KC.iso_case(so, param)
+    _check(c, _iso_oracle(c))
+
+
+@pytest.mark.parametrize('name', ['subbox', 'nz67', 'zm3'])
+def test_iso_reference_boxes_and_fallback_shapes(name):
+    """The boxes of the sub-box and fallback GPU cases: an interior box (z_m % 4 == 0), nz % 4 != 0, z_m = 3."""
+    if name == 'subbox':
+        c = KC.iso_case(8, 'vp', box=KC.SUBBOX)
+    elif name == 'nz67':
+        c = KC.iso_case(8, 'vp', shape=(37, 45, 67))
+    else:
+        c = KC.iso_case(8, 'vp', box=((0, 0, 3), (36, 44, 67)))
+    _check(c, _iso_oracle(c))
+    # outside the box nothing moves
+    lo, hi, so = c['lo'], c['hi'], c['so']
+    ref, _ = KC.reference(c)
+    keep = np.ones(ref[0].shape[1:], dtype=bool)
+    keep[tuple(slice(l + so, h + so + 1) for l, h in zip(lo, hi))] = False
+    assert np.array_equal(ref[0][:, keep], c['u'][:, keep].astype(np.float64))
+
+
+@pytest.mark.parametrize('so,arrays', TTI)
+def test_tti_reference_matches_oracle_and_mutations_show(so, arrays):
+    c = KC.tti_case(so, arrays)
+    _check(c, _tti_oracle(c))
+
+
+@pytest.mark.parametrize('param', ['vp', 'm'])
+@pytest.mark.parametrize('interpolation', ['linear', 'sinc'])
+def test_sparse_reference_matches_oracle(param, interpolation):
+    """Injection and interpolation at the faces, outside the domain and two points in one cell."""
+    c = KC.iso_case(8, param)
+    coords = KC.sparse_coordinates()
+    src = KC.sparse_tables(coords, interpolation, KC.K + 2)
+    rec = dict(src, data=np.zeros_like(src['data']))
+    ref, tr = KC.reference(c, src=src, rec=rec)
+    orec = dict(rec, data=rec['data'].copy())
+    fields = _iso_oracle(c, src=src, rec=orec)
+    assert _distance(fields, ref) < KC.TOL['iso']
+    assert rel_linf(orec['data'], tr) < KC.TOL['iso']
+    # the sources matter: without them the wavefield differs far beyond the tolerance (near the faces too)
+    bare, _ = KC.reference(c, rec=rec)
+    assert _distance(bare, ref) > 100 * KC.TOL['iso']
+    # the point far outside has no support cell; every other point samples something
+    far = 12
+    assert not tr[1:KC.K + 1, far].any()
+    assert np.all(np.abs(np.delete(tr[1:KC.K + 1], far, axis=1)).max(axis=0) > 0)
+    # the halo was written: sources outside the domain deposit into it
+    so = c['so']
+    dom = np.zeros(ref[0].shape[1:], dtype=bool)
+    dom[so:-so, so:-so, so:-so] = True
+    assert np.abs(ref[0][:, ~dom] - bare[0][:, ~dom]).max() > 0

@@ -115,6 +115,29 @@ def test_point_kernels_match_the_oracle(emu, case):
         assert not u_emu[dom][(nsteps + 1) % 3][..., 0].any()
 
 
+@pytest.mark.parametrize('param', ['scalar', 'vp', 'm'])
+def test_point_kernel_per_axis_spacing_and_sub_box_vs_float64(emu, param):
+    """The generic point code with spacing (10, 12.5, 8), an interior update box that still reads the halo, and white
+    noise in every time slot and in the halo, against the float64 reference (tests/ref64.py): a weight list or stride
+    applied to the wrong axis in b2_iso_point.cuh, or a box bound off by one, fails here."""
+    import kernel_cases as KC
+    so = 8
+    c = KC.iso_case(so, param, shape=(21, 26, 30), box=((1, 2, 3), (18, 22, 26)))
+    _, w = KC.weights('iso', so)
+    kind, pv = c['param']
+    pk = 0 if np.ndim(pv) == 0 else (1 if kind == 'vp' else 2)
+    u = c['u'].copy()
+    alloc = np.array(u.shape[1:], dtype=np.int32)
+    lo, hi = np.array(c['lo'], dtype=np.int32), np.array(c['hi'], dtype=np.int32)
+    for time in range(1, KC.K + 1):
+        rc = emu.emu_iso_step(_fp(u), _ip(alloc), so, so // 2, 3, _fp(w[0]), _fp(w[1]), _fp(w[2]), _fp(c['damp']), pk,
+                              _fp(pv) if pk else None, float(pv) if pk == 0 else 1.0, c['dt'], _ip(lo), _ip(hi),
+                              time % 3, (time - 1) % 3, (time + 1) % 3, 0, 0, None)
+        assert rc == 0
+    (ref,), _ = KC.reference(c)
+    assert rel_linf(u, ref) < KC.TOL['iso']
+
+
 @pytest.mark.parametrize('dmh', [0, 3])
 def test_born_point_kernels_match_the_oracle(emu, dmh):
     so, shape, h, nsteps = 8, (21, 18, 16), 10.0, 6
