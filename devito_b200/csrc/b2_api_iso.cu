@@ -242,6 +242,9 @@ static int iso_forward_streamed(const b2_iso_args *a, IsoPlan &p, FieldGeom g, D
     int dim = decomposed ? 1 : 0;
     if (!decomposed) if (const char *e = getenv("B2_STREAM_DIM")) dim = atoi(e) == 1 ? 1 : 0;
     const int n = p.n[dim], R = p.radius[dim], so = p.so, ad = p.a[dim], a0 = p.a[0];
+    // ranges [ra, rb) count from the first point of the update box; `org` is that point's domain index along
+    // `dim` (x_m or y_m), so range cell i is domain cell org + i and allocated index so + org + i
+    const int org = g.lo[dim];
     const int L = a->time_M - a->time_m + 1;
     const size_t plane = (size_t)p.sx, rowlen = (size_t)p.a[2];
     int W = 128;
@@ -307,7 +310,7 @@ static int iso_forward_streamed(const b2_iso_args *a, IsoPlan &p, FieldGeom g, D
     std::vector<int> ulo(K), uhi(K);
     for (int c = 0; c < K; ++c) {
         ulo[c] = c == 0 ? 0 : uhi[c - 1];
-        uhi[c] = c == K - 1 ? ad : std::min(ad, so + std::min(n, (c + 1) * W) + R);
+        uhi[c] = c == K - 1 ? ad : std::min(ad, so + org + std::min(n, (c + 1) * W) + R);
         for (int t = 0; t < 3; ++t)
             if ((rc = copy_chunk((float *)u.d, (float *)u.h, (size_t)t * p.slot_elems, ulo[c], uhi[c], true, S.up))) return rc;
         if (damp && damp_io && (rc = copy_chunk((float *)damp->d, (float *)damp->h, 0, ulo[c], uhi[c], true, S.up))) return rc;
@@ -326,8 +329,8 @@ static int iso_forward_streamed(const b2_iso_args *a, IsoPlan &p, FieldGeom g, D
 
     auto range_geom = [&](int ra, int rb) {
         FieldGeom q = g;
-        q.lo[dim] = ra;
-        q.hi[dim] = rb - 1;
+        q.lo[dim] = org + ra;                                        // FieldGeom bounds are domain indices
+        q.hi[dim] = org + rb - 1;
         if (dim == 0) {
             q.nb_lo = ra > 0;        // an interior cut: the cells beyond it belong to another range
             q.nb_hi = rb < n;
@@ -351,7 +354,7 @@ static int iso_forward_streamed(const b2_iso_args *a, IsoPlan &p, FieldGeom g, D
             if (rc) return rc;
             if (rec.present && !a->rec_toff) {
                 // the initial time level is complete on the chunk that just arrived
-                const int ra = std::max(0, ulo[ph] - so), rb = std::min(n, uhi[ph] - so);
+                const int ra = std::max(0, ulo[ph] - so - org), rb = std::min(n, uhi[ph] - so - org);
                 if (rb > ra)
                     if ((rc = launch_interp(rec, range_geom(ra, rb), p.u + (size_t)t0_first * p.slot_elems, nullptr, a->time_m)))
                         return rc;
@@ -398,8 +401,11 @@ static int iso_forward_streamed(const b2_iso_args *a, IsoPlan &p, FieldGeom g, D
                 if (row <= a->time_M && (rc = launch_interp(rec, qi, f1, nullptr, row))) return rc;
             }
         }
-        // what lies left of (ph+1)W - (L-1)R has seen all L steps: send it home while the sweep goes on
-        int dhi = ph == P - 1 ? ad : std::min(ad, std::max(0, so + (ph + 1) * W - (L - 1) * R));
+        // what lies left of (ph+1)W - (L-1)R has seen all L steps: send it home while the sweep goes on. Until that
+        // bound is positive, the last step has not run its first range, whose sources may still deposit into the
+        // cells below the box: nothing there is final yet.
+        const int fin = (ph + 1) * W - (L - 1) * R;
+        int dhi = ph == P - 1 ? ad : (fin > 0 ? std::min(ad, so + org + fin) : 0);
         if (ph == P - 1 || dhi - dlo >= W / 2) {
             if (dhi > dlo) {
                 cudaEvent_t e = S.next();

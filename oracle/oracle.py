@@ -121,14 +121,15 @@ def iso_forward(u, so, w, dt, time_m, time_M, damp=None, vp=1.5, param=None, par
 
 
 def born_forward(u, U, dm, so, w, dt, time_m, time_M, damp=None, vp=1.5, param=None, param_kind=0,
-                 src=None, rec=None, dmhalo=0, fast=False):
+                 src=None, rec=None, dmhalo=0, lo=None, hi=None, fast=False):
     """The reference's `Born` operator (examples/seismic/acoustic/operators.py:235-277): u driven by
-    `src`, the linearised field U driven by -dm * u.dt2, `rec` sampled from U. 3-D."""
+    `src`, the linearised field U driven by -dm * u.dt2, `rec` sampled from U. 3-D; lo/hi: inclusive update box
+    (default: the whole domain)."""
     L = load(fast)
     R = len(w[0]) - 1
     alloc = np.array(u.shape[1:], dtype=np.int32)
-    lo = np.array([0] * 3, dtype=np.int32)
-    hi = np.array([s - 2 * so - 1 for s in u.shape[1:]], dtype=np.int32)
+    lo = np.array(lo if lo is not None else [0] * 3, dtype=np.int32)
+    hi = np.array(hi if hi is not None else [s - 2 * so - 1 for s in u.shape[1:]], dtype=np.int32)
     wa = [np.ascontiguousarray(x, dtype=np.float32) for x in w]
     keep = []
     s = _sparse(src['data'], src['gp'], src['w'], src['r'], keep) if src else None

@@ -32,7 +32,7 @@ def iso_case(so, param, shape=SHAPE, box=None, seed=0):
     damp = (0.1 * rng.uniform(0.0, 1.0, a)).astype(np.float32)
     vp = rng.uniform(1.5, 2.5, a).astype(np.float32)
     p = {'scalar': ('vp', np.float32(2.0)), 'vp': ('vp', vp), 'm': ('m', (1.0 / (vp * vp)).astype(np.float32))}[param]
-    lo, hi = box if box is not None else ((0, 0, 0), tuple(n - 1 for n in shape))
+    lo, hi = box if box is not None else ((0,) * len(shape), tuple(n - 1 for n in shape))
     return dict(kind='iso', so=so, shape=shape, u=u, damp=damp, param=p, lo=tuple(lo), hi=tuple(hi),
                 dt=float(O.critical_dt(so, 3, min(SPACING), 2.5)))
 
@@ -97,6 +97,58 @@ def weights(kind, so):
     w164 = [ref64.fd1_half_weights(so, h) for h in SPACING]
     w132 = [O.fd1_half_weights(so, h) for h in SPACING]
     return (w64, w164), (w32, w132)
+
+
+GRAD_HALO = 1                            # grad is a Function with its own (smaller) halo
+SNAP_HALO = 3                            # snapshot halo != so
+SNAP_FACTOR = 2
+SNAP_SENTINEL = -7.25                    # exactly representable: unvisited snapshot cells must keep it bit for bit
+
+
+def scheme_case(scheme, so, param, box=None, dmh=0, shape=SHAPE, seed=0):
+    """An iso case plus what a scheme needs, white noise throughout:
+    'plain' | 'adjoint' | 'fs' | 'adjoint_fs' | 'ot4' | 'adjoint_ot4' (nothing more), 'grad' (adjoint + imaging condition:
+    usave for times 0 .. K+1 with u's layout, grad with halo GRAD_HALO), 'born' (U, dm with halo `dmh`),
+    'snap' / 'snap_fwd' (Eq(usave, u) / Eq(usave, u.forward): a snapshot array of halo SNAP_HALO, filled with
+    SNAP_SENTINEL). 2-D cases pass a 2-D `shape` (the time-slot noise and the parameters are drawn the same way)."""
+    c = iso_case(so, param, shape=shape, box=box, seed=seed)
+    if len(shape) == 2:
+        c['dt'] = float(O.critical_dt(so, 2, min(SPACING[1:]), 2.5))
+    c['scheme'] = scheme
+    rng = np.random.default_rng(seed + 100 * so + 31)
+    if scheme == 'grad':
+        c['usave'] = rng.standard_normal((K + 2,) + c['u'].shape[1:]).astype(np.float32)
+        c['grad'] = rng.standard_normal(tuple(n + 2 * GRAD_HALO for n in shape)).astype(np.float32)
+    elif scheme == 'born':
+        c['U'] = rng.standard_normal(c['u'].shape).astype(np.float32)
+        c['dm'] = (0.05 * rng.standard_normal(tuple(n + 2 * dmh for n in shape))).astype(np.float32)
+        c['dmh'] = dmh
+    elif scheme in ('snap', 'snap_fwd'):
+        c['snap'] = np.full((K // SNAP_FACTOR + 2,) + tuple(n + 2 * SNAP_HALO for n in shape), SNAP_SENTINEL,
+                            dtype=np.float32)
+    return c
+
+
+def scheme_reference(c, src=None, rec=None, mut=None):
+    """float64 run of a scheme case: dict of every output ('u', 'traces', and 'U', 'grad' or 'snap')."""
+    so, s = c['so'], c['scheme']
+    w64 = [ref64.fd2_weights(so, h) for h in SPACING[3 - len(c['shape']):]]
+    kw = dict(damp=c['damp'], param=c['param'], lo=c['lo'], hi=c['hi'], src=src, rec=rec, mut=mut)
+    if s == 'born':
+        u, U, tr = ref64.born_forward(c['u'], c['U'], c['dm'], c['dmh'], so, w64, c['dt'], 1, K, **kw)
+        return dict(u=u, U=U, traces=tr)
+    out = {}
+    if s == 'grad':
+        out['grad'] = c['grad'].astype(np.float64)
+        kw.update(grad=out['grad'], gh=GRAD_HALO, usave=c['usave'])
+    if s in ('snap', 'snap_fwd'):
+        out['snap'] = c['snap'].astype(np.float64)
+        kw.update(snap=out['snap'], snap_h=SNAP_HALO, snap_factor=SNAP_FACTOR, snap_toff=int(s == 'snap_fwd'))
+    u, tr = ref64.iso_forward(c['u'], so, w64, c['dt'], 1, K, adjoint=s in ('adjoint', 'adjoint_fs', 'adjoint_ot4',
+                                                                              'grad'),
+                              free_surface=s in ('fs', 'adjoint_fs'), ot4=s in ('ot4', 'adjoint_ot4'), **kw)
+    out.update(u=u, traces=tr)
+    return out
 
 
 def reference(c, src=None, rec=None, mut=None):

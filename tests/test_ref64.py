@@ -123,3 +123,137 @@ def test_sparse_reference_matches_oracle(param, interpolation):
     dom = np.zeros(ref[0].shape[1:], dtype=bool)
     dom[so:-so, so:-so, so:-so] = True
     assert np.abs(ref[0][:, ~dom] - bare[0][:, ~dom]).max() > 0
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# The schemes built on the iso update: adjoint, free surface, OT4, imaging condition, Born, snapshots, 2-D.
+# Same inputs as the GPU scheme matrix (tests/test_scheme_matrix.py): white noise in every slot and halo, the KC
+# sparse points (faces, outside the domain, two in one cell) as sources and receivers.
+# ---------------------------------------------------------------------------------------------------------------
+OUT_TOL = {'u': 1e-5, 'snap': 1e-5, 'traces': 1e-5, 'U': 1e-4, 'grad': 1e-4}
+
+
+def _out_tol(c, name):
+    return 1e-4 if c['scheme'] == 'born' and name == 'traces' else OUT_TOL[name]
+
+
+def scheme_sparse(c):
+    """sinc points (r = 4) from so = 8 on, linear below; receivers record into zeros."""
+    src = KC.sparse_tables(KC.sparse_coordinates(c['shape']), 'sinc' if c['so'] >= 8 else 'linear', KC.K + 2)
+    return src, dict(src, data=np.zeros_like(src['data']))
+
+
+def _scheme_oracle(c, src, rec):
+    """float32 C oracle of a scheme case: dict of the outputs it has (no snapshots)."""
+    _, w32 = KC.weights('iso', c['so'])
+    w32 = w32[3 - len(c['shape']):]
+    kind, pv = c['param']
+    pk = 0 if np.ndim(pv) == 0 else (1 if kind == 'vp' else 2)
+    pkw = dict(damp=c['damp'], vp=float(pv) if pk == 0 else 1.0, param=pv if pk else None, param_kind=pk)
+    orec = dict(rec, data=rec['data'].copy()) if rec is not None else None
+    u = c['u'].copy()
+    s = c['scheme']
+    if s == 'born':
+        U = c['U'].copy()
+        O.born_forward(u, U, c['dm'], c['so'], w32, c['dt'], 1, KC.K, src=src, rec=orec, dmhalo=c['dmh'],
+                       lo=c['lo'], hi=c['hi'], **pkw)
+        return dict(u=u, U=U, traces=orec['data'])
+    out = {}
+    kw = {}
+    if s == 'grad':
+        out['grad'] = c['grad'].copy()
+        kw = dict(grad=out['grad'], ghalo=KC.GRAD_HALO, usave=c['usave'])
+    O.iso_forward(u, c['so'], w32, c['dt'], 1, KC.K, lo=c['lo'], hi=c['hi'], src=src, rec=orec,
+                  adjoint=s in ('adjoint', 'adjoint_fs', 'adjoint_ot4', 'grad'),
+                  free_surface=s in ('fs', 'adjoint_fs'), ot4=s in ('ot4', 'adjoint_ot4'), **kw, **pkw)
+    out['u'] = u
+    if orec is not None:
+        out['traces'] = orec['data']
+    return out
+
+
+def scheme_mutations(c):
+    """The mutations of ref64.MUTATIONS a kernel of this scheme could have."""
+    s = c['scheme']
+    arrays = np.ndim(c['param'][1]) > 0
+    out = ['w_xy', 'halo_zero', 'swap_levels']
+    if len(c['shape']) == 3:
+        out += ['w_yz', 'transpose_xy', 'tail_y', 'tail_z']
+        if arrays:
+            out += ['shift_x', 'shift_y', 'shift_z']
+    if s in ('adjoint', 'adjoint_fs', 'adjoint_ot4', 'grad'):
+        out.append('adj_inject_level')
+    if s in ('fs', 'adjoint_fs'):
+        out += ['fs_surface_tap', 'fs_mirror_sign', 'fs_keep_row0']
+        # Row z = R differs from the plain update only by its outermost lower tap, w_R u[0], and u[0] is non-zero
+        # only in the initial level and where a source deposited into the surface row. At so = 8 that moves u by
+        # about 4x the tolerance (w_4 / w_0 = 1/1594), so the mutation is claimed at so = 4 only.
+        if c['so'] == 4:
+            out.append('fs_rows_lt_R')
+    if s in ('ot4', 'adjoint_ot4'):
+        out.append('ot4_factor')
+        if arrays:
+            out.append('ot4_m_at_output')           # with a scalar m the two places hold the same value
+    if s == 'born':
+        out += ['born_before_inject', 'born_dm_shift']
+    if s == 'grad':
+        out += ['grad_usave_time', 'grad_assign', 'grad_halo']
+    if s in ('snap', 'snap_fwd'):
+        out += ['snap_level', 'snap_index']
+    return out
+
+
+def scheme_distance(c, got, want):
+    """max over the outputs of rel L-inf / that output's tolerance (1 = at the tolerance)."""
+    return max(rel_linf(got[k], want[k]) / _out_tol(c, k) for k in want if want[k] is not None)
+
+
+def _check_scheme(c, sparse=True, oracle=True):
+    src, rec = scheme_sparse(c) if sparse else (None, None)
+    ref = KC.scheme_reference(c, src=src, rec=rec)
+    assert np.abs(ref['u']).max() > 0.5
+    if oracle:
+        got = _scheme_oracle(c, src, rec)
+        for k, v in got.items():
+            err = rel_linf(v, ref[k])
+            assert err < _out_tol(c, k), f"oracle vs float64, {k}: {err:.2e}"
+    for mut in scheme_mutations(c):
+        moved = scheme_distance(c, KC.scheme_reference(c, src=src, rec=rec, mut=mut), ref)
+        assert moved >= 100, f"mutation {mut!r} moves the result by only {moved:.0f}x the tolerance"
+    return ref
+
+
+SCHEME_CASES = [(s, so, p, b) for s in ('adjoint', 'ot4', 'grad', 'born')
+                for so in (4, 8, 16) for p in ('scalar', 'vp', 'm') for b in ('full', 'sub')] + \
+               [(s, so, p, 'full') for s in ('fs', 'adjoint_fs', 'adjoint_ot4') for so in (4, 8, 16)
+                for p in ('scalar', 'vp', 'm')]
+
+
+@pytest.mark.parametrize('scheme,so,param,box', SCHEME_CASES)
+def test_scheme_reference_matches_oracle_and_mutations_show(scheme, so, param, box):
+    c = KC.scheme_case(scheme, so, param, box=KC.SUBBOX if box == 'sub' else None, dmh=3 if so == 8 else 0)
+    _check_scheme(c)
+
+
+@pytest.mark.parametrize('scheme', ['snap', 'snap_fwd'])
+@pytest.mark.parametrize('box', ['full', 'sub'])
+def test_snapshot_reference_mutations_show(scheme, box):
+    """Snapshots have no oracle counterpart (a plain copy): the mutation distances are their check here, and the
+    cells the reference leaves alone keep the sentinel."""
+    c = KC.scheme_case(scheme, 8, 'vp', box=KC.SUBBOX if box == 'sub' else None)
+    ref = _check_scheme(c, oracle=False)
+    snap = ref['snap']
+    visited = np.zeros(snap.shape, dtype=bool)
+    sh = KC.SNAP_HALO
+    for time in range(1, KC.K + 1):
+        if time % KC.SNAP_FACTOR == 0:
+            visited[(time // KC.SNAP_FACTOR,) + tuple(slice(l + sh, h + sh + 1) for l, h in zip(c['lo'], c['hi']))] = True
+    assert np.all(snap[~visited] == KC.SNAP_SENTINEL) and not np.any(snap[visited] == KC.SNAP_SENTINEL)
+
+
+@pytest.mark.parametrize('scheme', ['plain', 'fs'])
+@pytest.mark.parametrize('param', ['scalar', 'vp'])
+def test_2d_reference_matches_oracle_and_mutations_show(scheme, param):
+    """2-D (45, 68), spacing (12.5, 8): the plain update and the free surface on the last axis."""
+    c = KC.scheme_case(scheme, 8, param, shape=KC.SHAPE[1:])
+    _check_scheme(c, sparse=False)

@@ -220,3 +220,55 @@ def test_linear_point_kernel_runs_the_diffusion_example(emu):
             (ref[1:-1, 2:] - 2 * ref[1:-1, 1:-1] + ref[1:-1, :-2]) / hy ** 2)
         ref = new
     assert rel_linf(f[nt % 2, so:-so, so:-so], ref) < 1e-5
+
+
+def _emu_scheme(emu, c):
+    """K steps of a KC scheme case through the point kernels (emu_iso_step / emu_born_step), no sparse points."""
+    import kernel_cases as KC
+    so = c['so']
+    _, w = KC.weights('iso', so)
+    kind, pv = c['param']
+    pk = 0 if np.ndim(pv) == 0 else (1 if kind == 'vp' else 2)
+    u = c['u'].copy()
+    alloc = np.array(u.shape[1:], dtype=np.int32)
+    lo, hi = np.array(c['lo'], dtype=np.int32), np.array(c['hi'], dtype=np.int32)
+    par, vp = (_fp(pv) if pk else None), (float(pv) if pk == 0 else 1.0)
+    if c['scheme'] == 'born':
+        U = c['U'].copy()
+        for time in range(1, KC.K + 1):
+            rc = emu.emu_born_step(_fp(u), _fp(U), _fp(c['dm']), _ip(np.array(c['dm'].shape, dtype=np.int32)),
+                                   c['dmh'], _ip(alloc), so, so // 2, _fp(w[0]), _fp(w[1]), _fp(w[2]), _fp(c['damp']),
+                                   pk, par, vp, c['dt'], _ip(lo), _ip(hi), time % 3, (time - 1) % 3, (time + 1) % 3)
+            assert rc == 0
+        return dict(u=u, U=U)
+    fs, ot4 = c['scheme'] == 'fs', c['scheme'] == 'ot4'
+    W = np.zeros(int(np.prod(alloc)), dtype=np.float32) if ot4 else None
+    for time in range(1, KC.K + 1):
+        rc = emu.emu_iso_step(_fp(u), _ip(alloc), so, so // 2, 3, _fp(w[0]), _fp(w[1]), _fp(w[2]), _fp(c['damp']), pk,
+                              par, vp, c['dt'], _ip(lo), _ip(hi), time % 3, (time - 1) % 3, (time + 1) % 3,
+                              int(fs), int(ot4), _fp(W))
+        assert rc == 0
+    return dict(u=u)
+
+
+@pytest.mark.parametrize('scheme,so,param,dmh', [
+    ('fs', 4, 'scalar', 0), ('fs', 8, 'vp', 0), ('fs', 8, 'm', 0),
+    ('ot4', 4, 'vp', 0), ('ot4', 8, 'scalar', 0), ('ot4', 8, 'm', 0),
+    ('born', 8, 'vp', 0), ('born', 8, 'm', 3), ('born', 4, 'vp', 3),
+])
+def test_scheme_point_kernels_per_axis_spacing_vs_float64(emu, scheme, so, param, dmh):
+    """`iso_fs_point`, `ot4_w_point` + `iso_point` and `born_src_point` with spacing (10, 12.5, 8), shape (21, 26, 32),
+    white noise in every slot and halo, against tests/ref64.py. OT4 and Born run an interior box (which OT4 grows
+    by R into the halo); the free surface needs z_m = 0, so its box is interior in x and y only. The vertical
+    weights of the mirrored taps, of both OT4 Laplacians and of Born's U update are those of z only here."""
+    import kernel_cases as KC
+    shape = (21, 26, 32)
+    box = ((1, 2, 0), (18, 22, 31)) if scheme == 'fs' else ((1, 2, 3), (18, 22, 26))
+    c = KC.scheme_case(scheme, so, param, box=box, dmh=dmh, shape=shape)
+    got = _emu_scheme(emu, c)
+    want = KC.scheme_reference(c)
+    assert rel_linf(got['u'], want['u']) < KC.TOL['iso']
+    if scheme == 'born':
+        assert rel_linf(got['U'], want['U']) < 1e-4
+    if scheme == 'fs':
+        assert not got['u'][(KC.K + 1) % 3][so + 1:so + 19, so + 2:so + 23, so].any()
