@@ -68,7 +68,8 @@ class TtiArgs(Structure):
                 ('halo', c_void_p), ('timers', POINTER(Profiler)),
                 ('vp_arr', POINTER(Dataobj)), ('epsilon_arr', POINTER(Dataobj)),
                 ('delta_arr', POINTER(Dataobj)), ('theta_arr', POINTER(Dataobj)),
-                ('phi_arr', POINTER(Dataobj))]
+                ('phi_arr', POINTER(Dataobj)),
+                ('born_du', POINTER(Dataobj)), ('born_dv', POINTER(Dataobj)), ('born_dm', POINTER(Dataobj))]
 
 
 class Tap(Structure):

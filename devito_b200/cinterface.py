@@ -120,6 +120,10 @@ def signature(plan, name, distributed=False):
                 head.append(_Param(n, 'struct dataobj *restrict', f'{n}_vec'))
             else:
                 head.append(_Param(n, 'const float', n))
+        for key in ('born_du', 'born_dv', 'born_dm'):
+            f = plan.get(key)
+            if f is not None:
+                head.append(_Param(f.name, 'struct dataobj *restrict', f'{f.name}_vec'))
     for sf in (plan['src'], plan['rec']):
         if sf is not None:
             head.extend(_sparse_params(sf, nd))
@@ -269,6 +273,10 @@ def _tti_body(plan, distributed):
             L.append(f"  a.{n} = {n};")
     L.append("  a.dt = dt;")
     _bounds(plan, L)
+    if plan.get('born_du') is not None:
+        L.append(f"  a.born_du = (struct b2_dataobj *){plan['born_du'].name}_vec;")
+        L.append(f"  a.born_dv = (struct b2_dataobj *){plan['born_dv'].name}_vec;")
+        L.append(f"  a.born_dm = (struct b2_dataobj *){plan['born_dm'].name}_vec;")
     _tail(plan, 'b2_tti_forward', L, distributed)
     return L
 

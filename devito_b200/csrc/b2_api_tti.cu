@@ -1,7 +1,10 @@
 // C-ABI entry point b2_tti_forward: time loop of the reference's generated `ForwardTTI`
 // (examples/seismic/tti/operators.py:431-480): coupled u, v update, injection of the same
 // source into both fields (:475-476), receivers sample u+v (:477); halo exchange of both
-// fields in one call (tests/test_mpi.py:3690-3694).
+// fields in one call (tests/test_mpi.py:3690-3694). With born_du / born_dv / born_dm the loop is that of the
+// reference's `BornTTI` (tti/operators.py:532-586): the background pair is stepped and the source injected into it,
+// then the linearised pair is stepped with the same sweep and driven by -dm * u0.dt2 / -dm * v0.dt2, and the
+// receivers sample du + dv.
 #include "b2_tti.cuh"
 #include "b2_sparse.cuh"
 #include "b2_halo.cuh"
@@ -21,24 +24,27 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
     const int so = a->space_order;
     int rc = B2_OK;
 
-    DevArray u, v, damp, parr[5];
+    DevArray u, v, damp, parr[5], bdu, bdv, bdm;
     bool sparr[5] = {false, false, false, false, false};
     SparseDev src, rec;
-    TtiPlan p;
+    TtiPlan p, pd;
     FieldGeom g;
-    bool su = false, sv = false, sd = false;
+    bool su = false, sv = false, sd = false, sdu = false, sdv = false, sdm = false;
 
     auto cleanup = [&](int code) {
         const bool back = code == B2_OK || code == B2_ERR_NAN;
         int r1 = su ? stage_out(u, back) : B2_OK;
         int r2 = sv ? stage_out(v, back) : B2_OK;
+        const int r4 = sdu ? stage_out(bdu, back) : B2_OK;
+        const int r5 = sdv ? stage_out(bdv, back) : B2_OK;
+        if (sdm) stage_out(bdm, false);
         if (sd) stage_out(damp, false);
         for (int i = 0; i < 5; ++i) if (sparr[i]) stage_out(parr[i], false);
         sparse_stage_out(src, false);
         int r3 = sparse_stage_out(rec, back);
         tti_plan_free(p);
         if (code != B2_OK) return code;
-        return r1 ? r1 : (r2 ? r2 : r3);
+        return r1 ? r1 : (r2 ? r2 : (r3 ? r3 : (r4 ? r4 : r5)));
     };
 
     if ((rc = stage_in(a->u, 4, u, true))) return cleanup(rc);
@@ -55,6 +61,35 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
             if (pa[i]) {
                 if ((rc = stage_in(pa[i], 3, parr[i], true))) return cleanup(rc);
                 sparr[i] = true;
+            }
+    }
+    const bool born = a->born_du || a->born_dv || a->born_dm;
+    int dmh = 0;
+    if (born) {
+        if (!a->born_du || !a->born_dv || !a->born_dm) {
+            set_error("b2_tti_forward: Born modelling needs born_du, born_dv and born_dm together");
+            return cleanup(B2_ERR_INVALID);
+        }
+        if (a->halo) {
+            set_error("b2_tti_forward: Born modelling is not combined with halo exchange in this version");
+            return cleanup(B2_ERR_INVALID);
+        }
+        if ((rc = stage_in(a->born_du, 4, bdu, true))) return cleanup(rc);
+        sdu = true;
+        if ((rc = stage_in(a->born_dv, 4, bdv, true))) return cleanup(rc);
+        sdv = true;
+        if ((rc = stage_in(a->born_dm, 3, bdm, true))) return cleanup(rc);
+        sdm = true;
+        for (int d = 0; d < 4; ++d)
+            if (bdu.size[d] != u.size[d] || bdv.size[d] != u.size[d]) {
+                set_error("b2_tti_forward: born_du and born_dv must have the layout of u");
+                return cleanup(B2_ERR_INVALID);
+            }
+        dmh = a->born_dm->hsize ? a->born_dm->hsize[0] : (bdm.size[0] - (u.size[1] - 2 * so)) / 2;
+        for (int d = 0; d < 3; ++d)
+            if (dmh < 0 || bdm.size[d] != u.size[d + 1] - 2 * so + 2 * dmh) {
+                set_error("b2_tti_forward: born_dm extent %d on dim %d does not match the grid", bdm.size[d], d);
+                return cleanup(B2_ERR_INVALID);
             }
     }
     if ((rc = sparse_stage_in(a->src, 3, src, true))) return cleanup(rc);
@@ -104,7 +139,14 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
         for (int i = 0; i <= a->radius; ++i) p.w2[d][i] = a->w2[d][i];
         for (int i = 0; i < a->radius; ++i) p.w1[d][i] = a->w1[d][i];
     }
-    if ((rc = tti_plan_init(p, a->kernel))) return cleanup(rc);
+    {
+        // both pairs run one sweep variant: a linearised pair that cannot take the fused kernel sends both to the
+        // two-pass kernel (a forced fused kernel fails in tti_plan_retarget instead)
+        int kernel = a->kernel;
+        if (born && kernel != 2 && ((uintptr_t)bdu.d % 16 != 0 || (uintptr_t)bdv.d % 16 != 0)) kernel = 1;
+        if ((rc = tti_plan_init(p, kernel))) return cleanup(rc);
+        if (born && (rc = tti_plan_retarget(p, (float *)bdu.d, (float *)bdv.d, pd))) return cleanup(rc);
+    }
 
     g.sx = p.sx;
     g.sy = p.sy;
@@ -151,12 +193,23 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
             // arrive with the neighbours' stores of this same step
             if (a->rec_toff && rec.present && (rc = halo_p2p_wait(a->halo))) return cleanup(rc);
         }
+        if (born) {
+            if ((rc = tti_step(pd, t0, t2, t1, 0, p.n[0]))) return cleanup(rc);
+            if ((rc = tti_born_source(p, pd, t0, t2, t1, (const float *)bdm.d, (long long)bdm.size[1] * bdm.size[2],
+                                      bdm.size[2], dmh)))
+                return cleanup(rc);
+        }
         const size_t ro = (size_t)(a->rec_toff ? t1 : t0) * p.slot_elems;
-        if ((rc = launch_interp(rec, g, p.u + ro, p.v + ro, time))) return cleanup(rc);
+        const TtiPlan &pr = born ? pd : p;
+        if ((rc = launch_interp(rec, g, pr.u + ro, pr.v + ro, time))) return cleanup(rc);
         if (a->errctl && ((time - a->time_m) % 100 == 99 || time == a->time_M)) {
             bool bad = false;
             if ((rc = check_finite(fu, p.slot_elems, bad))) return cleanup(rc);
             if (bad) { set_error("NaN/Inf detected in u at time=%d", time); return cleanup(B2_ERR_NAN); }
+            if (born) {
+                if ((rc = check_finite(pd.u + (size_t)t1 * p.slot_elems, p.slot_elems, bad))) return cleanup(rc);
+                if (bad) { set_error("NaN/Inf detected in du at time=%d", time); return cleanup(B2_ERR_NAN); }
+            }
         }
     }
     if (a->halo && (rc = halo_p2p_drain(a->halo))) return cleanup(rc);

@@ -15,6 +15,7 @@
 // Kernel 1 (two-pass, any even radius): pass A writes Gz(u), Gz(v) to scratch, pass B
 // applies the outer derivatives + Laplacian + time update.
 #include "b2_tti.cuh"
+#include "b2_tti_point.cuh"
 #include "b2_ptx.cuh"
 #include <algorithm>
 #include <cstdlib>
@@ -1138,6 +1139,7 @@ int tti_plan_init(TtiPlan &p, int kernel) {
         }
         count_launch();
         B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+        p.tm_rows = ty + 2 * p.R;
         if ((rc = tti_make_tmap(&p.tm_u, p.u, p.a, p.tsize, 72, ty + 2 * p.R))) return rc;
         if ((rc = tti_make_tmap(&p.tm_v, p.v, p.a, p.tsize, 72, ty + 2 * p.R))) return rc;
         p.tm_cx = p.tm_cy = p.tm_cz = p.tm_u;
@@ -1159,6 +1161,124 @@ void tti_plan_free(TtiPlan &p) {
     p.gzu = p.gzv = nullptr;       // scratch is cached in the library
     p.coefA = nullptr;
     p.tCx = p.tCy = p.tCz = p.tE2 = p.tSD = p.tMD = nullptr;
+}
+
+int tti_plan_retarget(const TtiPlan &p, float *u, float *v, TtiPlan &out) {
+    out = p;
+    out.u = u;
+    out.v = v;
+    if (!p.use_fused) return B2_OK;
+    if ((uintptr_t)u % 16 != 0 || (uintptr_t)v % 16 != 0) {
+        set_error("tti: the second field pair is not 16-byte aligned, so it cannot run the fused kernel of the first");
+        return B2_ERR_INVALID;
+    }
+    int rc;
+    if ((rc = tti_make_tmap(&out.tm_u, u, p.a, p.tsize, 72, p.tm_rows))) return rc;
+    if ((rc = tti_make_tmap(&out.tm_v, v, p.a, p.tsize, 72, p.tm_rows))) return rc;
+    if (!p.arr_ct) out.tm_cx = out.tm_cy = out.tm_cz = out.tm_u;
+    return B2_OK;
+}
+
+// Born source term, 48 B/point: dm, u0 and v0 at t+1, t, t-1 and A (or the parameters of the denominator) read once,
+// du[t+1] and dv[t+1] read and written. V4: four consecutive z points per thread with 16-byte accesses; the streams
+// read once go through `ld.global.nc.L1::no_allocate`.
+__device__ __forceinline__ float4 ld_once4(const float *p) {
+    float4 r;
+    asm("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
+        : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
+    return r;
+}
+
+__device__ __forceinline__ void tti_born_point4(const TtiBK &k, int x, int y, int z) {
+    const long long idx = (long long)(k.o0 + x) * k.sx + (long long)(k.o1 + y) * k.sy + (k.o2 + z);
+    const long long j = (long long)(k.dg0 + x) * k.dsx + (long long)(k.dg1 + y) * k.dsy + (k.dg2 + z);
+    const float4 d = ld_once4(k.dm + j);
+    const float4 a1 = ld_once4(k.u1 + idx), a0 = ld_once4(k.u0 + idx), am = ld_once4(k.um + idx);
+    const float4 b1 = ld_once4(k.v1 + idx), b0 = ld_once4(k.v0 + idx), bm = ld_once4(k.vm + idx);
+    float4 du = *reinterpret_cast<const float4 *>(k.du1 + idx);
+    float4 dv = *reinterpret_cast<const float4 *>(k.dv1 + idx);
+    const float dd[4] = {d.x, d.y, d.z, d.w};
+    const float u1[4] = {a1.x, a1.y, a1.z, a1.w}, u0[4] = {a0.x, a0.y, a0.z, a0.w}, um[4] = {am.x, am.y, am.z, am.w};
+    const float v1[4] = {b1.x, b1.y, b1.z, b1.w}, v0[4] = {b0.x, b0.y, b0.z, b0.w}, vm[4] = {bm.x, bm.y, bm.z, bm.w};
+    float ou[4] = {du.x, du.y, du.z, du.w}, ov[4] = {dv.x, dv.y, dv.z, dv.w};
+    float4 c;
+    if (k.A) {
+        c = ld_once4(k.A + idx);
+    } else {
+        const float4 md = k.tMD ? ld_once4(k.tMD + idx) : make_float4(k.m_dt2, k.m_dt2, k.m_dt2, k.m_dt2);
+        const float4 dp = k.damp ? ld_once4(k.damp + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+        c = make_float4(md.x + dp.x * k.inv_dt, md.y + dp.y * k.inv_dt, md.z + dp.z * k.inv_dt,
+                        md.w + dp.w * k.inv_dt);
+    }
+    const float cc[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const float qu = tti_born_q(dd[e], u1[e], u0[e], um[e], k.inv_dt2);
+        const float qv = tti_born_q(dd[e], v1[e], v0[e], vm[e], k.inv_dt2);
+        if (k.A) {
+            ou[e] += qu * cc[e];
+            ov[e] += qv * cc[e];
+        } else {
+            ou[e] += qu / cc[e];
+            ov[e] += qv / cc[e];
+        }
+    }
+    *reinterpret_cast<float4 *>(k.du1 + idx) = make_float4(ou[0], ou[1], ou[2], ou[3]);
+    *reinterpret_cast<float4 *>(k.dv1 + idx) = make_float4(ov[0], ov[1], ov[2], ov[3]);
+}
+
+template <bool V4>
+__global__ void __launch_bounds__(256) k_tti_born_src(const TtiBK k) {
+    const int z = (V4 ? 4 : 1) * (blockIdx.x * blockDim.x + threadIdx.x);
+    const int y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (z >= k.n2 || y >= k.n1) return;
+    for (int x = blockIdx.z; x < k.n0; x += gridDim.z) {
+        if constexpr (V4) tti_born_point4(k, x, y, z);
+        else tti_born_point(k, x, y, z);
+    }
+}
+
+int tti_born_source(const TtiPlan &p, const TtiPlan &pd, int slot0, int slotm, int slot1, const float *dm,
+                    long long dsx, long long dsy, int dmh) {
+    TtiBK k;
+    k.u1 = p.u + (size_t)slot1 * p.slot_elems;
+    k.u0 = p.u + (size_t)slot0 * p.slot_elems;
+    k.um = p.u + (size_t)slotm * p.slot_elems;
+    k.v1 = p.v + (size_t)slot1 * p.slot_elems;
+    k.v0 = p.v + (size_t)slot0 * p.slot_elems;
+    k.vm = p.v + (size_t)slotm * p.slot_elems;
+    k.du1 = pd.u + (size_t)slot1 * p.slot_elems;
+    k.dv1 = pd.v + (size_t)slot1 * p.slot_elems;
+    // the fused plans tabulated A; the two-pass plans have m/dt^2 per point only with array parameters
+    k.A = p.use_fused ? p.coefA : nullptr;
+    k.tMD = p.use_fused ? nullptr : p.tMD;
+    k.damp = p.damp;
+    k.dm = dm;
+    k.sx = p.sx;
+    k.sy = p.sy;
+    k.dsx = dsx;
+    k.dsy = dsy;
+    k.n0 = p.n[0]; k.n1 = p.n[1]; k.n2 = p.n[2];
+    k.o0 = p.o[0]; k.o1 = p.o[1]; k.o2 = p.o[2];
+    k.dg0 = p.o[0] - p.so + dmh; k.dg1 = p.o[1] - p.so + dmh; k.dg2 = p.o[2] - p.so + dmh;
+    k.inv_dt = 1.0f / p.dt;
+    k.inv_dt2 = 1.0f / (p.dt * p.dt);
+    k.m_dt2 = (1.0f / (p.vp * p.vp)) * k.inv_dt2;
+    auto a16 = [](const void *q) { return (uintptr_t)q % 16 == 0; };
+    const bool v4 = k.o2 % 4 == 0 && k.n2 % 4 == 0 && k.sy % 4 == 0 && k.dg2 % 4 == 0 && k.dsy % 4 == 0 &&
+                    p.slot_elems % 4 == 0 && a16(p.u) && a16(p.v) && a16(pd.u) && a16(pd.v) && a16(dm) &&
+                    (!k.A || a16(k.A)) && (!k.tMD || a16(k.tMD)) && (!k.damp || a16(k.damp));
+    dim3 block(64, 4, 1);
+    const int nz = v4 ? k.n2 / 4 : k.n2;
+    dim3 grid((nz + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
+    char sweep[64];
+    snprintf(sweep, sizeof(sweep), "%s", b2_last_sweep_kernel());
+    note_sweep_kernel("%s+born_%s", sweep, v4 ? "v4" : "s");
+    if (v4) k_tti_born_src<true><<<grid, block, 0, stream()>>>(k);
+    else k_tti_born_src<false><<<grid, block, 0, stream()>>>(k);
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
 }
 
 static int env_int_tti(const char *name, int dflt) {

@@ -33,11 +33,20 @@ struct TtiPlan {
     // tabulated per-point coefficients (library scratch) when any parameter is an array
     float *tCx = nullptr, *tCy = nullptr, *tCz = nullptr, *tE2 = nullptr, *tSD = nullptr, *tMD = nullptr;
     bool has_arrays = false;
+    int tm_rows = 0;             // rows of the u / v tensor-map boxes (fused plans)
 };
 
 int tti_plan_init(TtiPlan &p, int kernel);
 void tti_plan_free(TtiPlan &p);
+// A plan for a second field pair (u, v) of the same layout that shares p's tables, scratch and sweep variant: only the
+// tensor maps are rebuilt for the new pointers. Fails (210) when p is fused and the new pointers do not qualify.
+int tti_plan_retarget(const TtiPlan &p, float *u, float *v, TtiPlan &out);
 // one time step over x in [xlo, xlo+xcount)
 int tti_step(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount);
+// Born source term (b2_tti_point.cuh) over the whole box after the linearised pair `pd` was stepped with the same
+// sweep as the background pair `p`: adds -dm * f.dt2 / (m/dt^2 + damp/dt) of p's u / v to pd's u / v at slot1.
+// `dm` has strides dsx, dsy and its own halo width dmh. Appends "+born_v4" / "+born_s" to the sweep-kernel name.
+int tti_born_source(const TtiPlan &p, const TtiPlan &pd, int slot0, int slotm, int slot1, const float *dm,
+                    long long dsx, long long dsy, int dmh);
 
 }  // namespace b2

@@ -322,6 +322,10 @@ class Operator:
                     return self._recognise_born(updates, injs, itps)
                 except _Unrecognised as born_why:
                     raise _Unrecognised(f"neither TTI ({tti_why}) nor Born ({born_why})") from None
+        if len(updates) == 4:
+            if any(_space_offsets(e.lhs, None)[0] != 1 for _, e in updates):
+                raise _Unrecognised("TTI Born is on the fast path forward in time only")
+            return self._recognise_tti_born(updates, injs, itps)
         raise _Unrecognised("unsupported number of update equations")
 
     @staticmethod
@@ -964,6 +968,144 @@ class Operator:
         self._attach_sparse(plan, injs, itps, [u, v], funcs, consts, syms, plan['m_role'])
         return plan
 
+    def _recognise_tti_born(self, updates, injs, itps):
+        """The reference's centred-TTI linearised-modelling operator `BornTTI` (examples/seismic/tti/operators.py:
+        532-586): `kernel_centered(model, u0, v0)`, the source injected into (u0.forward, v0.forward),
+        `kernel_centered(model, du, dv, qu=-dm*u0.dt2, qv=-dm*v0.dt2)`, the receivers sampling du + dv. The
+        linearised equations must be the background ones applied to (du, dv) plus `-dm * u0.dt2` (du) and
+        `-dm * v0.dt2` (dv) over the same denominator, with the same parameter objects."""
+        fields = [f for f, _ in updates]
+
+        def reads(eq):
+            return {id(n.function) for n in eq.rhs.evaluate.preorder() if n.is_Access} & {id(f) for f in fields}
+        rd = {id(f): reads(e) for f, e in updates}
+        pairs = [(i, j) for i in range(4) for j in range(i + 1, 4)
+                 if rd[id(fields[i])] | rd[id(fields[j])] <= {id(fields[i]), id(fields[j])}]
+        if len(pairs) != 1:
+            raise _Unrecognised("TTI Born: no unique background pair that reads no other field")
+        bg = [updates[k] for k in pairs[0]]
+        lin = [x for k, x in enumerate(updates) if k not in pairs[0]]
+        plan = self._recognise_tti(bg, [], [])
+        u0, v0 = plan['u'], plan['v']
+        grid, so, damp, consts = plan['grid'], plan['so'], plan['damp'], plan['consts']
+        for f, _ in lin:
+            if f.grid is not grid or f.space_order != so:
+                raise _Unrecognised("TTI Born: the linearised fields need the background grid and space order")
+        ku0 = {}
+        for acc, coef in self._coeffs(bg[0][1].rhs, [u0, v0]).items():
+            ku0[(0 if acc.function is u0 else 1,) + _space_offsets(acc, None)] = coef
+        kv0 = {}
+        for acc, coef in self._coeffs(bg[1][1].rhs, [u0, v0]).items():
+            kv0[(0 if acc.function is u0 else 1,) + _space_offsets(acc, None)] = coef
+        # split each linearised equation into taps on the linearised pair and on the background pair
+        (fa, ea), (fb, eb) = lin
+        ta = self._coeffs(ea.rhs, [fa, fb, u0, v0])
+        tb = self._coeffs(eb.rhs, [fa, fb, u0, v0])
+
+        def split(terms, du, dv):
+            own, ext = {}, {}
+            for acc, coef in terms.items():
+                k = _space_offsets(acc, None)
+                if k is None:
+                    raise _Unrecognised("non-affine wavefield access")
+                f = acc.function
+                if f is du or f is dv:
+                    own[(0 if f is du else 1,) + k] = coef
+                else:
+                    ext[(0 if f is u0 else 1,) + k] = coef
+            return own, ext
+        # du is the field whose equation carries the background u0 taps; dv the v0 ones
+        cand = []
+        for du, edu, dv, edv, tdu, tdv in ((fa, ea, fb, eb, ta, tb), (fb, eb, fa, ea, tb, ta)):
+            own_u, ext_u = split(tdu, du, dv)
+            own_v, ext_v = split(tdv, du, dv)
+            if set(own_u) == set(ku0) and set(own_v) == set(kv0):
+                cand.append((du, dv, own_u, ext_u, own_v, ext_v))
+        if not cand:
+            raise _Unrecognised("TTI Born: the linearised pair is not updated with the background taps")
+        allc = list(ku0.values()) + list(kv0.values())
+        for c in cand[0][2:]:
+            allc += list(c.values())
+        funcs, csts, syms = self._leaves(allc)
+        pnames = ('vp', 'epsilon', 'delta', 'theta', 'phi')
+        known = {id(c) for c in consts.values()}
+        if damp is not None:
+            known.add(id(damp))
+        for cst in csts:
+            if id(cst) not in known:
+                raise _Unrecognised(f"TTI Born: Constant {cst.name} is not one of the background parameters")
+        extra = {id(a.function): a.function for a in funcs if id(a.function) not in known}
+        if len(extra) != 1:
+            raise _Unrecognised("TTI Born: cannot identify the model perturbation dm (the linearised pair must use the "
+                                "background parameters)")
+        dm = next(iter(extra.values()))
+        if getattr(dm, 'is_TimeFunction', False) or dm.name in pnames:
+            raise _Unrecognised("TTI Born: cannot identify the model perturbation dm")
+        for ex in allc:
+            for n in ex.preorder():
+                if n.is_Access and n.function is dm:
+                    k = _space_offsets(n, None)
+                    if k is None or any(k[1]):
+                        raise _Unrecognised("dm accessed off-centre")
+        dtsym = plan['dt']
+        spv = {sp.name: float(v) for sp, v in grid.spacing_map.items()}
+        zero = (0, 0, 0)
+        rng = np.random.default_rng(2718)
+        errors = []
+        for du, dv, own_u, ext_u, own_v, ext_v in cand:
+            try:
+                for probe in range(2):
+                    base = {n: rng.uniform(0.2, 0.8) for n in pnames}
+                    gradv = {n: (rng.uniform(-0.02, 0.02, size=3) if isinstance(consts.get(n), Function)
+                                 else np.zeros(3)) for n in pnames}
+                    if 'phi' not in consts:
+                        base['phi'] = 0.0
+                    dt = rng.uniform(0.5, 2.0)
+                    dval = rng.uniform(0.5, 2.0) if damp is not None else 0.0
+                    dmv = rng.uniform(0.5, 2.0)
+
+                    def leaf(n):
+                        if n.is_Access:
+                            f = n.function
+                            if f is damp:
+                                return dval
+                            if f is dm:
+                                return dmv
+                            return float(base[f.name] + np.dot(gradv[f.name], _space_offsets(n, None)[1]))
+                        if n.is_Constant:
+                            return base[n.name]
+                        if n.name == dtsym.name:
+                            return dt
+                        if n.name in spv:
+                            return spv[n.name]
+                        raise _Unrecognised(f"unknown symbol {n.name}")
+                    for got, want in ((own_u, ku0), (own_v, kv0)):
+                        for k, c in want.items():
+                            w = eval_scalar(c, leaf)
+                            if abs(eval_scalar(got[k], leaf) - w) > 1e-9 * max(1.0, abs(w)):
+                                raise _Unrecognised(f"the linearised pair is not updated with the background stencil "
+                                                    f"(tap {k})")
+                    vp = base['vp']
+                    den = 1.0 / (vp * vp) / dt ** 2 + dval / dt
+                    for ext, src in ((ext_u, 0), (ext_v, 1)):
+                        want = {(src, 1, zero): -dmv / dt ** 2 / den, (src, 0, zero): 2 * dmv / dt ** 2 / den,
+                                (src, -1, zero): -dmv / dt ** 2 / den}
+                        if set(ext) != set(want):
+                            raise _Unrecognised("the linearised pair is not driven by a centred u0.dt2 / v0.dt2 term")
+                        for k, wv in want.items():
+                            if abs(eval_scalar(ext[k], leaf) - wv) > 1e-9 * max(1.0, abs(wv)):
+                                raise _Unrecognised("the source of the linearised pair is not -dm * u0.dt2 / "
+                                                    "-dm * v0.dt2")
+            except _Unrecognised as e:
+                errors.append(str(e))
+                continue
+            fu, cu, su = self._leaves(ku0.values())
+            self._attach_sparse(plan, injs, [], [u0, v0], fu, cu, su, plan['m_role'])
+            self._attach_sparse(plan, [], itps, [du, dv], fu, cu, su, plan['m_role'])
+            plan['born_du'], plan['born_dv'], plan['born_dm'] = du, dv, dm
+            return plan
+        raise _Unrecognised(f"TTI Born: {errors[0]}")
+
     # ------------------------------------------------------------------------------------------
     # introspection
     # ------------------------------------------------------------------------------------------
@@ -1028,7 +1170,7 @@ class Operator:
             out.append(p['m_role'][1])
         else:
             out.extend(p['consts'].values())
-        out += [p.get('born_U'), p.get('born_dm'), p.get('snap')]
+        out += [p.get('born_U'), p.get('born_du'), p.get('born_dv'), p.get('born_dm'), p.get('snap')]
         out += [s for s in (p['src'], p['rec']) if s is not None]
         return tuple(o for o in out if o is not None)
 
@@ -1200,7 +1342,19 @@ class Operator:
             if not isinstance(sn, TimeFunction) or sn.is_buffered or sn.grid.shape != grid.shape:
                 raise InvalidArgument("the snapshot override must be a saved TimeFunction on the same grid")
         args['born_U'] = self._resolve(kwargs, p.get('born_U'), post)
+        args['born_du'] = self._resolve(kwargs, p.get('born_du'), post)
+        args['born_dv'] = self._resolve(kwargs, p.get('born_dv'), post)
         args['born_dm'] = self._resolve(kwargs, p.get('born_dm'), post)
+        for key in ('born_du', 'born_dv'):
+            bu = args[key]
+            if bu is not None and (not isinstance(bu, TimeFunction) or bu.space_order != p['so'] or
+                                   bu.grid.shape != grid.shape):
+                raise InvalidArgument("incompatible override for a linearised wavefield")
+        if args['born_du'] is not None:
+            if not isinstance(args['born_dm'], Function):
+                raise InvalidArgument("`dm` must be a Function or an array of its allocated shape")
+            if grid.distributor.is_parallel:
+                raise InvalidArgument("TTI Born modelling does not run on a decomposed grid in this version")
         if args['born_U'] is not None:
             bu = args['born_U']
             if not isinstance(bu, TimeFunction) or bu.space_order != p['so'] or bu.grid.shape != grid.shape:
@@ -1738,6 +1892,10 @@ class Operator:
         a.deviceid = dev
         a.kernel = args['kernel']
         a.halo = distributed.halo_context(dev) if grid.distributor.is_parallel else None
+        if args.get('born_du') is not None:
+            a.born_du = self._field_obj(args['born_du'], dev, res, hold, written=True).ptr
+            a.born_dv = self._field_obj(args['born_dv'], dev, res, hold, written=True).ptr
+            a.born_dm = self._field_obj(args['born_dm'], dev, res, hold).ptr
         timers = L_.Profiler()
         a.timers = ctypes.pointer(timers)
         t0 = _time.perf_counter()

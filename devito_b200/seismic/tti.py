@@ -1,9 +1,9 @@
-"""TTI (centred kernel) forward modelling — mirror of examples/seismic/tti/operators.py:12-247,
-431-480 and tti/wavesolver.py (forward only)."""
-from .. import Eq, Operator, TimeFunction, solve, cos, sin, sqrt
+"""TTI (centred kernel) forward and linearised (Born) modelling — mirror of examples/seismic/tti/operators.py:12-247,
+431-480, 532-586 and tti/wavesolver.py (forward and jacobian)."""
+from .. import Eq, Function, Operator, TimeFunction, solve, cos, sin, sqrt
 from ..tools import memoized_meth
 
-__all__ = ['kernel_centered', 'ForwardOperator', 'AnisotropicWaveSolver']
+__all__ = ['kernel_centered', 'ForwardOperator', 'JacobianOperator', 'AnisotropicWaveSolver']
 
 
 def trig_func(model):
@@ -29,16 +29,27 @@ def Gzz_centered(model, field):
     return Gzz
 
 
-def kernel_centered(model, u, v):
-    """operators.py:186-247 + :12-39"""
+def _is_zero(q):
+    return isinstance(q, (int, float)) and q == 0
+
+
+def kernel_centered(model, u, v, qu=0, qv=0):
+    """operators.py:186-247 + :12-39; `qu` / `qv` are extra sources of the u / v equations (the linearised
+    operator passes -dm * u0.dt2 / -dm * v0.dt2)."""
     delta, epsilon = sqrt(1 + 2 * model.delta), 1 + 2 * model.epsilon
     Gxx = u.laplace - Gzz_centered(model, u)
     Gzz = Gzz_centered(model, v)
     H0 = epsilon * Gxx + delta * Gzz
     Hz = delta * Gxx + Gzz
     m, damp = model.m, model.damp
-    stencilp = solve(m * u.dt2 - H0 + damp * u.dt, u.forward)
-    stencilr = solve(m * v.dt2 - Hz + damp * v.dt, v.forward)
+    pdeu = m * u.dt2 - H0 + damp * u.dt
+    pdev = m * v.dt2 - Hz + damp * v.dt
+    if not _is_zero(qu):
+        pdeu = m * u.dt2 - H0 - qu + damp * u.dt
+    if not _is_zero(qv):
+        pdev = m * v.dt2 - Hz - qv + damp * v.dt
+    stencilp = solve(pdeu, u.forward)
+    stencilr = solve(pdev, v.forward)
     sd = model.grid.subdomains['physdomain']
     return [Eq(u.forward, stencilp, subdomain=sd), Eq(v.forward, stencilr, subdomain=sd)]
 
@@ -58,6 +69,24 @@ def ForwardOperator(model, geometry, space_order=4, save=False, kernel='centered
     stencils += src.inject(field=(u.forward, v.forward), expr=src * dt ** 2 / m)
     stencils += rec.interpolate(expr=u + v)
     return Operator(stencils, subs=model.spacing_map, name='ForwardTTI', **kwargs)
+
+
+def JacobianOperator(model, geometry, space_order=4, **kwargs):
+    """operators.py:532-586: the background pair (u0, v0) driven by the source, the linearised pair (du, dv) by
+    -dm * u0.dt2 / -dm * v0.dt2, the receivers sampling du + dv."""
+    if model.dim != 3:
+        raise NotImplementedError("only the 3-D centred TTI kernel is on this backend's path")
+    dt = model.grid.stepping_dim.spacing
+    m = model.m
+    mk = lambda n: TimeFunction(name=n, grid=model.grid, save=None, time_order=2, space_order=space_order)
+    u0, v0, du, dv = mk('u0'), mk('v0'), mk('du'), mk('dv')
+    dm = Function(name='dm', grid=model.grid, space_order=0)
+    src, rec = geometry.src, geometry.rec
+    eqn1 = kernel_centered(model, u0, v0)
+    eqn2 = kernel_centered(model, du, dv, qu=-dm * u0.dt2, qv=-dm * v0.dt2)
+    src_term = src.inject(field=(u0.forward, v0.forward), expr=src * dt ** 2 / m)
+    rec_term = rec.interpolate(expr=du + dv)
+    return Operator(eqn1 + src_term + eqn2 + rec_term, subs=model.spacing_map, name='BornTTI', **kwargs)
 
 
 class AnisotropicWaveSolver:
@@ -91,3 +120,23 @@ class AnisotropicWaveSolver:
         kwargs.update(model.physical_params(**kwargs))
         summary = self.op_fwd(save).apply(src=src, rec=rec, u=u, v=v, dt=kwargs.pop('dt', self.dt), **kwargs)
         return rec, u, v, summary
+
+    @memoized_meth
+    def op_jac(self):
+        return JacobianOperator(self.model, self.geometry, space_order=self.space_order, **self._kwargs)
+
+    def jacobian(self, dm, src=None, rec=None, u0=None, v0=None, du=None, dv=None, model=None, **kwargs):
+        """wavesolver.py:232-293: linearised (Born) modelling for the model perturbation `dm` (a Function, or an
+        array of the grid's shape). Returns (rec, u0, v0, du, dv, summary)."""
+        dt = kwargs.pop('dt', self.dt)
+        src = src or self.geometry.src
+        rec = rec or self.geometry.rec
+        mk = lambda n: TimeFunction(name=n, grid=self.model.grid, time_order=2, space_order=self.space_order)
+        u0 = u0 or mk('u0')
+        v0 = v0 or mk('v0')
+        du = du or mk('du')
+        dv = dv or mk('dv')
+        model = model or self.model
+        kwargs.update(model.physical_params(**kwargs))
+        summary = self.op_jac().apply(dm=dm, u0=u0, v0=v0, du=du, dv=dv, src=src, rec=rec, dt=dt, **kwargs)
+        return rec, u0, v0, du, dv, summary

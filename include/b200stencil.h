@@ -188,6 +188,15 @@ struct b2_tti_args {
      * factors are sampled where the reference samples them: at the Gz point inside Gz, at the
      * shifted point in the outer derivative `(Gz*cos(theta)).dz(...)` (tti/operators.py:92-102). */
     struct b2_dataobj *vp_arr, *epsilon_arr, *delta_arr, *theta_arr, *phi_arr;
+    /* Linearised (Born) modelling, the reference's `BornTTI` operator (tti/operators.py:532-586): all three NULL ->
+     * the forward operator above. All three non-NULL -> after (u, v) is stepped and `src` injected into it, the pair
+     * (born_du, born_dv) (same layout as u) is stepped with the same sweep and the extra sources
+     * -born_dm * u.dt2 (into du) and -born_dm * v.dt2 (into dv), divided by m/dt^2 + damp/dt, with u.dt2 taken after
+     * the injection; `rec` then samples born_du + born_dv instead of u + v. `born_dm` is a space array with its own
+     * halo width (hsize). born_du and born_dv are written back to the host when staged, born_dm is not. Not combined
+     * with halo exchange in this version; a missing member of the triple, a shape mismatch or a wrong born_dm
+     * extent returns 210.                                                                                 */
+    struct b2_dataobj *born_du, *born_dv, *born_dm;
 };
 int b2_tti_forward(const struct b2_tti_args *a);
 
@@ -325,7 +334,8 @@ void   b2_kernel_timing_enable(int on);
 /* name of the sweep kernel variant the last b2_iso_forward / b2_tti_forward call on this process launched, e.g.
  * "iso_generic", "iso_tma<4,vp>", "iso_tma2_v4<6,m>" (template radius, parameter kind scalar|vp|m), "tti_two_pass",
  * "tti_fused<2>", "tti_ws<pf1>", "tti_arr_ct2<4>" (radius); "" if the call launched none. Several kernels are
- * selected at run time (layout checks, B2_* switches): this tells which one computed the answer. */
+ * selected at run time (layout checks, B2_* switches): this tells which one computed the answer. A TTI Born call
+ * appends the path of its source term: "+born_v4" (float4 along z) or "+born_s" (one point per thread). */
 const char *b2_last_sweep_kernel(void);
 /* device memory helpers for hosts that do not use torch */
 void *b2_malloc_device(unsigned long nbytes, int deviceid);
