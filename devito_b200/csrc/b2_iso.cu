@@ -769,13 +769,17 @@ static int make_tmap(CUtensorMap *tm, const void *base, int rank, const int *dim
     return B2_OK;
 }
 
-// tile configuration per radius (TY, TZ4): sized so that the Q-stage plane ring plus the
-// (R+1)-stage tile ring fit the 227 KB of shared memory of one SM
-template <int R> struct TileOf;
-template <> struct TileOf<2> { static constexpr int TY = 32, TZ4 = 16; };
-template <> struct TileOf<4> { static constexpr int TY = 32, TZ4 = 16; };
-template <> struct TileOf<6> { static constexpr int TY = 16, TZ4 = 16; };
-template <> struct TileOf<8> { static constexpr int TY = 8, TZ4 = 16; };
+// tile configuration per radius (TY, TZ4) and coefficient kind (ARR: an array vp|m streams a third tile):
+// sized so that the Q-stage plane ring plus the (R+1)-stage tile ring fit the 227 KB of shared memory of one SM.
+// so=8 with a scalar vp: 16 x 128, so that every TMA box row and every warp's store is 512 contiguous bytes
+// rather than 256 (profiles/h100_iso_probe.json: the sweep's stream mix copies 7 % faster with 512-byte rows);
+// with an array vp|m the third tile ring does not fit beside the 16 x 128 plane ring, and it keeps 32 x 64.
+template <int R, bool ARR> struct TileOf;
+template <bool ARR> struct TileOf<2, ARR> { static constexpr int TY = 32, TZ4 = 16; };
+template <> struct TileOf<4, false> { static constexpr int TY = 16, TZ4 = 32; };
+template <> struct TileOf<4, true> { static constexpr int TY = 32, TZ4 = 16; };
+template <bool ARR> struct TileOf<6, ARR> { static constexpr int TY = 16, TZ4 = 16; };
+template <bool ARR> struct TileOf<8, ARR> { static constexpr int TY = 8, TZ4 = 16; };
 
 // k_iso_tma2 (two rows per thread, no tile ring): the radii whose k_iso_tma tile had to shrink
 template <int R> struct Tile2Of { static constexpr bool on = false; static constexpr int TY = 32, TZ4 = 16; };
@@ -870,7 +874,9 @@ static int iso_coef_tabulate(IsoPlan &p) {
 
 template <int R>
 static int plan_tma(IsoPlan &p) {
-    using T = TileOf<R>;
+    const bool arr = p.param_kind != B2_PARAM_SCALAR;
+    const int TY = arr ? TileOf<R, true>::TY : TileOf<R, false>::TY;
+    const int TZ4 = arr ? TileOf<R, true>::TZ4 : TileOf<R, false>::TZ4;
     constexpr int RZ = ceil4(R);
     const int dims4[4] = {p.a[2], p.a[1], p.a[0], p.tsize};
     const int dims3[3] = {p.a[2], p.a[1], p.a[0]};
@@ -900,11 +906,11 @@ static int plan_tma(IsoPlan &p) {
         }
         return B2_OK;
     }
-    if ((rc = make_tmap(&p.tm_uh, p.u, 4, dims4, 4 * T::TZ4 + 2 * RZ, T::TY + 2 * R))) return rc;
-    if ((rc = make_tmap(&p.tm_uc, p.u, 4, dims4, 4 * T::TZ4, T::TY))) return rc;
-    if ((rc = make_tmap(&p.tm_damp, p.coefA, 3, dims3, 4 * T::TZ4, T::TY))) return rc;
-    if (p.param_kind != B2_PARAM_SCALAR) {
-        if ((rc = make_tmap(&p.tm_par, p.coefB, 3, dims3, 4 * T::TZ4, T::TY))) return rc;
+    if ((rc = make_tmap(&p.tm_uh, p.u, 4, dims4, 4 * TZ4 + 2 * RZ, TY + 2 * R))) return rc;
+    if ((rc = make_tmap(&p.tm_uc, p.u, 4, dims4, 4 * TZ4, TY))) return rc;
+    if ((rc = make_tmap(&p.tm_damp, p.coefA, 3, dims3, 4 * TZ4, TY))) return rc;
+    if (arr) {
+        if ((rc = make_tmap(&p.tm_par, p.coefB, 3, dims3, 4 * TZ4, TY))) return rc;
     } else {
         p.tm_par = p.tm_damp;
     }
@@ -956,7 +962,7 @@ int iso_plan_init(IsoPlan &p, int kernel) {
 template <int R, int PK>
 static int launch_tma(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount,
                       const IsoFuse *fz = nullptr) {
-    using T = TileOf<R>;
+    using T = TileOf<R, PK != B2_PARAM_SCALAR>;
     using T2 = Tile2Of<R>;
     using C = IsoTmaCfg<R, T::TY, T::TZ4, PK>;
     using C2 = IsoTma2Cfg<R, T2::TY, T2::TZ4>;
