@@ -69,7 +69,9 @@ class TtiArgs(Structure):
                 ('vp_arr', POINTER(Dataobj)), ('epsilon_arr', POINTER(Dataobj)),
                 ('delta_arr', POINTER(Dataobj)), ('theta_arr', POINTER(Dataobj)),
                 ('phi_arr', POINTER(Dataobj)),
-                ('born_du', POINTER(Dataobj)), ('born_dv', POINTER(Dataobj)), ('born_dm', POINTER(Dataobj))]
+                ('born_du', POINTER(Dataobj)), ('born_dv', POINTER(Dataobj)), ('born_dm', POINTER(Dataobj)),
+                ('adjoint', c_int), ('grad', POINTER(Dataobj)), ('usave', POINTER(Dataobj)),
+                ('vsave', POINTER(Dataobj))]
 
 
 class Tap(Structure):

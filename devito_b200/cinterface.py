@@ -120,7 +120,7 @@ def signature(plan, name, distributed=False):
                 head.append(_Param(n, 'struct dataobj *restrict', f'{n}_vec'))
             else:
                 head.append(_Param(n, 'const float', n))
-        for key in ('born_du', 'born_dv', 'born_dm'):
+        for key in ('born_du', 'born_dv', 'born_dm', 'grad', 'usave', 'vsave'):
             f = plan.get(key)
             if f is not None:
                 head.append(_Param(f.name, 'struct dataobj *restrict', f'{f.name}_vec'))
@@ -277,6 +277,12 @@ def _tti_body(plan, distributed):
         L.append(f"  a.born_du = (struct b2_dataobj *){plan['born_du'].name}_vec;")
         L.append(f"  a.born_dv = (struct b2_dataobj *){plan['born_dv'].name}_vec;")
         L.append(f"  a.born_dm = (struct b2_dataobj *){plan['born_dm'].name}_vec;")
+    if plan.get('adjoint'):
+        L.append("  a.adjoint = 1;")
+    if plan.get('grad') is not None:
+        L.append(f"  a.grad = (struct b2_dataobj *){plan['grad'].name}_vec;")
+        L.append(f"  a.usave = (struct b2_dataobj *){plan['usave'].name}_vec;")
+        L.append(f"  a.vsave = (struct b2_dataobj *){plan['vsave'].name}_vec;")
     _tail(plan, 'b2_tti_forward', L, distributed)
     return L
 

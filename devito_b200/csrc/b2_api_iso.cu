@@ -43,19 +43,9 @@ int check_finite(const float *f, size_t n, bool &bad) {
     return B2_OK;
 }
 
-// Imaging condition (reference: `Inc(grad, -u * v.dt2)`, acoustic/operators.py:222):
-// grad[p] -= usave[time][p] * (v[t+1][p] - 2 v[t][p] + v[t-1][p]) / dt^2 over the iterated box.
-struct ImgK {
-    float *__restrict__ grad;
-    const float *__restrict__ us;
-    const float *__restrict__ v0;
-    const float *__restrict__ v1;
-    const float *__restrict__ v2;
-    long long sx, sy, gsx, gsy;      // strides of the wavefields / of grad
-    int n0, n1, n2, o0, o1, o2, g0, g1, g2;
-    float inv_dt2;
-};
-
+// Imaging condition (reference: `Inc(grad, -u * v.dt2)`, acoustic/operators.py:222; the TTI gradient's
+// `Inc(dm, -(u0 * du.dt2 + v0 * dv.dt2))`, tti/operators.py `JacobianAdjOperator`, with the second pair):
+// grad[p] -= usave[time][p] * (v[t+1][p] - 2 v[t][p] + v[t-1][p]) / dt^2 (+ the same of us2, w) over the iterated box.
 __global__ void __launch_bounds__(256) k_imaging(ImgK k) {
     const int z = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
@@ -64,8 +54,21 @@ __global__ void __launch_bounds__(256) k_imaging(ImgK k) {
         const long long i = (long long)(k.o0 + x) * k.sx + (long long)(k.o1 + y) * k.sy + (k.o2 + z);
         const long long g = (long long)(k.g0 + x) * k.gsx + (long long)(k.g1 + y) * k.gsy + (k.g2 + z);
         const float d2 = (k.v1[i] - 2.0f * k.v0[i] + k.v2[i]) * k.inv_dt2;
-        k.grad[g] = k.grad[g] - k.us[i] * d2;
+        if (k.us2) {
+            const float e2 = (k.w1[i] - 2.0f * k.w0[i] + k.w2[i]) * k.inv_dt2;
+            k.grad[g] = k.grad[g] - fmaf(k.us[i], d2, k.us2[i] * e2);
+        } else {
+            k.grad[g] = k.grad[g] - k.us[i] * d2;
+        }
     }
+}
+
+int launch_imaging(const ImgK &ik) {
+    dim3 blk(64, 4, 1), grd((ik.n2 + 63) / 64, (ik.n1 + 3) / 4, (unsigned)(ik.n0 < 65535 ? ik.n0 : 65535));
+    k_imaging<<<grd, blk, 0, stream()>>>(ik);
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
 }
 
 // Section timing with a reusable pool of CUDA events: 4 events per time step.
@@ -823,6 +826,7 @@ extern "C" int b2_iso_forward(const struct b2_iso_args *a) {
                 return cleanup(B2_ERR_INVALID);
             }
             ImgK ik;
+            ik.us2 = ik.w0 = ik.w1 = ik.w2 = nullptr;
             ik.grad = (float *)grad.d;
             ik.us = (const float *)usave.d + (size_t)time * p.slot_elems;
             ik.v0 = p.u + (size_t)t0 * p.slot_elems;
@@ -836,10 +840,7 @@ extern "C" int b2_iso_forward(const struct b2_iso_args *a) {
             ik.o0 = p.o[0]; ik.o1 = p.o[1]; ik.o2 = p.o[2];
             ik.g0 = a->x_m + gh; ik.g1 = a->y_m + gh; ik.g2 = a->z_m + gh;
             ik.inv_dt2 = 1.0f / (a->dt * a->dt);
-            dim3 blk(64, 4, 1), grd((ik.n2 + 63) / 64, (ik.n1 + 3) / 4, (unsigned)(ik.n0 < 65535 ? ik.n0 : 65535));
-            k_imaging<<<grd, blk, 0, stream()>>>(ik);
-            count_launch();
-            B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+            if ((rc = launch_imaging(ik))) return cleanup(rc);
         }
         if (per_step_events) se.next();
         if (a->errctl && ((time - a->time_m) % 100 == 99 || time == (a->adjoint ? a->time_m : a->time_M))) {

@@ -4,7 +4,9 @@
 // fields in one call (tests/test_mpi.py:3690-3694). With born_du / born_dv / born_dm the loop is that of the
 // reference's `BornTTI` (tti/operators.py:532-586): the background pair is stepped and the source injected into it,
 // then the linearised pair is stepped with the same sweep and driven by -dm * u0.dt2 / -dm * v0.dt2, and the
-// receivers sample du + dv.
+// receivers sample du + dv. With `adjoint` the loop is that of the reference's `AdjointTTI` (time reversed, the
+// mixes e2 p + sd r / sd p + r formed by k_tti_adj_mix and swept with the forward kernels' adjoint variants), and
+// with grad / usave / vsave that of `GradientTTI` (the imaging condition after each step and its injection).
 #include "b2_tti.cuh"
 #include "b2_sparse.cuh"
 #include "b2_halo.cuh"
@@ -24,12 +26,13 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
     const int so = a->space_order;
     int rc = B2_OK;
 
-    DevArray u, v, damp, parr[5], bdu, bdv, bdm;
+    DevArray u, v, damp, parr[5], bdu, bdv, bdm, grad, usave, vsave;
     bool sparr[5] = {false, false, false, false, false};
     SparseDev src, rec;
-    TtiPlan p, pd;
+    TtiPlan p, pd, pa;
     FieldGeom g;
-    bool su = false, sv = false, sd = false, sdu = false, sdv = false, sdm = false;
+    bool su = false, sv = false, sd = false, sdu = false, sdv = false, sdm = false, sg = false, sus = false,
+         svs = false;
 
     auto cleanup = [&](int code) {
         const bool back = code == B2_OK || code == B2_ERR_NAN;
@@ -38,13 +41,16 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
         const int r4 = sdu ? stage_out(bdu, back) : B2_OK;
         const int r5 = sdv ? stage_out(bdv, back) : B2_OK;
         if (sdm) stage_out(bdm, false);
+        if (sus) stage_out(usave, false);
+        if (svs) stage_out(vsave, false);
+        const int r6 = sg ? stage_out(grad, back) : B2_OK;
         if (sd) stage_out(damp, false);
         for (int i = 0; i < 5; ++i) if (sparr[i]) stage_out(parr[i], false);
         sparse_stage_out(src, false);
         int r3 = sparse_stage_out(rec, back);
         tti_plan_free(p);
         if (code != B2_OK) return code;
-        return r1 ? r1 : (r2 ? r2 : (r3 ? r3 : (r4 ? r4 : r5)));
+        return r1 ? r1 : (r2 ? r2 : (r3 ? r3 : (r4 ? r4 : (r5 ? r5 : r6))));
     };
 
     if ((rc = stage_in(a->u, 4, u, true))) return cleanup(rc);
@@ -89,6 +95,43 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
         for (int d = 0; d < 3; ++d)
             if (dmh < 0 || bdm.size[d] != u.size[d + 1] - 2 * so + 2 * dmh) {
                 set_error("b2_tti_forward: born_dm extent %d on dim %d does not match the grid", bdm.size[d], d);
+                return cleanup(B2_ERR_INVALID);
+            }
+    }
+    const bool adj = a->adjoint != 0;
+    int gh = 0;
+    if (adj && a->halo) {
+        set_error("b2_tti_forward: the adjoint is not combined with halo exchange in this version");
+        return cleanup(B2_ERR_INVALID);
+    }
+    if (adj && born) {
+        set_error("b2_tti_forward: the adjoint is not combined with Born modelling");
+        return cleanup(B2_ERR_INVALID);
+    }
+    if (a->grad || a->usave || a->vsave) {
+        if (!a->grad || !a->usave || !a->vsave) {
+            set_error("b2_tti_forward: the imaging condition needs grad, usave and vsave together");
+            return cleanup(B2_ERR_INVALID);
+        }
+        if (!adj) {
+            set_error("b2_tti_forward: the imaging condition runs with the adjoint only");
+            return cleanup(B2_ERR_INVALID);
+        }
+        if ((rc = stage_in(a->grad, 3, grad, true))) return cleanup(rc);
+        sg = true;
+        if ((rc = stage_in(a->usave, 4, usave, true))) return cleanup(rc);
+        sus = true;
+        if ((rc = stage_in(a->vsave, 4, vsave, true))) return cleanup(rc);
+        svs = true;
+        for (int d = 1; d < 4; ++d)
+            if (usave.size[d] != u.size[d] || vsave.size[d] != u.size[d]) {
+                set_error("b2_tti_forward: usave and vsave must have the space layout of u");
+                return cleanup(B2_ERR_INVALID);
+            }
+        gh = a->grad->hsize ? a->grad->hsize[0] : (grad.size[0] - (u.size[1] - 2 * so)) / 2;
+        for (int d = 0; d < 3; ++d)
+            if (gh < 0 || grad.size[d] != u.size[d + 1] - 2 * so + 2 * gh) {
+                set_error("b2_tti_forward: grad extent %d on dim %d does not match the grid", grad.size[d], d);
                 return cleanup(B2_ERR_INVALID);
             }
     }
@@ -146,6 +189,7 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
         if (born && kernel != 2 && ((uintptr_t)bdu.d % 16 != 0 || (uintptr_t)bdv.d % 16 != 0)) kernel = 1;
         if ((rc = tti_plan_init(p, kernel))) return cleanup(rc);
         if (born && (rc = tti_plan_retarget(p, (float *)bdu.d, (float *)bdv.d, pd))) return cleanup(rc);
+        if (adj && (rc = tti_plan_adjoint(p, pa))) return cleanup(rc);
     }
 
     g.sx = p.sx;
@@ -170,11 +214,15 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
     }
     const bool p2p = a->halo && halo_p2p_active(a->halo, p.u) && halo_p2p_active(a->halo, p.v);
     if (a->halo) a->halo->reset_primed();
-    for (int time = a->time_m; time <= a->time_M; ++time) {
+    const int dir = adj ? -1 : 1;
+    for (int time = adj ? a->time_M : a->time_m; adj ? time >= a->time_m : time <= a->time_M; time += dir) {
         const int t0 = ((time % T) + T) % T;
-        const int t1 = (((time + 1) % T) + T) % T;
-        const int t2 = (((time - 1) % T) + T) % T;
-        if (a->halo) {
+        const int t1 = (((time + dir) % T) + T) % T;     // written
+        const int t2 = (((time - dir) % T) + T) % T;     // the other level read
+        if (adj) {
+            if ((rc = tti_adj_mix(pa, t0))) return cleanup(rc);
+            if ((rc = tti_step(pa, t0, t2, t1, 0, p.n[0]))) return cleanup(rc);
+        } else if (a->halo) {
             if ((rc = halo_exchange_and_step_tti(a->halo, p, t0, t2, t1))) return cleanup(rc);
         } else {
             if ((rc = tti_step(p, t0, t2, t1, 0, p.n[0]))) return cleanup(rc);
@@ -202,7 +250,32 @@ extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
         const size_t ro = (size_t)(a->rec_toff ? t1 : t0) * p.slot_elems;
         const TtiPlan &pr = born ? pd : p;
         if ((rc = launch_interp(rec, g, pr.u + ro, pr.v + ro, time))) return cleanup(rc);
-        if (a->errctl && ((time - a->time_m) % 100 == 99 || time == a->time_M)) {
+        if (sg) {
+            if (time < 0 || time >= usave.size[0] || time >= vsave.size[0]) {
+                set_error("b2_tti_forward: time=%d outside the saved wavefields (nt=%d, %d)", time, usave.size[0],
+                          vsave.size[0]);
+                return cleanup(B2_ERR_INVALID);
+            }
+            ImgK ik;
+            ik.grad = (float *)grad.d;
+            ik.us = (const float *)usave.d + (size_t)time * p.slot_elems;
+            ik.v0 = p.u + (size_t)t0 * p.slot_elems;
+            ik.v1 = p.u + (size_t)t1 * p.slot_elems;
+            ik.v2 = p.u + (size_t)t2 * p.slot_elems;
+            ik.us2 = (const float *)vsave.d + (size_t)time * p.slot_elems;
+            ik.w0 = p.v + (size_t)t0 * p.slot_elems;
+            ik.w1 = p.v + (size_t)t1 * p.slot_elems;
+            ik.w2 = p.v + (size_t)t2 * p.slot_elems;
+            ik.sx = p.sx; ik.sy = p.sy;
+            ik.gsy = grad.size[2];
+            ik.gsx = (long long)grad.size[1] * grad.size[2];
+            ik.n0 = p.n[0]; ik.n1 = p.n[1]; ik.n2 = p.n[2];
+            ik.o0 = p.o[0]; ik.o1 = p.o[1]; ik.o2 = p.o[2];
+            ik.g0 = a->x_m + gh; ik.g1 = a->y_m + gh; ik.g2 = a->z_m + gh;
+            ik.inv_dt2 = 1.0f / (a->dt * a->dt);
+            if ((rc = launch_imaging(ik))) return cleanup(rc);
+        }
+        if (a->errctl && ((time - a->time_m) % 100 == 99 || time == (adj ? a->time_m : a->time_M))) {
             bool bad = false;
             if ((rc = check_finite(fu, p.slot_elems, bad))) return cleanup(rc);
             if (bad) { set_error("NaN/Inf detected in u at time=%d", time); return cleanup(B2_ERR_NAN); }

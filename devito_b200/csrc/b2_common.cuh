@@ -101,6 +101,25 @@ struct DevArray {
 int stage_in(const b2_dataobj *obj, int ndim, DevArray &out, bool copy_in);
 int stage_out(DevArray &a, bool copy_back);
 
+// Imaging condition over the iterated box, after the step and its injection (k_imaging, b2_api_iso.cu):
+// grad -= us * (v1 - 2 v0 + v2) / dt^2, and with us2 != nullptr also - us2 * (w1 - 2 w0 + w2) / dt^2 (the TTI
+// gradient's second pair). 24 B/point with one pair, 40 with two.
+struct ImgK {
+    float *__restrict__ grad;
+    const float *__restrict__ us;
+    const float *__restrict__ v0;
+    const float *__restrict__ v1;
+    const float *__restrict__ v2;
+    const float *__restrict__ us2;
+    const float *__restrict__ w0;
+    const float *__restrict__ w1;
+    const float *__restrict__ w2;
+    long long sx, sy, gsx, gsy;      // strides of the wavefields / of grad
+    int n0, n1, n2, o0, o1, o2, g0, g1, g2;
+    float inv_dt2;
+};
+int launch_imaging(const ImgK &k);
+
 // section timers: CUDA-event accumulation per section, flushed to b2_profiler at exit
 struct SectionTimer {
     bool enabled = false;

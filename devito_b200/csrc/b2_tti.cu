@@ -48,6 +48,9 @@ struct TtiK {
     const float *__restrict__ tE2;
     const float *__restrict__ tSD;
     const float *__restrict__ tMD;
+    // ADJ: the centre of the update, p[t] / r[t] (u0 / v0 then hold the mixes of the adjoint plan)
+    const float *__restrict__ pc;
+    const float *__restrict__ rc;
 };
 
 // time-invariant tables for array-valued parameters (the reference hoists the same quantities:
@@ -97,6 +100,9 @@ __global__ void __launch_bounds__(256) k_tti_gz(TtiK k) {
     }
 }
 
+// ADJ: the adjoint step -- stencil inputs are the mixes a, b (combined with e2 = 1, sd = 0), the centre of the
+// time update comes from p[t], r[t]
+template <bool ADJ>
 __global__ void __launch_bounds__(256) k_tti_update(TtiK k) {
     const int h = k.R / 2;
     const int z = blockIdx.x * blockDim.x + threadIdx.x;
@@ -125,14 +131,22 @@ __global__ void __launch_bounds__(256) k_tti_update(TtiK k) {
             gv = fmaf(cz * k.w1[2][j], k.gzv[iz], gv);
         }
         const float gh = lap - gu;                  // Gxx + Gyy applied to u
-        const float e2 = k.tE2 ? k.tE2[idx] : k.e2, sd = k.tSD ? k.tSD[idx] : k.sd;
         const float md = k.tMD ? k.tMD[idx] : k.m_dt2;
-        const float H0 = e2 * gh + sd * gv;
-        const float Hz = sd * gh + gv;
+        float H0, Hz, fu = uc, fv = vc;
+        if constexpr (ADJ) {
+            H0 = gh;
+            Hz = gv;
+            fu = k.pc[idx];
+            fv = k.rc[idx];
+        } else {
+            const float e2 = k.tE2 ? k.tE2[idx] : k.e2, sd = k.tSD ? k.tSD[idx] : k.sd;
+            H0 = e2 * gh + sd * gv;
+            Hz = sd * gh + gv;
+        }
         const float d = k.damp ? k.damp[idx] * k.inv_dt : 0.f;
         const float den = md + d;
-        k.u1[idx] = (md * (2.f * uc - k.um[idx]) + d * uc + H0) / den;
-        k.v1[idx] = (md * (2.f * vc - k.vm[idx]) + d * vc + Hz) / den;
+        k.u1[idx] = (md * (2.f * fu - k.um[idx]) + d * fu + H0) / den;
+        k.v1[idx] = (md * (2.f * fv - k.vm[idx]) + d * fv + Hz) / den;
     }
 }
 
@@ -186,6 +200,9 @@ struct TtiFK {
     int ay, az;                // allocated extents of dims 1, 2 (bounds of the table reads on the extended tile)
     int pfc;                   // != 0: prefetch next iteration's stage-A factor groups into L2
     int hint;                  // != 0: once-per-CTA table reads bypass L1 allocation
+    // ADJ: the centre of the update, p[t] / r[t]; the tensor maps then cover the mixes of the adjoint plan
+    const float *__restrict__ pc;
+    const float *__restrict__ rc;
 };
 
 // D = how many batches the producer may run ahead of the slowest consumer (ring depths follow); CT = the array-
@@ -222,7 +239,10 @@ struct TtiCfg {
 // iteration. 52 B/point instead of 28.
 // CT = true (needs ARR): cx, cy, cz of stage A's plane arrive by TMA with the u / v batch instead (boxes of the
 // extended tile, zero-filled outside the array), so stage A has no global loads at all.
-template <int R, int TY, bool ARR, int CT>
+// ADJ: the adjoint step. The tensor maps cover the mixes a = e2 p + sd r, b = sd p + r, combined with e2 = 1, sd = 0;
+// the centre of the time update is loaded from p[t], r[t] (with ARR in place of the e2 / sd tables, so the array
+// kernel moves the same bytes as the forward one).
+template <int R, int TY, bool ARR, int CT, bool ADJ = false>
 __global__ void __launch_bounds__(TY * 16 + 32, 1)
 k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_v,
             const __grid_constant__ CUtensorMap tm_cx, const __grid_constant__ CUtensorMap tm_cy,
@@ -391,12 +411,28 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
                 pa = make_float4(t[8], t[9], t[10], t[11]);
             }
         }
+        float4 pcn = make_float4(0, 0, 0, 0), rcn = pcn;      // ADJ: p[t], r[t] at the four points
+        if constexpr (ADJ && !ARR) {
+            if (x >= xs && zcnt > 0) {
+                if (zcnt == 4) {
+                    pcn = *reinterpret_cast<const float4 *>(k.pc + gi);
+                    rcn = *reinterpret_cast<const float4 *>(k.rc + gi);
+                } else {
+                    float t[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+                    for (int i = 0; i < zcnt; ++i) { t[i] = k.pc[gi + i]; t[4 + i] = k.rc[gi + i]; }
+                    pcn = make_float4(t[0], t[1], t[2], t[3]);
+                    rcn = make_float4(t[4], t[5], t[6], t[7]);
+                }
+            }
+        }
         float4 pe2 = pu, psd = pu, pmd = pu;
         if constexpr (ARR) {
             // the 16-byte table reads stay inside the array for every gz < nz (az % 4 == 0, >= 4 cells of halo)
             if (x >= xs && zcnt > 0) {
-                pe2 = ldt(k.tE2 + gi);
-                psd = ldt(k.tSD + gi);
+                if constexpr (!ADJ) {
+                    pe2 = ldt(k.tE2 + gi);
+                    psd = ldt(k.tSD + gi);
+                }
                 pmd = ldt(k.tMD + gi);
             }
             // stage A of the NEXT iteration reads cx, cy, cz of plane x+H for the first time: ask L2 for them now
@@ -502,6 +538,12 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
 
         // ---- stage B: output plane x ----
         if (x >= xs) {
+            if constexpr (ADJ && ARR && CT != 0) {   // in place of the e2 / sd tables; issued here, where registers are free
+                if (zcnt > 0) {
+                    pcn = ldt(k.pc + gi);
+                    rcn = ldt(k.rc + gi);
+                }
+            }
             // ARR: cy at the R rows and cz on the z segment around the four points, issued ahead of their use
             float4 cyq[ARR ? R : 1];
             float czr[ARR ? 12 : 1];
@@ -615,16 +657,27 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
                     }
                 }
             }
+            if constexpr (ADJ && ARR && CT == 0) {   // CT = 0 holds the factor queues longest: load just before use
+                if (zcnt > 0) {
+                    pcn = ldt(k.pc + gi);
+                    rcn = ldt(k.rc + gi);
+                }
+            }
             float4 ou, ov;
 #define B2_TTI_UPD(F)                                                              \
             {                                                                      \
                 const float gh = lap.F - zu4.F;                                    \
-                const float e2_ = ARR ? pe2.F : k.e2, sd_ = ARR ? psd.F : k.sd;    \
                 const float md_ = ARR ? pmd.F : k.m_dt2;                           \
+                if constexpr (ADJ) {                                               \
+                    ou.F = fmaf(pa.F, fmaf(md_, pcn.F - pu.F, gh), pcn.F);         \
+                    ov.F = fmaf(pa.F, fmaf(md_, rcn.F - pv.F, zv4.F), rcn.F);      \
+                } else {                                                           \
+                const float e2_ = ARR ? pe2.F : k.e2, sd_ = ARR ? psd.F : k.sd;    \
                 const float H0 = fmaf(e2_, gh, sd_ * zv4.F);                       \
                 const float Hz = fmaf(sd_, gh, zv4.F);                             \
                 ou.F = fmaf(pa.F, fmaf(md_, c.F - pu.F, H0), c.F);                 \
                 ov.F = fmaf(pa.F, fmaf(md_, vcn.F - pv.F, Hz), vcn.F);             \
+                }                                                                  \
             }
             B2_TTI_UPD(x) B2_TTI_UPD(y) B2_TTI_UPD(z) B2_TTI_UPD(w)
 #undef B2_TTI_UPD
@@ -1071,8 +1124,9 @@ template <> struct TtiTileArr2<4> { static constexpr int TY = 20; };
 static int env_int_tti(const char *name, int dflt);
 
 // scratch cached across calls
-static float *g_tti_scratch[9] = {};
-static size_t g_tti_scratch_elems[9] = {};
+// 0: A, 1-2: Gz(u), Gz(v) (two-pass), 3-8: per-point tables, 9-10: the adjoint's mixes
+static float *g_tti_scratch[11] = {};
+static size_t g_tti_scratch_elems[11] = {};
 static int tti_scratch(int which, size_t elems, float **out) {
     if (g_tti_scratch_elems[which] != elems) {
         if (g_tti_scratch[which]) cudaFree(g_tti_scratch[which]);
@@ -1179,6 +1233,26 @@ int tti_plan_retarget(const TtiPlan &p, float *u, float *v, TtiPlan &out) {
     return B2_OK;
 }
 
+int tti_plan_adjoint(const TtiPlan &p, TtiPlan &out) {
+    float *a = nullptr, *b = nullptr;
+    int rc;
+    if ((rc = tti_scratch(9, p.slot_elems, &a))) return rc;
+    if ((rc = tti_scratch(10, p.slot_elems, &b))) return rc;
+    out = p;                // tables, A and two-pass scratch shared; u / v stay p / r
+    out.ma = a;
+    out.mb = b;
+    out.adj = true;
+    if (p.use_fused) {      // one slot each (cudaMalloc'ed, so 16-byte aligned): the sweep reads slot 0 of the maps
+        // the scalar so=8 adjoint sweeps with k_tti_fused<4> where the forward takes k_tti_ws (its own tile height)
+        if (!p.arr_fused) out.tm_rows = (p.R == 2 ? TtiTile<2>::TY : TtiTile<4>::TY) + 2 * p.R;
+        if ((rc = tti_make_tmap(&out.tm_u, a, p.a, 1, 72, out.tm_rows))) return rc;
+        if ((rc = tti_make_tmap(&out.tm_v, b, p.a, 1, 72, out.tm_rows))) return rc;
+        if (!p.arr_ct) out.tm_cx = out.tm_cy = out.tm_cz = out.tm_u;
+    }
+    return B2_OK;
+}
+
+
 // Born source term, 48 B/point: dm, u0 and v0 at t+1, t, t-1 and A (or the parameters of the denominator) read once,
 // du[t+1] and dv[t+1] read and written. V4: four consecutive z points per thread with 16-byte accesses; the streams
 // read once go through `ld.global.nc.L1::no_allocate`.
@@ -1281,6 +1355,63 @@ int tti_born_source(const TtiPlan &p, const TtiPlan &pd, int slot0, int slotm, i
     return B2_OK;
 }
 
+// a = e2 p + sd r, b = sd p + r over the whole slot; e2 / sd are the scalars or the per-point tables (which cover
+// the whole allocation too). V4: four consecutive points per thread, the streams read once bypass L1.
+struct TtiMixK {
+    const float *__restrict__ p;
+    const float *__restrict__ r;
+    float *__restrict__ a;
+    float *__restrict__ b;
+    const float *__restrict__ tE2;
+    const float *__restrict__ tSD;
+    float e2, sd;
+    size_t n;
+};
+
+template <bool V4>
+__global__ void __launch_bounds__(256) k_tti_adj_mix(const TtiMixK k) {
+    size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    if constexpr (V4) {
+        for (; 4 * i < k.n; i += stride) {
+            const float4 p = ld_once4(k.p + 4 * i), r = ld_once4(k.r + 4 * i);
+            const float4 e = k.tE2 ? ld_once4(k.tE2 + 4 * i) : make_float4(k.e2, k.e2, k.e2, k.e2);
+            const float4 s = k.tSD ? ld_once4(k.tSD + 4 * i) : make_float4(k.sd, k.sd, k.sd, k.sd);
+            float4 a, b;
+            tti_adj_mix_point(e.x, s.x, p.x, r.x, a.x, b.x);
+            tti_adj_mix_point(e.y, s.y, p.y, r.y, a.y, b.y);
+            tti_adj_mix_point(e.z, s.z, p.z, r.z, a.z, b.z);
+            tti_adj_mix_point(e.w, s.w, p.w, r.w, a.w, b.w);
+            *reinterpret_cast<float4 *>(k.a + 4 * i) = a;
+            *reinterpret_cast<float4 *>(k.b + 4 * i) = b;
+        }
+    } else {
+        for (; i < k.n; i += stride)
+            tti_adj_mix_point(k.tE2 ? k.tE2[i] : k.e2, k.tSD ? k.tSD[i] : k.sd, k.p[i], k.r[i], k.a[i], k.b[i]);
+    }
+}
+
+int tti_adj_mix(const TtiPlan &pa, int slot0) {
+    TtiMixK k;
+    k.p = pa.u + (size_t)slot0 * pa.slot_elems;
+    k.r = pa.v + (size_t)slot0 * pa.slot_elems;
+    k.a = pa.ma;
+    k.b = pa.mb;
+    k.tE2 = pa.has_arrays ? pa.tE2 : nullptr;
+    k.tSD = pa.has_arrays ? pa.tSD : nullptr;
+    k.e2 = 1.0f + 2.0f * pa.epsilon;
+    k.sd = sqrtf(1.0f + 2.0f * pa.delta);
+    k.n = pa.slot_elems;
+    auto a16 = [](const void *q) { return q == nullptr || (uintptr_t)q % 16 == 0; };
+    const bool v4 = k.n % 4 == 0 && a16(k.p) && a16(k.r) && a16(k.a) && a16(k.b) && a16(k.tE2) && a16(k.tSD);
+    B2_SM_COUNT(sms);
+    if (v4) k_tti_adj_mix<true><<<sms * 8, 256, 0, stream()>>>(k);
+    else k_tti_adj_mix<false><<<sms * 8, 256, 0, stream()>>>(k);
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
+}
+
 static int env_int_tti(const char *name, int dflt) {
     const char *v = getenv(name);
     return v ? atoi(v) : dflt;
@@ -1293,16 +1424,16 @@ static int tti_launch_fused_arr(const TtiPlan &p, int slot0, int slotm, int slot
     using C0 = TtiCfg<R, TY1, 3, 0>;
     using C1 = TtiCfg<R, TY1, 2, 1>;
     using C2 = TtiCfg<R, TY2, 2, 2>;
-    auto kern0 = k_tti_fused<R, TY1, true, 0>;
-    auto kern1 = k_tti_fused<R, TY1, true, 1>;
-    auto kern2 = k_tti_fused<R, TY2, true, 2>;
+    auto kern0 = p.adj ? k_tti_fused<R, TY1, true, 0, true> : k_tti_fused<R, TY1, true, 0>;
+    auto kern1 = p.adj ? k_tti_fused<R, TY1, true, 1, true> : k_tti_fused<R, TY1, true, 1>;
+    auto kern2 = p.adj ? k_tti_fused<R, TY2, true, 2, true> : k_tti_fused<R, TY2, true, 2>;
     static_assert(C0::SMEM <= 232448 && C1::SMEM <= 232448 && C2::SMEM <= 232448, "shared memory per CTA");
-    static bool attr_set = false;
-    if (!attr_set) {
+    static bool attr_set[2] = {false, false};
+    if (!attr_set[p.adj]) {
         B2_CUDA(cudaFuncSetAttribute(kern0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C0::SMEM), B2_ERR_LAUNCH);
         B2_CUDA(cudaFuncSetAttribute(kern1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C1::SMEM), B2_ERR_LAUNCH);
         B2_CUDA(cudaFuncSetAttribute(kern2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2::SMEM), B2_ERR_LAUNCH);
-        attr_set = true;
+        attr_set[p.adj] = true;
     }
     const int TY = p.arr_ct == 2 ? TY2 : TY1;
     using C = C0;      // TZ is common to the three configurations
@@ -1334,14 +1465,18 @@ static int tti_launch_fused_arr(const TtiPlan &p, int slot0, int slotm, int slot
     lx = std::min(lx, xcount);
     k.lx = lx;
     const int ntx = (xcount + lx - 1) / lx;
-    k.slot0 = slot0;
+    k.slot0 = p.adj ? 0 : slot0;
+    if (p.adj) {
+        k.pc = p.u + (size_t)slot0 * p.slot_elems;
+        k.rc = p.v + (size_t)slot0 * p.slot_elems;
+    }
     k.tCx = p.tCx; k.tCy = p.tCy; k.tCz = p.tCz; k.tE2 = p.tE2; k.tSD = p.tSD; k.tMD = p.tMD;
     k.pfc = env_int_tti("B2_TTI_ARR_PREFETCH", 1);
     k.hint = env_int_tti("B2_TTI_ARR_HINT", 1);
     for (int i = 0; i <= R; ++i) { k.w2x[i] = p.w2[0][i]; k.w2y[i] = p.w2[1][i]; k.w2z[i] = p.w2[2][i]; }
     for (int i = 0; i < R; ++i) { k.w1x[i] = p.w1[0][i]; k.w1y[i] = p.w1[1][i]; k.w1z[i] = p.w1[2][i]; }
     timing_begin();
-    note_sweep_kernel("tti_arr_ct%d<%d>", p.arr_ct == 2 ? 2 : (p.arr_ct == 1 ? 1 : 0), R);
+    note_sweep_kernel("tti_arr_ct%d<%d>%s", p.arr_ct == 2 ? 2 : (p.arr_ct == 1 ? 1 : 0), R, p.adj ? "+adj" : "");
     const unsigned nblk = (unsigned)(k.ntz * k.nty * ntx);
     if (p.arr_ct == 2)
         kern2<<<nblk, TY2 * 16 + 32, C2::SMEM, stream()>>>(p.tm_u, p.tm_v, p.tm_cx, p.tm_cy, p.tm_cz, k);
@@ -1358,20 +1493,22 @@ static int tti_launch_fused_arr(const TtiPlan &p, int slot0, int slotm, int slot
 static bool tti_use_ws(int R) { return R == 4 && env_int_tti("B2_TTI_KERNEL", 3) == 3; }
 template <int R>
 static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount) {
-    const bool ws = tti_use_ws(R);
+    // k_tti_ws is register-bound (DESIGN.md §3.5): with the centre loads of the adjoint it spills, so the adjoint
+    // sweeps with k_tti_fused<4, .., ADJ>, which does not
+    const bool ws = tti_use_ws(R) && !p.adj;
     constexpr int TYF = TtiTile<R>::TY;
     const int TY = ws ? kTtiWsTY : TYF;
     using C = TtiCfg<R, TYF>;
     using CW = TtiWsCfg<kTtiWsTY>;
-    auto kern = k_tti_fused<R, TYF, false, 0>;
+    auto kern = p.adj ? k_tti_fused<R, TYF, false, 0, true> : k_tti_fused<R, TYF, false, 0>;
     static const int pf = env_int_tti("B2_TTI_PF", 1);   // two-deep prefetch spills registers
     auto kern_ws = pf == 1 ? k_tti_ws<kTtiWsTY, 1> : k_tti_ws<kTtiWsTY, 2>;
-    static bool attr_set = false;
-    if (!attr_set) {
+    static bool attr_set[2] = {false, false};
+    if (!attr_set[p.adj]) {
         B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM), B2_ERR_LAUNCH);
         B2_CUDA(cudaFuncSetAttribute(k_tti_ws<kTtiWsTY, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CW::SMEM), B2_ERR_LAUNCH);
         B2_CUDA(cudaFuncSetAttribute(k_tti_ws<kTtiWsTY, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CW::SMEM), B2_ERR_LAUNCH);
-        attr_set = true;
+        attr_set[p.adj] = true;
     }
     TtiFK k;
     k.u1 = p.u + (size_t)slot1 * p.slot_elems;
@@ -1398,7 +1535,9 @@ static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, i
     lx = std::min(lx, xcount);
     k.lx = lx;
     const int ntx = (xcount + lx - 1) / lx;
-    k.slot0 = slot0;
+    k.slot0 = p.adj ? 0 : slot0;
+    k.pc = p.adj ? p.u + (size_t)slot0 * p.slot_elems : nullptr;
+    k.rc = p.adj ? p.v + (size_t)slot0 * p.slot_elems : nullptr;
     k.m_dt2 = (1.0f / (p.vp * p.vp)) * (1.0f / (p.dt * p.dt));
     const float st = sinf(p.theta), ct = cosf(p.theta), sp = sinf(p.phi), cp = cosf(p.phi);
     k.cx = st * cp;
@@ -1418,8 +1557,8 @@ static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, i
         k.p_mdt2 = make_float2(k.m_dt2, k.m_dt2);
     }
     timing_begin();
-    if (ws) note_sweep_kernel("tti_ws<pf%d>", pf == 1 ? 1 : 2);
-    else note_sweep_kernel("tti_fused<%d>", R);
+    if (ws) note_sweep_kernel("tti_ws<pf%d>%s", pf == 1 ? 1 : 2, p.adj ? "+adj" : "");
+    else note_sweep_kernel("tti_fused<%d>%s", R, p.adj ? "+adj" : "");
     if (ws)
         kern_ws<<<(unsigned)(k.ntz * k.nty * ntx), kTtiWsTY * 16 + 128, CW::SMEM, stream()>>>(p.tm_u, p.tm_v, k);
     else
@@ -1439,8 +1578,10 @@ int tti_step(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xco
         return p.R == 2 ? tti_launch_fused<2>(p, slot0, slotm, slot1, xlo, xcount)
                         : tti_launch_fused<4>(p, slot0, slotm, slot1, xlo, xcount);
     TtiK k;
-    k.u0 = p.u + (size_t)slot0 * p.slot_elems;
-    k.v0 = p.v + (size_t)slot0 * p.slot_elems;
+    k.u0 = p.adj ? p.ma : p.u + (size_t)slot0 * p.slot_elems;
+    k.v0 = p.adj ? p.mb : p.v + (size_t)slot0 * p.slot_elems;
+    k.pc = p.u + (size_t)slot0 * p.slot_elems;
+    k.rc = p.v + (size_t)slot0 * p.slot_elems;
     k.um = p.u + (size_t)slotm * p.slot_elems;
     k.vm = p.v + (size_t)slotm * p.slot_elems;
     k.u1 = p.u + (size_t)slot1 * p.slot_elems;
@@ -1471,11 +1612,12 @@ int tti_step(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xco
     dim3 block(64, 4, 1);
     dim3 gridA((k.n2 + k.R + 63) / 64, (k.n1 + k.R + 3) / 4, (unsigned)std::min(xcount + k.R, 65535));
     timing_begin();
-    note_sweep_kernel("tti_two_pass");
+    note_sweep_kernel("tti_two_pass%s", p.adj ? "+adj" : "");
     k_tti_gz<<<gridA, block, 0, stream()>>>(k);
     count_launch();
     dim3 gridB((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(xcount, 65535));
-    k_tti_update<<<gridB, block, 0, stream()>>>(k);
+    if (p.adj) k_tti_update<true><<<gridB, block, 0, stream()>>>(k);
+    else k_tti_update<false><<<gridB, block, 0, stream()>>>(k);
     timing_end();
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);

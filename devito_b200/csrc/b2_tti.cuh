@@ -34,6 +34,11 @@ struct TtiPlan {
     float *tCx = nullptr, *tCy = nullptr, *tCz = nullptr, *tE2 = nullptr, *tSD = nullptr, *tMD = nullptr;
     bool has_arrays = false;
     int tm_rows = 0;             // rows of the u / v tensor-map boxes (fused plans)
+    // adjoint plan (tti_plan_adjoint): the sweep's stencil inputs are the one-slot mixes ma = e2 p + sd r and
+    // mb = sd p + r (library scratch, tm_u / tm_v cover them), combined with (1, 0); u / v stay p / r, whose level
+    // slot0 gives the centre of the update, slotm the previous level and slot1 the level written
+    bool adj = false;
+    float *ma = nullptr, *mb = nullptr;
 };
 
 int tti_plan_init(TtiPlan &p, int kernel);
@@ -48,5 +53,11 @@ int tti_step(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xco
 // `dm` has strides dsx, dsy and its own halo width dmh. Appends "+born_v4" / "+born_s" to the sweep-kernel name.
 int tti_born_source(const TtiPlan &p, const TtiPlan &pd, int slot0, int slotm, int slot1, const float *dm,
                     long long dsx, long long dsy, int dmh);
+// The adjoint plan of p (same sweep variant, tables and A): a copy of p whose tensor maps cover two one-slot scratch
+// buffers, the mixes written by tti_adj_mix.
+int tti_plan_adjoint(const TtiPlan &p, TtiPlan &out);
+// k_tti_adj_mix: the adjoint plan's scratch slots from level slot0 of p / r, over the whole allocated slot (the
+// sweep reads them up to R outside the box). 16 B/point with scalar parameters, 24 with the e2 / sd tables.
+int tti_adj_mix(const TtiPlan &pa, int slot0);
 
 }  // namespace b2

@@ -1,4 +1,5 @@
-// One-point form of the centred-TTI Born source term (k_tti_born_src, b2_tti.cu).
+// One-point forms of the centred-TTI Born source term (k_tti_born_src, b2_tti.cu) and of the adjoint's field mix
+// (k_tti_adj_mix).
 //
 // `__host__ __device__` like b2_iso_point.cuh, so that tests/support/emu_points.cu can loop the SAME body on the
 // CPU and compare it with the float64 reference without a GPU.
@@ -62,6 +63,15 @@ B2_HD void tti_born_point(const TtiBK &k, int x, int y, int z) {
         k.du1[idx] += qu / den;
         k.dv1[idx] += qv / den;
     }
+}
+
+// The reference's adjoint (tti/operators.py `kernel_centered(..., forward=False)`) takes H0 = Gh(e2 p + sd r) and
+// Hz = Gzz(sd p + r) with e2 = 1+2eps and sd = sqrt(1+2delta) sampled at every tap point. k_tti_adj_mix forms the
+// two mixes over the whole slot (halo included), so that the forward sweep with the combination (1, 0) computes
+// H0 and Hz from them.
+B2_HD void tti_adj_mix_point(float e2, float sd, float p, float r, float &a, float &b) {
+    a = fmaf(e2, p, sd * r);
+    b = fmaf(sd, p, r);
 }
 
 }  // namespace b2

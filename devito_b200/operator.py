@@ -292,8 +292,8 @@ class Operator:
             updates.append((f, e))
         if len(injs) > 1 or len(itps) > 1:
             raise _Unrecognised("more than one injection/interpolation")
-        if incs and len(updates) != 1:
-            raise _Unrecognised("increments are only supported next to a single acoustic update")
+        if incs and len(updates) not in (1, 2):
+            raise _Unrecognised("increments are only supported next to a single acoustic update or a TTI pair")
         if len(incs) > 1:
             raise _Unrecognised("more than one increment")
         if fss and (len(updates) != 1 or len(fss) != 1 or fss[0].field is not updates[0][0]):
@@ -312,9 +312,14 @@ class Operator:
             return plan
         if snaps:
             raise _Unrecognised("snapshots are on the fast path next to the single-field acoustic update only")
+        if len(updates) == 2 and (self._dirn != 1 or incs):
+            if any(_space_offsets(e.lhs, None)[0] != -1 for _, e in updates):
+                raise _Unrecognised("the TTI imaging condition needs the backward (adjoint) pair")
+            plan = self._recognise_tti_adjoint(updates, injs, itps)
+            if incs:
+                self._attach_tti_imaging(plan, incs[0])
+            return plan
         if len(updates) == 2:
-            if self._dirn != 1:
-                raise _Unrecognised("adjoint TTI is not on the fast path")
             try:
                 return self._recognise_tti(updates, injs, itps)
             except _Unrecognised as tti_why:
@@ -867,8 +872,80 @@ class Operator:
         plan['grad'] = lhs.function
         plan['usave'] = us.function
 
+    def _attach_tti_imaging(self, plan, inc):
+        """`Inc(dm, -(u0 * p.dt2 + v0 * r.dt2))` next to the adjoint TTI pair = the reference's `GradientTTI`
+        (tti/operators.py `JacobianAdjOperator`): u0, v0 saved forward wavefields read at (time, x, y, z)."""
+        p, r = plan['u'], plan['v']
+        grid = plan['grid']
+        lhs = inc.lhs
+        if not (lhs.is_Access and isinstance(lhs.function, Function) and not lhs.function.is_TimeFunction):
+            raise _Unrecognised("increment target is not a Function")
+        if lhs.function.grid is not grid:
+            raise _Unrecognised("increment target lives on another grid")
+        k = _space_offsets(lhs, None)
+        if k is None or any(k[1]):
+            raise _Unrecognised("increment target accessed off-centre")
+        rhs = inc.rhs.evaluate
+        if self._subs:
+            rhs = rhs.subs(self._subs)
+        try:
+            terms, rest = linear_terms(rhs, lambda a: a.function is p or a.function is r)
+        except NonLinear as e:
+            raise _Unrecognised(f"increment is not linear in the adjoint wavefields: {e}") from None
+        if not (rest.is_Number and float(rest.value) == 0.0):
+            raise _Unrecognised("increment has terms without the adjoint wavefields")
+        keyed = {id(p): {}, id(r): {}}
+        for acc, coef in terms.items():
+            kk = _space_offsets(acc, None)
+            if kk is None or any(kk[1]):
+                raise _Unrecognised("increment reads an adjoint wavefield off-centre")
+            keyed[id(acc.function)][kk[0]] = coef
+        saved = []
+        for f in (p, r):
+            if set(keyed[id(f)]) != {-1, 0, 1}:
+                raise _Unrecognised("increment is not u0 * p.dt2 + v0 * r.dt2 (both fields, second derivative)")
+            funcs, consts, _ = self._leaves(keyed[id(f)].values())
+            sv = [a for a in funcs if getattr(a.function, 'is_TimeFunction', False)]
+            if len(sv) != 1 or len(funcs) != 1 or consts:
+                raise _Unrecognised("each term of the increment must multiply f.dt2 by one saved wavefield")
+            us = sv[0]
+            ku = _space_offsets(us, None)
+            if us.function.is_buffered or ku is None or ku[0] != 0 or any(ku[1]) or \
+                    us.function.space_order != p.space_order or us.function.grid is not grid:
+                raise _Unrecognised("the forward wavefields must be saved (save=nt) and read at (time, x, y, z)")
+            saved.append(us.function)
+        if saved[0] is saved[1]:
+            raise _Unrecognised("the two terms of the increment must use the two saved wavefields")
+        rng = np.random.default_rng(17)
+        dtname = plan['dt'].name
+        for probe in range(2):
+            val = {id(saved[0]): rng.uniform(0.5, 2.0), id(saved[1]): rng.uniform(2.5, 4.0)}
+            dt = rng.uniform(0.5, 2.0)
+
+            def leaf(n):
+                if n.is_Access:
+                    return val[id(n.function)]
+                if n.name == dtname:
+                    return dt
+                raise _Unrecognised(f"unknown symbol {n.name} in the increment")
+            for f, sfn in ((p, saved[0]), (r, saved[1])):
+                c = {t: eval_scalar(e, leaf) for t, e in keyed[id(f)].items()}
+                s_ = val[id(sfn)]
+                want = {-1: -s_ / dt ** 2, 0: 2 * s_ / dt ** 2, 1: -s_ / dt ** 2}
+                for t in want:
+                    if abs(c[t] - want[t]) > 1e-9 * abs(want[t]):
+                        raise _Unrecognised("increment is not -(u0 * p.dt2 + v0 * r.dt2)")
+        plan['grad'] = lhs.function
+        plan['usave'], plan['vsave'] = saved
+
     # -- TTI -------------------------------------------------------------------------------------
-    def _recognise_tti(self, updates, injs, itps):
+    def _recognise_tti_adjoint(self, updates, injs, itps):
+        """The reference's centred-TTI adjoint `AdjointTTI` (tti/operators.py `AdjointOperator`, `kernel_centered(...,
+        forward=False)`): (p.backward, r.backward) from H0 = Gh(e2 p + sd r), Hz = Gzz(sd p + r), e2 and sd sampled at
+        every tap point, with the backward damping; the receivers injected into both fields at the level written."""
+        return self._recognise_tti(updates, injs, itps, adjoint=True)
+
+    def _recognise_tti(self, updates, injs, itps, adjoint=False):
         (u, equ), (v, eqv) = updates
         grid = u.grid
         if grid.dim != 3 or v.grid is not grid:
@@ -953,7 +1030,7 @@ class Operator:
                 if n.name in spv:
                     return spv[n.name]
                 raise _Unrecognised(f"unknown symbol {n.name}")
-            pu, pv = predict_tti(w2, w1, R, P, dval, dt)
+            pu, pv = predict_tti(w2, w1, R, P, dval, dt, adjoint=adjoint)
             for got, pred, nm in ((ku, pu, 'u'), (kv, pv, 'v')):
                 keys = set(got) | set(pred)
                 for k in keys:
@@ -964,7 +1041,7 @@ class Operator:
         m_role = ('vp_f', byname['vp']) if isinstance(byname['vp'], Function) else ('vp_c', byname['vp'])
         plan = {'kind': 'tti', 'u': u, 'v': v, 'grid': grid, 'so': so, 'R': R, 'w2': w2, 'w1': w1,
                 'consts': byname, 'damp': damp, 'dt': dtsym, 'src': None, 'rec': None, 'rec_toff': 0,
-                'm_role': m_role}
+                'm_role': m_role, 'adjoint': adjoint}
         self._attach_sparse(plan, injs, itps, [u, v], funcs, consts, syms, plan['m_role'])
         return plan
 
@@ -1171,6 +1248,8 @@ class Operator:
         else:
             out.extend(p['consts'].values())
         out += [p.get('born_U'), p.get('born_du'), p.get('born_dv'), p.get('born_dm'), p.get('snap')]
+        if p['kind'] == 'tti':
+            out += [p.get('grad'), p.get('usave'), p.get('vsave')]
         out += [s for s in (p['src'], p['rec']) if s is not None]
         return tuple(o for o in out if o is not None)
 
@@ -1363,10 +1442,12 @@ class Operator:
                 raise InvalidArgument("`dm` must be a Function or an array of its allocated shape")
         args['grad'] = self._resolve(kwargs, p.get('grad'), post)
         args['usave'] = self._resolve(kwargs, p.get('usave'), post)
-        if args['usave'] is not None:
-            us = args['usave']
-            if not isinstance(us, TimeFunction) or us.is_buffered or us.space_order != p['so']:
+        args['vsave'] = self._resolve(kwargs, p.get('vsave'), post)
+        for us in (args['usave'], args['vsave']):
+            if us is not None and (not isinstance(us, TimeFunction) or us.is_buffered or us.space_order != p['so']):
                 raise InvalidArgument("the forward wavefield override must be a saved TimeFunction")
+        if p['kind'] == 'tti' and p.get('adjoint') and grid.distributor.is_parallel:
+            raise InvalidArgument("the TTI adjoint does not run on a decomposed grid in this version")
         # parameters
         if p['kind'] == 'iso':
             kind, obj = p['m_role']
@@ -1443,6 +1524,8 @@ class Operator:
         sized += [f for f in fields if not f.is_buffered]
         if args.get('usave') is not None:
             sized.append(args['usave'])
+        if args.get('vsave') is not None:
+            sized.append(args['vsave'])
         time_m = kwargs.pop('time_m', None)
         time_M = kwargs.pop('time_M', kwargs.pop('time', None))
         if time_m is None:
@@ -1896,6 +1979,11 @@ class Operator:
             a.born_du = self._field_obj(args['born_du'], dev, res, hold, written=True).ptr
             a.born_dv = self._field_obj(args['born_dv'], dev, res, hold, written=True).ptr
             a.born_dm = self._field_obj(args['born_dm'], dev, res, hold).ptr
+        a.adjoint = 1 if p.get('adjoint') else 0
+        if args.get('grad') is not None:
+            a.grad = self._field_obj(args['grad'], dev, res, hold, written=True).ptr
+            a.usave = self._field_obj(args['usave'], dev, res, hold).ptr
+            a.vsave = self._field_obj(args['vsave'], dev, res, hold).ptr
         timers = L_.Profiler()
         a.timers = ctypes.pointer(timers)
         t0 = _time.perf_counter()
@@ -1910,9 +1998,10 @@ class Operator:
 # the stencil the TTI kernels implement, as linear coefficients (float64) — used only by the
 # recogniser to confirm that a user's equations are this scheme.
 # ---------------------------------------------------------------------------------------------
-def predict_tti(w2, w1, R, P, damp, dt):
+def predict_tti(w2, w1, R, P, damp, dt, adjoint=False):
     """`P(name, offset)` -> value of parameter `name` sampled `offset` grid points from the output
-    point (constants ignore the offset)."""
+    point (constants ignore the offset). `adjoint`: the backward pair of `kernel_centered(..., forward=False)`,
+    H0 = Gh(e2 p + sd r), Hz = Gzz(sd p + r) with e2, sd sampled at each tap point, the previous level t+1."""
     h = R // 2
     z3 = (0, 0, 0)
 
@@ -1951,18 +2040,32 @@ def predict_tti(w2, w1, R, P, damp, dt):
     m_dt2 = 1.0 / (vp * vp) / (dt * dt)
     den = m_dt2 + damp / dt
     pu, pv = {}, {}
-    for k, val in lap.items():
-        add(pu, ('u', 0) + (k,), e2 * val / den)
-        add(pv, ('u', 0) + (k,), sd * val / den)
-    for k, val in gzz.items():
-        add(pu, ('u', 0) + (k,), -e2 * val / den)
-        add(pu, ('v', 0) + (k,), sd * val / den)
-        add(pv, ('u', 0) + (k,), -sd * val / den)
-        add(pv, ('v', 0) + (k,), val / den)
+    if adjoint:
+        E2 = lambda k: 1 + 2 * P('epsilon', k)
+        SD = lambda k: np.sqrt(1 + 2 * P('delta', k))
+        gh = dict(lap)
+        for k, val in gzz.items():
+            add(gh, k, -val)
+        for k, val in gh.items():              # H0 = Gh(e2 p + sd r)
+            add(pu, ('u', 0) + (k,), E2(k) * val / den)
+            add(pu, ('v', 0) + (k,), SD(k) * val / den)
+        for k, val in gzz.items():             # Hz = Gzz(sd p + r)
+            add(pv, ('u', 0) + (k,), SD(k) * val / den)
+            add(pv, ('v', 0) + (k,), val / den)
+    else:
+        for k, val in lap.items():
+            add(pu, ('u', 0) + (k,), e2 * val / den)
+            add(pv, ('u', 0) + (k,), sd * val / den)
+        for k, val in gzz.items():
+            add(pu, ('u', 0) + (k,), -e2 * val / den)
+            add(pu, ('v', 0) + (k,), sd * val / den)
+            add(pv, ('u', 0) + (k,), -sd * val / den)
+            add(pv, ('v', 0) + (k,), val / den)
+    prev = 1 if adjoint else -1
     add(pu, ('u', 0, z3), (2 * m_dt2 + damp / dt) / den)
-    add(pu, ('u', -1, z3), -m_dt2 / den)
+    add(pu, ('u', prev, z3), -m_dt2 / den)
     add(pv, ('v', 0, z3), (2 * m_dt2 + damp / dt) / den)
-    add(pv, ('v', -1, z3), -m_dt2 / den)
+    add(pv, ('v', prev, z3), -m_dt2 / den)
     pu = {k: v for k, v in pu.items() if abs(v) > 1e-14}
     pv = {k: v for k, v in pv.items() if abs(v) > 1e-14}
     return pu, pv

@@ -197,6 +197,20 @@ struct b2_tti_args {
      * with halo exchange in this version; a missing member of the triple, a shape mismatch or a wrong born_dm
      * extent returns 210.                                                                                 */
     struct b2_dataobj *born_du, *born_dv, *born_dm;
+    /* Adjoint modelling, the reference's `AdjointTTI` operator (tti/operators.py `AdjointOperator`,
+     * `kernel_centered(..., forward=False)`): != 0 -> time runs from time_M down to time_m, (u, v) play (p, r) and
+     * each step writes level time-1 from H0 = Gh(e2 p + sd r), Hz = Gzz(sd p + r) (e2 = 1+2 epsilon,
+     * sd = sqrt(1+2 delta) sampled at every tap point), level time and level time+1 as the previous one; `src` is
+     * injected with dt^2/m into both fields at the level written, `rec` samples p + r at level time. 0 -> the
+     * forward operator. Not combined with halo exchange or the Born triple in this version (210).             */
+    int adjoint;
+    /* The gradient, the reference's `GradientTTI` operator (tti/operators.py `JacobianAdjOperator`): with
+     * `adjoint`, after each step and its injection grad -= usave[time] * p.dt2 + vsave[time] * r.dt2 over the
+     * iterated box. `usave` / `vsave` are saved forward wavefields (nt, x, y, z) with the space layout of u; `grad`
+     * is a space array with its own halo width (hsize), written back when staged. All NULL -> no imaging. grad
+     * without usave and vsave, grad without adjoint, or a saved field whose space layout differs from u's
+     * returns 210.                                                                                          */
+    struct b2_dataobj *grad, *usave, *vsave;
 };
 int b2_tti_forward(const struct b2_tti_args *a);
 
@@ -335,7 +349,8 @@ void   b2_kernel_timing_enable(int on);
  * "iso_generic", "iso_tma<4,vp>", "iso_tma2_v4<6,m>" (template radius, parameter kind scalar|vp|m), "tti_two_pass",
  * "tti_fused<2>", "tti_ws<pf1>", "tti_arr_ct2<4>" (radius); "" if the call launched none. Several kernels are
  * selected at run time (layout checks, B2_* switches): this tells which one computed the answer. A TTI Born call
- * appends the path of its source term: "+born_v4" (float4 along z) or "+born_s" (one point per thread). */
+ * appends the path of its source term: "+born_v4" (float4 along z) or "+born_s" (one point per thread); a TTI
+ * adjoint call appends "+adj" to the variant that ran its sweep. */
 const char *b2_last_sweep_kernel(void);
 /* device memory helpers for hosts that do not use torch */
 void *b2_malloc_device(unsigned long nbytes, int deviceid);
