@@ -112,10 +112,6 @@ struct IsoTK {
     int slot0, slotm;
     float m_dt2;
     float wx[R + 1], wy[R + 1], wz[R + 1];
-    // k_iso_tma2 (two y rows per thread): u[t-1] and the coefficient tables are read straight from global memory
-    // (coalesced 16-byte loads, prefetched into registers), fp32 pair weights {w, w}
-    const float *um, *cA, *cB;
-    float2 p_wx[R + 1], p_wy[R + 1], p_mdt2, p_wc;
     // ---- x-slab decomposition, halo step fused into the sweep (all zero / null on a single device) ----
     // The CTAs that produce a boundary plane also store it into the neighbour GPU's halo through the
     // CUDA-IPC mapped peer pointer (16-byte stores over NVLink), and the producer lane of a CTA that
@@ -390,318 +386,6 @@ k_iso_tma(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUt
 }
 
 
-// ------------------------------------------------------------------------------------------
-// k_iso_tma2: the same 2.5-D sweep with TWO y rows per consumer thread — for the large radii.
-// ------------------------------------------------------------------------------------------
-// k_iso_tma at so=12 (R=6) had to shrink its tile to 16x64 to fit the 13-stage plane ring plus the tile
-// ring, and became shared-memory-bandwidth bound: 12 y-tap LDS.128 per
-// float4 of output. Here
-//   * a thread owns rows 2*tr and 2*tr+1: the 2R rows around them are loaded ONCE for both (7 LDS.128 per
-//     output float4 instead of 12), each own row is the other's nearest y neighbour (registers);
-//   * the tile is 28 x 64 (halo re-reads 1.79x instead of 2.19x): the plane ring holds R+1 live planes + 4 of
-//     prefetch instead of 2R+1, u[t-1] and the coefficient tiles travel by TMA in a 5-stage tile ring (PF = 0,
-//     B2_ISO_V2=4; on an H100 slower than k_iso_tma, which stays the default). The first version read them straight from global memory (LDG.128 prefetched two planes ahead,
-//     PF = 2): correct but slower — with two warps per scheduler the prefetched loads stall on long scoreboard —
-//     kept as B2_ISO_V2=1 for the record;
-//   * the x-history of the own columns is kept in register queues with static slots (planes c+1..c+R in
-//     fut[(p+k) mod R], c-R..c-1 in pst[...], the loop unrolled R times — not 2R+1 = 13 times, which is
-//     what made the first "taller tile" experiment of round 1 miss the instruction cache);
-//   * y/x taps and the update written as fp32 pair operations (b2_ptx.cuh).
-// Halo step under decomposition: identical to k_iso_tma (peer stores, flag acquire, chunk 0 backwards).
-template <int R, int TY, int TZ4, int PF = 2, int NT = 2>
-struct IsoTma2Cfg {
-    static constexpr int RZ = ceil4(R);
-    static constexpr int TZ = 4 * TZ4;
-    static constexpr int BY = TY + 2 * R;
-    static constexpr int BZ = TZ + 2 * RZ;
-    // PF == 0: u[t-1] and the coefficient tiles travel by TMA with the planes (like k_iso_tma): the plane ring is
-    // R+1 live planes + 4 of prefetch, the tile ring 5 stages
-    static constexpr int NU = PF == 0 ? R + 5 : 2 * R + 1;
-    static constexpr int NS = PF == 0 ? 5 : 0;
-    static constexpr int PLANE = align32f(BY * BZ);
-    static constexpr int TILE = TY * TZ;
-    static constexpr int NCT = (TY / 2) * TZ4;          // consumer threads
-    static constexpr int NCW = NCT / 32;
-    static constexpr size_t SMEM = (size_t)(NU * PLANE + NS * NT * TILE) * 4 + 2 * NU * 8 + 128;
-};
-
-template <int R, int TY, int TZ4, int PK, int PF>
-__global__ void __launch_bounds__((TY / 2) * TZ4 + 32, 1)
-k_iso_tma2(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUtensorMap tm_uc,
-           const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, const IsoTK<R> k) {
-    constexpr int NT = PK != B2_PARAM_SCALAR ? 3 : 2;
-    using C = IsoTma2Cfg<R, TY, TZ4, PF, NT>;
-    using b2ptx::F4;
-    constexpr int RZ = C::RZ, TZ = C::TZ, BZ = C::BZ, NU = C::NU, PLANE = C::PLANE, NCW = C::NCW;
-    constexpr int NS = C::NS, TILE = C::TILE;
-    static_assert(TY % 2 == 0 && C::NCT % 32 == 0, "two rows per thread, whole warps");
-    static_assert(R % 2 == 0, "the prefetch buffers alternate with the parity of the unrolled iteration");
-
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    float *s_u = reinterpret_cast<float *>(smem_raw);
-    float *s_t = s_u + NU * PLANE;                       // tile ring (PF == 0): [stage][prev, A, (B)][TILE]
-    uint64_t *full = reinterpret_cast<uint64_t *>(s_t + NS * NT * TILE);
-    uint64_t *empty = full + NU;
-
-    int b = blockIdx.x;
-    const int iz = b % k.ntz;
-    b /= k.ntz;
-    const int iy = b % k.nty;
-    const int ix = b / k.nty;
-    const int z0 = iz * TZ, y0 = iy * TY;
-    const int xs = k.xlo + ix * k.lx;
-    const int xe = min(xs + k.lx, k.xlo + k.xcount);
-    const int NP = (xe - xs) + 2 * R;
-    const bool back = (ix == 0) && k.back0;
-    const int dx = back ? -1 : 1;
-    const int xb = back ? xe - 1 + R : xs - R;
-
-    const int tid = threadIdx.x;
-    const int warp = tid >> 5, lane = tid & 31;
-    if (tid == 0) {
-        for (int i = 0; i < NU; ++i) {
-            b2ptx::mbar_init(&full[i], 1);
-            b2ptx::mbar_init(&empty[i], NCW);
-        }
-        b2ptx::fence_mbar_init();
-    }
-    __syncthreads();
-
-    if (warp == NCW) {
-        if (lane == 0) {
-            b2ptx::tma_prefetch_desc(&tm_uh);
-            int slot = 0, round = 0, ss = 0;
-            bool need_lo = k.want >= 0 && k.flag_lo != nullptr, need_hi = k.want >= 0 && k.flag_hi != nullptr;
-            for (int j = 0; j < NP; ++j) {
-                if (round > 0) b2ptx::mbar_wait(&empty[slot], (round - 1) & 1);
-                const int xj = xb + dx * j;
-                if (need_lo && xj < 0) {
-                    while (b2ptx::ld_acquire_sys(k.flag_lo) < k.want) __nanosleep(40);
-                    b2ptx::fence_proxy_async_global();
-                    need_lo = false;
-                }
-                if (need_hi && xj >= k.nown) {
-                    while (b2ptx::ld_acquire_sys(k.flag_hi) < k.want) __nanosleep(40);
-                    b2ptx::fence_proxy_async_global();
-                    need_hi = false;
-                }
-                const bool tiles = PF == 0 && j >= 2 * R;
-                b2ptx::mbar_arrive_expect_tx(&full[slot], (uint32_t)(C::BY * BZ * 4) + (tiles ? (uint32_t)(TILE * 4 * NT) : 0u));
-                b2ptx::tma_load_4d(s_u + slot * PLANE, &tm_uh, &full[slot], k.oz + z0 - RZ, k.oy + y0 - R,
-                                   k.ox + xj, k.slot0);
-                if (tiles) {
-                    // the tiles of the output plane of iteration j travel with plane j
-                    const int xo = xj - dx * R;
-                    float *t = s_t + ss * NT * TILE;
-                    b2ptx::tma_load_4d(t, &tm_uc, &full[slot], k.oz + z0, k.oy + y0, k.ox + xo, k.slotm);
-                    b2ptx::tma_load_3d(t + TILE, &tm_a, &full[slot], k.oz + z0, k.oy + y0, k.ox + xo);
-                    if (PK != B2_PARAM_SCALAR)
-                        b2ptx::tma_load_3d(t + 2 * TILE, &tm_b, &full[slot], k.oz + z0, k.oy + y0, k.ox + xo);
-                    if (++ss == NS) ss = 0;
-                }
-                if (++slot == NU) { slot = 0; ++round; }
-            }
-        }
-        return;
-    }
-
-    // ---------------- consumers: rows (2 tr, 2 tr + 1), four z points ----------------
-    const int tr = tid / TZ4, tz4 = tid % TZ4;
-    const int gz = z0 + 4 * tz4;
-    const int gy0 = y0 + 2 * tr;
-    int zc[2];
-    long long row[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-        zc[r] = (gy0 + r < k.ny) ? min(max(k.nz - gz, 0), 4) : 0;
-        row[r] = (long long)(k.oy + gy0 + r) * k.sy + (k.oz + gz);
-    }
-    const int col = (2 * tr + R) * BZ + RZ + 4 * tz4;      // row 0 of this thread inside a shared plane
-    const long long osx = dx * k.sx;
-    const long long gbase = (long long)(k.ox + xb - dx * R) * k.sx;   // + j * osx = the output plane of iteration j
-    const bool fuse = (k.peer_lo != nullptr) | (k.peer_hi != nullptr);
-
-    F4 fut[2][R], pst[2][R], cen[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-        cen[r] = b2ptx::f4zero();
-#pragma unroll
-        for (int i = 0; i < R; ++i) { fut[r][i] = b2ptx::f4zero(); pst[r][i] = b2ptx::f4zero(); }
-    }
-    // u[t-1], A (and B) of the output plane of iteration j, loaded two iterations ahead
-    constexpr int PFB = PF > 0 ? PF : 1;
-    float4 pv[2][PFB], pa[2][PFB], pb[2][PFB];
-#pragma unroll
-    for (int r = 0; r < 2; ++r)
-#pragma unroll
-        for (int d = 0; d < PFB; ++d) { pv[r][d] = pa[r][d] = pb[r][d] = make_float4(0.f, 0.f, 0.f, 0.f); }
-    int ts_off = 0;                                       // tile-ring stage of the current output plane (PF == 0)
-    const int tcol = (2 * tr) * TZ + 4 * tz4;
-    auto prefetch = [&](int j, int d) {
-        // output plane of iteration j: x = xb + dx * (j - R), valid for 2R <= j < NP
-        if (j < 2 * R || j >= NP) return;
-        const long long g = gbase + (long long)j * osx;
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            if (zc[r] > 0) {
-                pv[r][d] = *reinterpret_cast<const float4 *>(k.um + g + row[r]);
-                pa[r][d] = *reinterpret_cast<const float4 *>(k.cA + g + row[r]);
-                if (PK != B2_PARAM_SCALAR) pb[r][d] = *reinterpret_cast<const float4 *>(k.cB + g + row[r]);
-            }
-        }
-    };
-    if (PF >= 1) prefetch(2 * R, 0);
-    if (PF == 2) prefetch(2 * R + 1, PF - 1);
-
-    int st_new = 0, st_cen = 0;           // shared-memory stage of plane j and of the centre plane j - R
-    uint32_t par_new = 0;
-
-    for (int jb = 0; jb < NP; jb += R) {
-#pragma unroll
-        for (int p = 0; p < R; ++p) {
-            const int j = jb + p;
-            if (j >= NP) break;
-            // slot of plane c + kk (c = j - R, c mod R == p): compile-time
-#define B2_SLOT(kk) ((((p) + (kk)) % R + R) % R)
-            b2ptx::mbar_wait(&full[st_new], par_new);
-            {
-                const float *np_ = s_u + st_new * PLANE + col;
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    pst[r][B2_SLOT(-1)] = cen[r];                        // plane c-1 (overwrites plane c-1-R)
-                    cen[r] = fut[r][p];                                  // plane c
-                    fut[r][p] = b2ptx::f4pack(b2ptx::lds128(np_ + r * BZ));   // plane c+R = j
-                }
-            }
-            if (j >= 2 * R) {
-                const float *cp0 = s_u + st_cen * PLANE + col;
-                F4 acc[2];
-                // z direction (scalar: the operands straddle register pairs)
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    const float *cp = cp0 + r * BZ;
-                    const float4 c = b2ptx::f4unpack(cen[r]);
-                    float zr[4 + 2 * RZ];
-#pragma unroll
-                    for (int m = 0; m < RZ / 4; ++m) {
-                        if (R % 4 == 2 && m == 0) {
-                            const float2 l = *reinterpret_cast<const float2 *>(cp - RZ + 2);
-                            zr[0] = 0.f; zr[1] = 0.f; zr[2] = l.x; zr[3] = l.y;
-                        } else {
-                            const float4 l = b2ptx::lds128(cp - RZ + 4 * m);
-                            zr[4 * m + 0] = l.x; zr[4 * m + 1] = l.y; zr[4 * m + 2] = l.z; zr[4 * m + 3] = l.w;
-                        }
-                        if (R % 4 == 2 && m == RZ / 4 - 1) {
-                            const float2 q = *reinterpret_cast<const float2 *>(cp + 4 + 4 * m);
-                            zr[RZ + 4 + 4 * m + 0] = q.x; zr[RZ + 4 + 4 * m + 1] = q.y;
-                            zr[RZ + 4 + 4 * m + 2] = 0.f; zr[RZ + 4 + 4 * m + 3] = 0.f;
-                        } else {
-                            const float4 q = b2ptx::lds128(cp + 4 + 4 * m);
-                            zr[RZ + 4 + 4 * m + 0] = q.x; zr[RZ + 4 + 4 * m + 1] = q.y;
-                            zr[RZ + 4 + 4 * m + 2] = q.z; zr[RZ + 4 + 4 * m + 3] = q.w;
-                        }
-                    }
-                    zr[RZ + 0] = c.x; zr[RZ + 1] = c.y; zr[RZ + 2] = c.z; zr[RZ + 3] = c.w;
-                    const float wc = k.p_wc.x;
-                    float4 a = make_float4(wc * c.x, wc * c.y, wc * c.z, wc * c.w);
-#pragma unroll
-                    for (int i = 1; i <= R; ++i) {
-                        a.x = fmaf(k.wz[i], zr[RZ + 0 - i] + zr[RZ + 0 + i], a.x);
-                        a.y = fmaf(k.wz[i], zr[RZ + 1 - i] + zr[RZ + 1 + i], a.y);
-                        a.z = fmaf(k.wz[i], zr[RZ + 2 - i] + zr[RZ + 2 + i], a.z);
-                        a.w = fmaf(k.wz[i], zr[RZ + 3 - i] + zr[RZ + 3 + i], a.w);
-                    }
-                    acc[r] = b2ptx::f4pack(a);
-                }
-                // y direction: rows -R..-1 and +2..R+1 (relative to row 0) are loaded once for both rows;
-                // each own row is the other's +-1 neighbour (registers)
-                b2ptx::f4fma2(acc[0], k.p_wy[1], cen[1]);
-                b2ptx::f4fma2(acc[1], k.p_wy[1], cen[0]);
-#pragma unroll
-                for (int d = -R; d <= R + 1; ++d) {
-                    if (d == 0 || d == 1) continue;
-                    const F4 v = b2ptx::f4pack(b2ptx::lds128(cp0 + d * BZ));
-                    const int a0 = d < 0 ? -d : d, a1 = d - 1 < 0 ? 1 - d : d - 1;
-                    if (a0 <= R) b2ptx::f4fma2(acc[0], k.p_wy[a0], v);
-                    if (a1 <= R) b2ptx::f4fma2(acc[1], k.p_wy[a1], v);
-                }
-                // x direction: own columns, register queues
-#pragma unroll
-                for (int r = 0; r < 2; ++r)
-#pragma unroll
-                    for (int i = 1; i <= R; ++i)
-                        b2ptx::f4fma2(acc[r], k.p_wx[i], b2ptx::f4add2(pst[r][B2_SLOT(-i)], fut[r][B2_SLOT(i)]));
-                // update  u+ = u + A (m/dt^2 (u - u-) + lap)   |   u + B (u - u-) + A lap
-                // compile-time buffer index (jb and 2R are even): a run-time index into a register array makes the
-                // compiler select/copy right after the load, i.e. wait for it — the first version stalled on exactly that
-                const int d = PF == 2 ? (p & 1) : 0;
-                const long long g = gbase + (long long)j * osx;
-                if (PF == 0) {
-#pragma unroll
-                    for (int r = 0; r < 2; ++r) {
-                        const float *t = s_t + ts_off + tcol + r * TZ;
-                        pv[r][0] = b2ptx::lds128(t);
-                        pa[r][0] = b2ptx::lds128(t + TILE);
-                        if (PK != B2_PARAM_SCALAR) pb[r][0] = b2ptx::lds128(t + 2 * TILE);
-                    }
-                    ts_off += NT * TILE;
-                    if (ts_off == NS * NT * TILE) ts_off = 0;
-                }
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    const F4 c = cen[r];
-                    const F4 dcp = b2ptx::f4sub2(c, b2ptx::f4pack(pv[r][d]));
-                    const F4 ca = b2ptx::f4pack(pa[r][d]);
-                    F4 o;
-                    if (PK == B2_PARAM_SCALAR) {
-                        F4 t = acc[r];
-                        b2ptx::f4fma2(t, k.p_mdt2, dcp);
-                        o = F4{b2ptx::fma2(ca.a, t.a, c.a), b2ptx::fma2(ca.b, t.b, c.b)};
-                    } else {
-                        const F4 cb = b2ptx::f4pack(pb[r][d]);
-                        const F4 t = F4{b2ptx::fma2(cb.a, dcp.a, c.a), b2ptx::fma2(cb.b, dcp.b, c.b)};
-                        o = F4{b2ptx::fma2(ca.a, acc[r].a, t.a), b2ptx::fma2(ca.b, acc[r].b, t.b)};
-                    }
-                    const float4 of = b2ptx::f4unpack(o);
-                    float *dst = k.u1 + g + row[r];
-                    if (zc[r] == 4) {
-                        *reinterpret_cast<float4 *>(dst) = of;
-                    } else if (zc[r] > 0) {
-                        dst[0] = of.x;
-                        if (zc[r] > 1) dst[1] = of.y;
-                        if (zc[r] > 2) dst[2] = of.z;
-                    }
-                    if (fuse) {
-                        const int xo = xb + dx * (j - R);
-                        float *pd = nullptr;
-                        const long long ro = row[r] - (long long)0;
-                        if (k.peer_lo && xo < k.pw) pd = k.peer_lo + (k.off_lo + (long long)xo * k.sx + ro);
-                        if (k.peer_hi && xo >= k.nown - k.pw) pd = k.peer_hi + (k.off_hi + (long long)xo * k.sx + ro);
-                        if (pd) {
-                            if (zc[r] == 4) {
-                                *reinterpret_cast<float4 *>(pd) = of;
-                            } else if (zc[r] > 0) {
-                                pd[0] = of.x;
-                                if (zc[r] > 1) pd[1] = of.y;
-                                if (zc[r] > 2) pd[2] = of.z;
-                            }
-                        }
-                    }
-                }
-                if (PF == 2) prefetch(j + 2, d);
-            }
-            if (PF == 1 && j + 1 >= 2 * R) prefetch(j + 1, 0);    // (after the stores of this plane were issued)
-            if (j >= R) {
-                __syncwarp();
-                if (lane == 0) b2ptx::mbar_arrive(&empty[st_cen]);
-                if (++st_cen == NU) st_cen = 0;
-            }
-            if (++st_new == NU) { st_new = 0; par_new ^= 1; }
-#undef B2_SLOT
-        }
-    }
-}
-
 // A = 1/(m/dt^2 + damp/dt), B = m/dt^2 * A on the full allocated array (halo included; halo
 // values are never used by the stencil)
 __global__ void __launch_bounds__(256)
@@ -780,16 +464,6 @@ template <> struct TileOf<4, false> { static constexpr int TY = 16, TZ4 = 32; };
 template <> struct TileOf<4, true> { static constexpr int TY = 32, TZ4 = 16; };
 template <bool ARR> struct TileOf<6, ARR> { static constexpr int TY = 16, TZ4 = 16; };
 template <bool ARR> struct TileOf<8, ARR> { static constexpr int TY = 8, TZ4 = 16; };
-
-// k_iso_tma2 (two rows per thread, no tile ring): the radii whose k_iso_tma tile had to shrink
-template <int R> struct Tile2Of { static constexpr bool on = false; static constexpr int TY = 32, TZ4 = 16; };
-// 28 x 64: 14 x 16 = 224 consumer threads + the producer warp = 8 warps, so that the register file splits
-// into 255 registers per thread (9 warps would be allocated as 12: 168 registers, and the queues spill)
-template <> struct Tile2Of<6> { static constexpr bool on = true; static constexpr int TY = 28, TZ4 = 16; };
-
-// opt-in dynamic shared memory per block on sm_90 (227 KB)
-constexpr size_t kSmemPerBlockMax = 232448;
-
 
 static int env_int(const char *name, int dflt) {
     const char *v = getenv(name);
@@ -881,31 +555,6 @@ static int plan_tma(IsoPlan &p) {
     const int dims4[4] = {p.a[2], p.a[1], p.a[0], p.tsize};
     const int dims3[3] = {p.a[2], p.a[1], p.a[0]};
     int rc;
-    // so=12 on an H100: the one-row k_iso_tma (default 0) is faster than variant 4 of k_iso_tma2 (DESIGN §5b)
-    p.v2 = Tile2Of<R>::on && p.n[1] >= 16 ? env_int("B2_ISO_V2", 0) : 0;
-    // only variants 1 and 4 exist: any other value would build the two-row tensor maps below and then launch the
-    // one-row kernel over them
-    if (p.v2 != 1 && p.v2 != 4) p.v2 = 0;
-    if (p.v2) {
-        using T2 = Tile2Of<R>;
-        // variant 4 with an array parameter rings three coefficient tiles: more shared memory than a block may have
-        constexpr size_t smem4 = IsoTma2Cfg<R, T2::TY, T2::TZ4, 0, 3>::SMEM;
-        if (p.v2 == 4 && p.param_kind != B2_PARAM_SCALAR && smem4 > kSmemPerBlockMax) {
-            set_error("iso: B2_ISO_V2=4 with an array-valued vp/m needs %zu bytes of shared memory per block (the "
-                      "device allows %zu); use B2_ISO_V2=0 (the default) or 1", smem4, kSmemPerBlockMax);
-            return B2_ERR_INVALID;
-        }
-        if ((rc = make_tmap(&p.tm_uh, p.u, 4, dims4, 4 * T2::TZ4 + 2 * RZ, T2::TY + 2 * R))) return rc;
-        // variant 4: u[t-1] and the coefficient tiles by TMA (28 x 64 tiles)
-        if ((rc = make_tmap(&p.tm_uc, p.u, 4, dims4, 4 * T2::TZ4, T2::TY))) return rc;
-        if ((rc = make_tmap(&p.tm_damp, p.coefA, 3, dims3, 4 * T2::TZ4, T2::TY))) return rc;
-        if (p.param_kind != B2_PARAM_SCALAR) {
-            if ((rc = make_tmap(&p.tm_par, p.coefB, 3, dims3, 4 * T2::TZ4, T2::TY))) return rc;
-        } else {
-            p.tm_par = p.tm_damp;
-        }
-        return B2_OK;
-    }
     if ((rc = make_tmap(&p.tm_uh, p.u, 4, dims4, 4 * TZ4 + 2 * RZ, TY + 2 * R))) return rc;
     if ((rc = make_tmap(&p.tm_uc, p.u, 4, dims4, 4 * TZ4, TY))) return rc;
     if ((rc = make_tmap(&p.tm_damp, p.coefA, 3, dims3, 4 * TZ4, TY))) return rc;
@@ -963,33 +612,15 @@ template <int R, int PK>
 static int launch_tma(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount,
                       const IsoFuse *fz = nullptr) {
     using T = TileOf<R, PK != B2_PARAM_SCALAR>;
-    using T2 = Tile2Of<R>;
     using C = IsoTmaCfg<R, T::TY, T::TZ4, PK>;
-    using C2 = IsoTma2Cfg<R, T2::TY, T2::TZ4>;
     auto kern = k_iso_tma<R, T::TY, T::TZ4, PK>;
-    // the shared-memory size is opted into per kernel, before its first launch: a variant that cannot run (variant 4
-    // with an array parameter, refused by plan_tma) must not make the others fail
-    static bool attr_set[3] = {false, false, false};      // k_iso_tma, k_iso_tma2 variant 1, variant 4
-    const int v2 = T2::on ? p.v2 : 0;           // 4: TMA tile ring, 1: LDG prefetch (experiment), 0: k_iso_tma
-    if (v2 == 0 && !attr_set[0]) {
+    // the shared-memory size is opted into once, before the kernel's first launch
+    static bool attr_set = false;
+    if (!attr_set) {
         B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM),
                 B2_ERR_LAUNCH);
-        attr_set[0] = true;
+        attr_set = true;
     }
-    if constexpr (T2::on) {
-        if (v2 == 1 && !attr_set[1]) {
-            B2_CUDA(cudaFuncSetAttribute(k_iso_tma2<R, T2::TY, T2::TZ4, PK, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)C2::SMEM), B2_ERR_LAUNCH);
-            attr_set[1] = true;
-        }
-        using C2t = IsoTma2Cfg<R, T2::TY, T2::TZ4, 0, (PK != B2_PARAM_SCALAR ? 3 : 2)>;
-        if (v2 == 4 && !attr_set[2]) {
-            B2_CUDA(cudaFuncSetAttribute(k_iso_tma2<R, T2::TY, T2::TZ4, PK, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)C2t::SMEM), B2_ERR_LAUNCH);
-            attr_set[2] = true;
-        }
-    }
-    const int TYeff = v2 ? T2::TY : T::TY;
     IsoTK<R> k;
     k.u1 = p.u + (size_t)slot1 * p.slot_elems;
     k.sx = p.sx;
@@ -1002,7 +633,7 @@ static int launch_tma(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo
     k.xlo = xlo;
     k.xcount = xcount;
     k.ntz = (p.n[2] + C::TZ - 1) / C::TZ;
-    k.nty = (p.n[1] + TYeff - 1) / TYeff;
+    k.nty = (p.n[1] + T::TY - 1) / T::TY;
     // x-chunk length: whole waves over the SMs, but chunks of at least 32 planes
     int lx = env_int("B2_ISO_LX", 0);
     if (lx <= 0) {
@@ -1040,33 +671,12 @@ static int launch_tma(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo
         k.wx[i] = p.w[0][i];
         k.wy[i] = p.w[1][i];
         k.wz[i] = p.w[2][i];
-        k.p_wx[i] = make_float2(k.wx[i], k.wx[i]);
-        k.p_wy[i] = make_float2(k.wy[i], k.wy[i]);
     }
-    k.p_mdt2 = make_float2(k.m_dt2, k.m_dt2);
-    {
-        const float wc = k.wx[0] + k.wy[0] + k.wz[0];
-        k.p_wc = make_float2(wc, wc);
-    }
-    k.um = p.u + (size_t)slotm * p.slot_elems;
-    k.cA = p.coefA;
-    k.cB = p.coefB;
     const unsigned grid = (unsigned)(k.ntz * k.nty * ntx);
     const char *pk = PK == B2_PARAM_VP ? "vp" : (PK == B2_PARAM_M ? "m" : "scalar");
     timing_begin();
-    bool launched = false;
-    if constexpr (T2::on) {
-        using C2t = IsoTma2Cfg<R, T2::TY, T2::TZ4, 0, (PK != B2_PARAM_SCALAR ? 3 : 2)>;
-        const unsigned nth = (T2::TY / 2) * T2::TZ4 + 32;
-        if (v2 == 1) k_iso_tma2<R, T2::TY, T2::TZ4, PK, 2><<<grid, nth, C2::SMEM, stream()>>>(p.tm_uh, p.tm_uc, p.tm_damp, p.tm_par, k);
-        if (v2 == 4) k_iso_tma2<R, T2::TY, T2::TZ4, PK, 0><<<grid, nth, C2t::SMEM, stream()>>>(p.tm_uh, p.tm_uc, p.tm_damp, p.tm_par, k);
-        launched = v2 == 1 || v2 == 4;
-        if (launched) note_sweep_kernel("iso_tma2_v%d<%d,%s>", v2, R, pk);
-    }
-    if (!launched) {
-        kern<<<grid, T::TY * T::TZ4 + 32, C::SMEM, stream()>>>(p.tm_uh, p.tm_uc, p.tm_damp, p.tm_par, k);
-        note_sweep_kernel("iso_tma<%d,%s>", R, pk);
-    }
+    kern<<<grid, T::TY * T::TZ4 + 32, C::SMEM, stream()>>>(p.tm_uh, p.tm_uc, p.tm_damp, p.tm_par, k);
+    note_sweep_kernel("iso_tma<%d,%s>", R, pk);
     timing_end();
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);

@@ -22,7 +22,6 @@ struct IsoPlan {
     float w[3][B2_MAX_RADIUS + 1] = {};
     // TMA path
     bool use_tma = false;
-    int v2 = 0;                  // k_iso_tma2 variant (two rows per thread; radius 6), 0 = k_iso_tma
     CUtensorMap tm_uh, tm_uc, tm_damp, tm_par;   // tm_damp/tm_par map coefA/coefB
     float *coefA = nullptr, *coefB = nullptr;    // tabulated update coefficients (library scratch)
     bool defer_coef = false;                     // plan init only allocates them (streamed loop: per chunk)

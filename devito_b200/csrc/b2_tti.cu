@@ -724,7 +724,7 @@ struct TtiWsCfg {
     static constexpr size_t SMEM = (size_t)((NUU + NUV) * PLANE + 2 * NG * GPLANE) * 4 + 2 * NB * 8 + 128;
 };
 
-template <int TY, int PF>
+template <int TY>
 __global__ void __launch_bounds__(TY * 16 + 128, 1)
 k_tti_ws(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_v, const TtiFK k) {
     using C = TtiWsCfg<TY>;
@@ -888,7 +888,6 @@ k_tti_ws(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUten
     int iu = ((xs - PRE) % NUU + NUU) % NUU, iv = ((xs - PRE) % NUV + NUV) % NUV,
         ig = ((xs - PRE) % NG + NG) % NG;
     float4 nu = zero4, nv = zero4, na = zero4;      // prefetched u[t-1], v[t-1], A of plane x+1
-    float4 mu = zero4, mv = zero4, ma = zero4;      // ... and of plane x+2
 
     for (int itb = 0; itb < NIT; itb += 4) {
 #pragma unroll
@@ -952,18 +951,9 @@ k_tti_ws(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUten
         // u[t-1], v[t-1], A: loaded one full iteration before they are used (the registers are
         // there: the main warpgroups own 152 each after setmaxnreg)
         const float4 pu = nu, pv = nv, pa = na;
-        if (PF == 2) {
-            nu = mu; nv = mv; na = ma;
-            // two-deep register prefetch; full 16-byte loads even on overhanging tiles (the row's
-            // halo makes them safe, stores are masked)
-            const long long gn = gi + 2 * k.sx;             // plane x + 2
-            if (x + 2 >= xs && x + 2 < xe && zcnt > 0) {
-                mu = *reinterpret_cast<const float4 *>(k.um + gn);
-                mv = *reinterpret_cast<const float4 *>(k.vm + gn);
-                ma = *reinterpret_cast<const float4 *>(k.A + gn);
-            }
-        } else {
-            // one-deep: 12 registers less (the 4x unrolled body with static queue slots is register-bound)
+        {
+            // one plane deep: a second plane would cost 12 registers, and the 4x unrolled body with static
+            // queue slots is register-bound
             const long long gn = gi + k.sx;                 // plane x + 1
             if (x + 1 >= xs && x + 1 < xe && zcnt > 0) {
                 nu = *reinterpret_cast<const float4 *>(k.um + gn);
@@ -1501,13 +1491,11 @@ static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, i
     using C = TtiCfg<R, TYF>;
     using CW = TtiWsCfg<kTtiWsTY>;
     auto kern = p.adj ? k_tti_fused<R, TYF, false, 0, true> : k_tti_fused<R, TYF, false, 0>;
-    static const int pf = env_int_tti("B2_TTI_PF", 1);   // two-deep prefetch spills registers
-    auto kern_ws = pf == 1 ? k_tti_ws<kTtiWsTY, 1> : k_tti_ws<kTtiWsTY, 2>;
+    auto kern_ws = k_tti_ws<kTtiWsTY>;
     static bool attr_set[2] = {false, false};
     if (!attr_set[p.adj]) {
         B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM), B2_ERR_LAUNCH);
-        B2_CUDA(cudaFuncSetAttribute(k_tti_ws<kTtiWsTY, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CW::SMEM), B2_ERR_LAUNCH);
-        B2_CUDA(cudaFuncSetAttribute(k_tti_ws<kTtiWsTY, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CW::SMEM), B2_ERR_LAUNCH);
+        B2_CUDA(cudaFuncSetAttribute(kern_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CW::SMEM), B2_ERR_LAUNCH);
         attr_set[p.adj] = true;
     }
     TtiFK k;
@@ -1557,7 +1545,7 @@ static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, i
         k.p_mdt2 = make_float2(k.m_dt2, k.m_dt2);
     }
     timing_begin();
-    if (ws) note_sweep_kernel("tti_ws<pf%d>%s", pf == 1 ? 1 : 2, p.adj ? "+adj" : "");
+    if (ws) note_sweep_kernel("tti_ws<pf1>");
     else note_sweep_kernel("tti_fused<%d>%s", R, p.adj ? "+adj" : "");
     if (ws)
         kern_ws<<<(unsigned)(k.ntz * k.nty * ntx), kTtiWsTY * 16 + 128, CW::SMEM, stream()>>>(p.tm_u, p.tm_v, k);

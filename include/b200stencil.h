@@ -346,7 +346,7 @@ void   b2_kernel_timing_reset(void);
 double b2_kernel_timing_ms(int *nlaunches);
 void   b2_kernel_timing_enable(int on);
 /* name of the sweep kernel variant the last b2_iso_forward / b2_tti_forward call on this process launched, e.g.
- * "iso_generic", "iso_tma<4,vp>", "iso_tma2_v4<6,m>" (template radius, parameter kind scalar|vp|m), "tti_two_pass",
+ * "iso_generic", "iso_tma<4,vp>" (template radius, parameter kind scalar|vp|m), "tti_two_pass",
  * "tti_fused<2>", "tti_ws<pf1>", "tti_arr_ct2<4>" (radius); "" if the call launched none. Several kernels are
  * selected at run time (layout checks, B2_* switches): this tells which one computed the answer. A TTI Born call
  * appends the path of its source term: "+born_v4" (float4 along z) or "+born_s" (one point per thread); a TTI

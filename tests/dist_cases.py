@@ -39,7 +39,7 @@ def run_case(kind, nranks, topology=None):
                              **({'topology': topology} if topology is not None else {}))
         out = AnisotropicWaveSolver(model, setup_geometry(model, TN), space_order=SO).forward()
         return {'rec': out[0].data, 'u': out[1].data, 'v': out[2].data}, model
-    if kind == 'iso12':                                    # so=12: the two-row sweep kernel with the fused halo step
+    if kind == 'iso12':                                    # so=12: the one-row sweep kernel with the fused halo step
         kw12 = dict(kw, space_order=12, nbl=14)
         model = demo_model('constant-isotropic', **kw12)
         rec, u, _ = AcousticWaveSolver(model, setup_geometry(model, TN), space_order=12).forward()

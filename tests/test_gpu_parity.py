@@ -191,29 +191,6 @@ def test_streamed_time_loop_array_velocity(monkeypatch):
     assert rel_linf(rec.data, g['rec']) < 1e-5
 
 
-@pytest.mark.parametrize('preset,n', [('constant-isotropic', 50), ('layers-isotropic', 41)])
-def test_so12_two_row_kernel_matches_the_one_row_kernel(preset, n, monkeypatch):
-    """`k_iso_tma2` (so=12: two y rows per thread, u[t-1]/coefficients in a TMA tile ring, fp32 pair
-    arithmetic) against `k_iso_tma` on the same inputs — tile-overhanging extents (n + 2 nbl is not a
-    multiple of the 28-row tile), scalar and array velocity — and against the oracle."""
-    from devito_b200.seismic import demo_model, setup_geometry, AcousticWaveSolver
-    so, nbl, tn = 12, 14, 120.0
-    kw = dict(nlayers=3) if preset.startswith('layers') else {}
-    model = demo_model(preset, spacing=(10., 10., 10.), shape=(n, n, n - 2), nbl=nbl, space_order=so, **kw)
-    geometry = setup_geometry(model, tn)
-    solver = AcousticWaveSolver(model, geometry, space_order=so)
-    monkeypatch.setenv('B2_ISO_V2', '4')                   # the two-row kernel (variant 4)
-    rec2, u2, _ = solver.forward()
-    monkeypatch.setenv('B2_ISO_V2', '0')                   # the one-row kernel (the default)
-    solver1 = AcousticWaveSolver(model, geometry, space_order=so)
-    rec1, u1, _ = solver1.forward()
-    assert rel_linf(u2.data, u1.data) < 2e-6               # same operations, other summation order in y
-    assert rel_linf(rec2.data, rec1.data) < 2e-6
-    # generic kernel (one thread per point, the reference's formula with the division) as third opinion
-    rec0, u0, _ = solver1.forward(kernel=1)
-    assert rel_linf(u2.data, u0.data) < 1e-5
-
-
 def test_restart_on_time_subranges():
     """Second caller of the C ABI in the reference (checkpointing/checkpoint.py:30-46): the loop
     must be restartable on arbitrary [time_m, time_M] sub-ranges."""

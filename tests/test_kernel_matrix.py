@@ -7,11 +7,9 @@ time 1..K, and every time slot, halo included, is compared with float64. Each ca
 meant to exercise and asserts it through `b2_last_sweep_kernel`: a layout that silently falls back to another
 kernel fails instead of passing vacuously. Tolerances: rel L-inf 1e-5 (iso), 1e-4 (TTI), receiver traces included.
 
-Switches are set with monkeypatch; the library reads them per call. `B2_TTI_PF` is the exception: it is read once
-per process, so the prefetch depth of `k_tti_ws` cannot be varied here and stays out of this matrix.
+Switches are set with monkeypatch; the library reads them per call.
 """
 import functools
-import os
 from types import SimpleNamespace
 
 import numpy as np
@@ -160,19 +158,6 @@ def test_iso_tma(so, param, lx, monkeypatch):
     _check_iso(('iso', so, param), f'iso_tma<{so // 2},{PK[param]}>')
 
 
-@pytest.mark.parametrize('variant', [4, 1])
-@pytest.mark.parametrize('param', PARAMS)
-def test_iso_two_row(param, variant, monkeypatch):
-    monkeypatch.setenv('B2_ISO_V2', str(variant))
-    if variant == 4 and param != 'scalar':
-        # three coefficient-tile rings need 248 KB of shared memory, above the 227 KB a block may have: refused
-        from devito_b200 import ExecutionError
-        with pytest.raises(ExecutionError, match='shared memory'):
-            _check_iso(('iso', 12, param), None)
-        return
-    _check_iso(('iso', 12, param), f'iso_tma2_v{variant}<6,{PK[param]}>')
-
-
 @pytest.mark.parametrize('shape,box', [((37, 45, 67), None), (KC.SHAPE, ((0, 0, 3), (36, 44, 67)))],
                          ids=['nz67', 'zm3'])
 def test_iso_fallback_to_generic(shape, box):
@@ -195,7 +180,7 @@ def test_tti_two_pass(so, arrays):
 @pytest.mark.parametrize('so,switch,expect', [
     (4, None, 'tti_fused<2>'),
     (8, '2', 'tti_fused<4>'),
-    (8, '3', 'tti_ws<pf1>' if os.environ.get('B2_TTI_PF', '1') == '1' else 'tti_ws<pf2>'),
+    (8, '3', 'tti_ws<pf1>'),
 ])
 def test_tti_fused_scalar(so, switch, expect, monkeypatch):
     monkeypatch.setenv('B2_TTI_LX', '12')

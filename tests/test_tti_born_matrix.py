@@ -9,7 +9,6 @@ and which path of the Born source term ran ("+born_v4": float4 along z, taken wh
 16-byte aligned; "+born_s" otherwise). Tolerance: rel L-inf 1e-4 for u0, v0, du, dv and the traces.
 """
 import functools
-import os
 from types import SimpleNamespace
 
 import numpy as np
@@ -22,7 +21,6 @@ import tti_born_ref as TB
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-4
-WS = 'tti_ws<pf1>' if os.environ.get('B2_TTI_PF', '1') == '1' else 'tti_ws<pf2>'
 
 
 def _last_kernel():
@@ -126,7 +124,7 @@ VARIANTS = [
     (4, False, {}, 0, 'tti_fused<2>'),
     (8, False, {}, 1, 'tti_two_pass'),
     (8, False, {'B2_TTI_KERNEL': '2'}, 0, 'tti_fused<4>'),
-    (8, False, {}, 0, WS),
+    (8, False, {}, 0, 'tti_ws<pf1>'),
     (12, False, {}, 0, 'tti_two_pass'),
     (4, True, {'B2_TTI_ARR_CT': '0'}, 0, 'tti_arr_ct0<2>'),
     (4, True, {'B2_TTI_ARR_CT': '1'}, 0, 'tti_arr_ct1<2>'),
