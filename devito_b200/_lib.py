@@ -83,7 +83,8 @@ class SysTap(Structure):
 
 
 class SysStage(Structure):
-    _fields_ = [('out_field', c_int), ('out_tshift', c_int), ('ntaps', c_int), ('taps', POINTER(SysTap))]
+    _fields_ = [('out_field', c_int), ('out_tshift', c_int), ('ntaps', c_int), ('taps', POINTER(SysTap)),
+                ('ext', c_int)]
 
 
 class SysInject(Structure):

@@ -2,9 +2,9 @@
 // (staggered) grid — the generated `ForwardElastic` (examples/seismic/elastic/operators.py:26-65) and its
 // relatives — as a tap-table executor: per time step a sequence of stages, each
 //     out[t + out_tshift][p] = sum_k coef_k * C_{cfield_k}[p] * F_{field_k}[t + tshift_k][p + off_k].
-// One thread per point, four z points per thread where the row allows 16-byte stores; taps in the kernel
-// parameter block. This is the generality path of §8f (staggered-grid systems), not a tuned sweep: the
-// acoustic / TTI propagators keep their own kernels.
+// One thread per point (z fastest, x strided over gridDim.z); taps in the kernel parameter block. This is
+// the generality path of §8f (staggered-grid systems), not a tuned sweep: the acoustic / TTI propagators
+// keep their own kernels. tests/system_ref.py restates these semantics in float64.
 #include "b2_common.cuh"
 #include "b2_sparse.cuh"
 #include <algorithm>
@@ -57,6 +57,22 @@ extern "C" int b2_system_forward(const struct b2_system_args *a) {
                   B2_SYS_MAX_FIELDS, B2_SYS_MAX_COEFS);
         return B2_ERR_INVALID;
     }
+    if (a->nstages < 0 || a->ninject < 0 || a->ninterp < 0 || (a->ninject && !a->inject) || (a->ninterp && !a->interp)) {
+        set_error("b2_system_forward: malformed stage / injection / interpolation counts");
+        return B2_ERR_INVALID;
+    }
+    // sparse terms index the fields: check them before anything is staged
+    for (int i = 0; i < a->ninject; ++i) {
+        const b2_sys_inject &q = a->inject[i];
+        bool ok = q.nfields >= 1 && q.nfields <= 3 && q.param_kind >= B2_PARAM_SCALAR && q.param_kind <= B2_PARAM_M;
+        for (int j = 0; ok && j < q.nfields; ++j) ok = q.fields[j] >= 0 && q.fields[j] < a->nfields;
+        if (!ok) { set_error("b2_system_forward: injection %d is malformed (fields / parameter kind)", i); return B2_ERR_INVALID; }
+    }
+    for (int i = 0; i < a->ninterp; ++i)
+        if (a->interp[i].field < 0 || a->interp[i].field >= a->nfields) {
+            set_error("b2_system_forward: interpolation %d samples field %d of %d", i, a->interp[i].field, a->nfields);
+            return B2_ERR_INVALID;
+        }
     if (a->time_M < a->time_m) return B2_OK;
     std::lock_guard<std::mutex> api_lock(api_mutex());
     if (int rc0 = use_device(a->deviceid)) return rc0;
@@ -80,6 +96,7 @@ extern "C" int b2_system_forward(const struct b2_system_args *a) {
     for (int i = 0; i < a->nfields; ++i) {
         if ((rc = stage_in(a->fields[i], nd + 1, F[i], true))) return cleanup(rc);
         ++staged_f;
+        if (F[i].size[0] < 1) { set_error("b2_system_forward: field %d has no time slot", i); return cleanup(B2_ERR_INVALID); }
         for (int d = 1; d <= nd; ++d)
             if (F[i].size[d] != F[0].size[d]) { set_error("b2_system_forward: field %d has another shape", i); return cleanup(B2_ERR_INVALID); }
     }
@@ -128,34 +145,39 @@ extern "C" int b2_system_forward(const struct b2_system_args *a) {
     k.csy = calloc_[2];
     k.csx = (long long)calloc_[1] * calloc_[2];
     const size_t slot = (size_t)alloc[0] * alloc[1] * alloc[2];
-    k.n0 = hi[0] - lo[0] + 1; k.n1 = hi[1] - lo[1] + 1; k.n2 = hi[2] - lo[2] + 1;
-    k.o0 = lo[0] + hal[0]; k.o1 = lo[1] + hal[1]; k.o2 = lo[2] + hal[2];
-    k.c0 = lo[0]; k.c1 = lo[1]; k.c2 = lo[2];
-    if (k.n0 <= 0 || k.n1 <= 0 || k.n2 <= 0) return cleanup(B2_OK);
+    if (hi[0] < lo[0] || hi[1] < lo[1] || hi[2] < lo[2]) return cleanup(B2_OK);
     for (int i = 0; i < a->ncoefs; ++i) k.cf[i] = (const float *)C[i].d;
     for (int i = a->ncoefs; i < B2_SYS_MAX_COEFS; ++i) k.cf[i] = nullptr;
+    auto slot_of = [&](int f, int time, int shift) {
+        const int T = F[f].size[0];
+        return (((time + shift) % T) + T) % T;
+    };
 
     // validate the stages once
     for (int s = 0; s < a->nstages; ++s) {
         const b2_sys_stage &st = a->stages[s];
-        if (st.out_field < 0 || st.out_field >= a->nfields || st.ntaps < 1 || st.ntaps > B2_SYS_MAX_TAPS || !st.taps) {
-            set_error("b2_system_forward: stage %d is malformed (%d taps, at most %d)", s, st.ntaps, B2_SYS_MAX_TAPS);
+        if (st.out_field < 0 || st.out_field >= a->nfields || st.ntaps < 1 || st.ntaps > B2_SYS_MAX_TAPS || !st.taps ||
+            st.ext < 0 || st.ext > h) {
+            set_error("b2_system_forward: stage %d is malformed (%d taps, at most %d; box widened by %d, at most %d)", s,
+                      st.ntaps, B2_SYS_MAX_TAPS, st.ext, h);
             return cleanup(B2_ERR_INVALID);
         }
         for (int i = 0; i < st.ntaps; ++i) {
             const b2_sys_tap &t = st.taps[i];
-            if (t.field < 0 || t.field >= a->nfields || t.tshift < 0 || t.tshift > 1 || t.cfield >= a->ncoefs) {
+            if (t.field < 0 || t.field >= a->nfields || t.tshift < 0 || t.tshift > 1 || t.cfield >= a->ncoefs ||
+                (st.ext > 0 && t.cfield >= 0)) {
                 set_error("b2_system_forward: stage %d tap %d is malformed", s, i);
                 return cleanup(B2_ERR_INVALID);
             }
-            if (t.field == st.out_field && t.tshift == st.out_tshift && F[t.field].size[0] > 1 &&
+            // the kernel reads and writes in place: a shifted read of the written level would race with the writes
+            if (t.field == st.out_field && slot_of(t.field, 0, t.tshift) == slot_of(t.field, 0, st.out_tshift) &&
                 (t.off[0] || t.off[1] || t.off[2])) {
                 set_error("b2_system_forward: stage %d reads shifted points of the level it writes", s);
                 return cleanup(B2_ERR_INVALID);
             }
             for (int d = 0; d < nd; ++d) {
                 const int di = 3 - nd + d;
-                if (lo[di] + hal[di] + t.off[d] < 0 || hi[di] + hal[di] + t.off[d] >= alloc[di]) {
+                if (lo[di] - st.ext + hal[di] + t.off[d] < 0 || hi[di] + st.ext + hal[di] + t.off[d] >= alloc[di]) {
                     set_error("b2_system_forward: stage %d tap offset %d on dim %d leaves the allocated array", s, t.off[d], d);
                     return cleanup(B2_ERR_INVALID);
                 }
@@ -171,11 +193,6 @@ extern "C" int b2_system_forward(const struct b2_system_args *a) {
     const bool timing = a->timers != nullptr;
     if (timing) for (auto &e : ev) cudaEventCreate(&e);
     dim3 block(64, 4, 1);
-    dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
-    auto slot_of = [&](int f, int time, int shift) {
-        const int T = F[f].size[0];
-        return (((time + shift) % T) + T) % T;
-    };
     const int nsteps = a->time_M - a->time_m + 1;
     const bool per_step = timing && nsteps <= 2048;
     std::vector<cudaEvent_t> pool;
@@ -185,6 +202,12 @@ extern "C" int b2_system_forward(const struct b2_system_args *a) {
         if (per_step) rec_ev();
         for (int s = 0; s < a->nstages; ++s) {
             const b2_sys_stage &st = a->stages[s];
+            // the box, widened by ext on the space axes (internal axis 0 of a 2-D grid is the dummy extent 1)
+            const int e0 = nd == 3 ? st.ext : 0, e = st.ext;
+            k.n0 = hi[0] - lo[0] + 1 + 2 * e0; k.n1 = hi[1] - lo[1] + 1 + 2 * e; k.n2 = hi[2] - lo[2] + 1 + 2 * e;
+            k.o0 = lo[0] - e0 + hal[0]; k.o1 = lo[1] - e + hal[1]; k.o2 = lo[2] - e + hal[2];
+            k.c0 = lo[0] - e0; k.c1 = lo[1] - e; k.c2 = lo[2] - e;       // unused when e > 0 (no cfield)
+            const dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
             k.out = (float *)F[st.out_field].d + (size_t)slot_of(st.out_field, time, st.out_tshift) * slot;
             for (int f = 0; f < a->nfields; ++f)
                 for (int t = 0; t < 2; ++t)

@@ -259,7 +259,7 @@ class _SystemPlan:
     def __init__(self):
         self.fields = []            # reference TimeFunctions, index = field id
         self.scratch = []           # (field id, name) of scratch fields (interpolated expressions)
-        self.stages = []            # (out id, out_tshift, [(fid, tshift, off, coef, key|None)])
+        self.stages = []            # (out id, out_tshift, [(fid, tshift, off, coef, key|None)], box widening)
         self.coef_exprs = {}        # key -> sympy expression of a coefficient array
         self.injections = []        # (sparse function, [fids], tshift, scale expression)
         self.interpolations = []    # (sparse function, fid, tshift)
@@ -402,7 +402,7 @@ def _restate_system(expressions, kwargs):
         tshift, offs = _array_offsets(lhs)
         if tshift != 1 or any(offs):
             raise _Unconvertible("lhs is not `f.forward` at the function's own position")
-        plan.stages.append((fid[lhs.function.name], 1, taps_of(rhs)))
+        plan.stages.append((fid[lhs.function.name], 1, taps_of(rhs), 0))
     dt = grid.stepping_dim.spacing
     for e in sparse_ops:
         sf = e.interpolator.sfunction
@@ -460,8 +460,15 @@ def _restate_system(expressions, kwargs):
                 # an expression (div(v) ...): an extra stage fills a scratch field that is then sampled
                 evx = ex.evaluate
                 sid = len(plan.fields) + len(plan.scratch)
+                taps = taps_of(evx)
+                # the interpolation guard samples cells up to r beyond the domain, where the reference evaluates the
+                # expression from the fields' halo: the stage's box is widened by r, which its taps must allow
+                r = int(sf.r)
+                if any(key is not None for *_, key in taps) or any(abs(o) + r > so for _, _, offs, _, _ in taps
+                                                                   for o in offs):
+                    raise _Unconvertible(f"{sf.name}: the expression cannot be evaluated {r} cells into the halo")
                 plan.scratch.append((sid, f"scratch_{sf.name}"))
-                plan.stages.append((sid, 0, taps_of(evx)))
+                plan.stages.append((sid, 0, taps, r))
                 plan.interpolations.append((sf, sid, 0))
     if len(plan.fields) + len(plan.scratch) > 16:
         raise _Unconvertible("too many fields")
@@ -643,8 +650,8 @@ class B200CudaOperator(Cpu64AdvOmpOperator):
         def scalar(ex):
             ex = sympy.sympify(ex)
             return float(ex.xreplace({q: values[q.name] for q in ex.free_symbols if q.name in values}))
-        stages = [Stage(out, ts, [Tap(f, t, o, scalar(c), kid[key] if key is not None else -1) for f, t, o, c, key in taps])
-                  for out, ts, taps in plan.stages]
+        stages = [Stage(out, ts, [Tap(f, t, o, scalar(c), kid[key] if key is not None else -1) for f, t, o, c, key in taps],
+                        ext) for out, ts, taps, ext in plan.stages]
 
         def sparse(sf):
             ws = [dataobj(f"{sf.name}_w{'xyz'[i]}" if f"{sf.name}_w{'xyz'[i]}" in args else f"wsincrp_{sf.name}{'xyz'[i]}")

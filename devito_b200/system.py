@@ -27,8 +27,10 @@ class Tap:
 
 
 class Stage:
-    def __init__(self, out_field, out_tshift, taps):
-        self.out_field, self.out_tshift = int(out_field), int(out_tshift)
+    def __init__(self, out_field, out_tshift, taps, ext=0):
+        """ext: the box widened by `ext` cells per side on every space axis (a scratch field that receivers sample
+        next to the domain's faces; such a stage may not use coefficient arrays)."""
+        self.out_field, self.out_tshift, self.ext = int(out_field), int(out_tshift), int(ext)
         self.taps = sorted(taps, key=lambda t: (t.cfield, t.field, t.tshift, t.off))     # the kernel caches C by run
         if not 1 <= len(self.taps) <= L_.SYS_MAX_TAPS:
             raise InvalidArgument(f"a stage has {len(self.taps)} taps (1..{L_.SYS_MAX_TAPS} supported)")
@@ -52,6 +54,17 @@ class LinearSystem:
         """fields: list of `_lib.ForeignDataobj` / DataobjHolder (host-staged or resident); coefs: list of float32
         arrays of the grid's shape; injections/interpolations hold `_lib.ForeignSparse`. Returns the timers."""
         L = L_.lib()
+        a, timers, hold = self.arguments(fields, coefs, lo, hi, time_m, time_M, deviceid)
+        t0 = _time.perf_counter()
+        rc = L.b2_system_forward(ctypes.byref(a))
+        wall = _time.perf_counter() - t0
+        if rc != 0:
+            from .exceptions import ExecutionError
+            raise ExecutionError(f"b2_system_forward failed with code {rc}: {L.b2_last_error().decode()}")
+        return timers, wall
+
+    def arguments(self, fields, coefs, lo, hi, time_m, time_M, deviceid=0):
+        """The `struct b2_system_args` of a call, its timers, and what must stay alive while it is in use."""
         nd = self.ndim
         hold = []
         a = L_.SystemArgs()
@@ -64,6 +77,7 @@ class LinearSystem:
         # (e.g. device-resident: the plugin keeps the tabulated arrays on the GPU across applies)
         cobjs = [c if hasattr(c, 'ptr') else L_.make_dataobj(host=np.ascontiguousarray(c, dtype=np.float32))
                  for c in coefs]
+        hold.append(cobjs)
         carr = (ctypes.POINTER(L_.Dataobj) * max(1, len(cobjs)))(*[c.ptr for c in cobjs])
         a.ncoefs, a.coefs = len(cobjs), carr
         st = (L_.SysStage * len(self.stages))()
@@ -75,6 +89,7 @@ class LinearSystem:
                     taps[j].off[d] = int(t.off[d])
             hold.append(taps)
             st[i].out_field, st[i].out_tshift, st[i].ntaps, st[i].taps = s.out_field, s.out_tshift, len(s.taps), taps
+            st[i].ext = s.ext
         a.nstages, a.stages = len(self.stages), st
 
         def sparse(sf):
@@ -101,10 +116,4 @@ class LinearSystem:
         a.time_m, a.time_M, a.deviceid = int(time_m), int(time_M), int(deviceid)
         timers = L_.Profiler()
         a.timers = ctypes.pointer(timers)
-        t0 = _time.perf_counter()
-        rc = L.b2_system_forward(ctypes.byref(a))
-        wall = _time.perf_counter() - t0
-        if rc != 0:
-            from .exceptions import ExecutionError
-            raise ExecutionError(f"b2_system_forward failed with code {rc}: {L.b2_last_error().decode()}")
-        return timers, wall
+        return a, timers, hold

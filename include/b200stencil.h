@@ -253,7 +253,11 @@ int b2_linear_forward(const struct b2_linear_args *a);
  * later stage may read what an earlier one wrote at t+1 (tshift = 1). After the stages of a step:
  * injections (into up to 3 fields at once: the diagonal of the stress tensor) and interpolations
  * (of a field, or of a scratch field that an extra stage filled, e.g. div(v)).
- * All fields share the grid extents and the halo width `halo`; a field with 1 time slot is scratch. */
+ * All fields share the grid extents and the halo width `halo`; a field with 1 time slot is scratch.
+ * A stage that reads shifted points of the level it writes is refused (every level of a 1-slot field is
+ * the level it writes). A stage may widen its box by `ext` cells on every space axis: a scratch field
+ * that receivers sample must also hold its values on the halo cells their support reaches (the
+ * interpolation guard is d_m - r <= cell <= d_M + r); such a stage may not use coefficient arrays. */
 struct b2_sys_tap {
     int field;                        /* index into `fields`                                    */
     int tshift;                       /* time level read: t + tshift (0 or 1)                   */
@@ -266,6 +270,7 @@ struct b2_sys_stage {
     int out_tshift;                   /* +1 for an update, 0 for a scratch field                */
     int ntaps;
     const struct b2_sys_tap *taps;
+    int ext;                          /* box widened by ext cells per side (0..halo; no cfield) */
 };
 struct b2_sys_inject {
     struct b2_sparse *s;
