@@ -125,7 +125,7 @@ SYMBOLS = ['b2_iso_forward', 'b2_tti_forward', 'b2_linear_forward', 'b2_system_f
            'b2_launch_count', 'b2_last_sweep_kernel', 'b2_kernel_timing_reset', 'b2_kernel_timing_ms',
            'b2_kernel_timing_enable', 'b2_malloc_device', 'b2_free_device', 'b2_memcpy_h2d',
            'b2_memcpy_d2h', 'b2_memset_device', 'b2_synchronize', 'b2_set_stream',
-           'b2_staging_cache_release', 'b2_last_call_profile', 'b2_device_pci_bus_id',
+           'b2_staging_cache_release', 'b2_staging_outstanding', 'b2_last_call_profile', 'b2_device_pci_bus_id',
            'b2_ipc_get_handle', 'b2_ipc_open', 'b2_ipc_close', 'b2_halo_p2p_setup',
            'b2_halo_p2p_register']
 
@@ -187,6 +187,8 @@ def load_library():
     L.b2_set_stream.restype = None
     L.b2_staging_cache_release.argtypes = []
     L.b2_staging_cache_release.restype = None
+    L.b2_staging_outstanding.argtypes = []
+    L.b2_staging_outstanding.restype = c_ulonglong
     L.b2_last_call_profile.argtypes = [POINTER(c_double)]
     L.b2_last_call_profile.restype = None
     L.b2_device_pci_bus_id.argtypes = [c_int, c_char_p, c_int]

@@ -20,57 +20,6 @@ using namespace b2;
 
 namespace b2 {
 
-// NaN/Inf check (reference: errctl='max' checks every 100 steps, passes/iet/errors.py:59-85)
-__global__ void k_check_finite(const float *__restrict__ f, size_t n, int *flag) {
-    size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-    const size_t stride = (size_t)gridDim.x * blockDim.x;
-    bool bad = false;
-    for (; i < n; i += stride) bad |= !isfinite(f[i]);
-    if (bad) atomicOr(flag, 1);
-}
-
-int check_finite(const float *f, size_t n, bool &bad) {
-    static int *d_flag = nullptr;
-    if (!d_flag) B2_CUDA(cudaMalloc(&d_flag, sizeof(int)), B2_ERR_MEMORY);
-    B2_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), stream()), B2_ERR_MEMORY);
-    B2_SM_COUNT(sms);
-    k_check_finite<<<sms * 4, 256, 0, stream()>>>(f, n, d_flag);
-    count_launch();
-    int h = 0;
-    B2_CUDA(cudaMemcpyAsync(&h, d_flag, sizeof(int), cudaMemcpyDeviceToHost, stream()), B2_ERR_MEMORY);
-    B2_CUDA(cudaStreamSynchronize(stream()), B2_ERR_DEVICE);
-    bad = h != 0;
-    return B2_OK;
-}
-
-// Imaging condition (reference: `Inc(grad, -u * v.dt2)`, acoustic/operators.py:222; the TTI gradient's
-// `Inc(dm, -(u0 * du.dt2 + v0 * dv.dt2))`, tti/operators.py `JacobianAdjOperator`, with the second pair):
-// grad[p] -= usave[time][p] * (v[t+1][p] - 2 v[t][p] + v[t-1][p]) / dt^2 (+ the same of us2, w) over the iterated box.
-__global__ void __launch_bounds__(256) k_imaging(ImgK k) {
-    const int z = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (z >= k.n2 || y >= k.n1) return;
-    for (int x = blockIdx.z; x < k.n0; x += gridDim.z) {
-        const long long i = (long long)(k.o0 + x) * k.sx + (long long)(k.o1 + y) * k.sy + (k.o2 + z);
-        const long long g = (long long)(k.g0 + x) * k.gsx + (long long)(k.g1 + y) * k.gsy + (k.g2 + z);
-        const float d2 = (k.v1[i] - 2.0f * k.v0[i] + k.v2[i]) * k.inv_dt2;
-        if (k.us2) {
-            const float e2 = (k.w1[i] - 2.0f * k.w0[i] + k.w2[i]) * k.inv_dt2;
-            k.grad[g] = k.grad[g] - fmaf(k.us[i], d2, k.us2[i] * e2);
-        } else {
-            k.grad[g] = k.grad[g] - k.us[i] * d2;
-        }
-    }
-}
-
-int launch_imaging(const ImgK &ik) {
-    dim3 blk(64, 4, 1), grd((ik.n2 + 63) / 64, (ik.n1 + 3) / 4, (unsigned)(ik.n0 < 65535 ? ik.n0 : 65535));
-    k_imaging<<<grd, blk, 0, stream()>>>(ik);
-    count_launch();
-    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
-    return B2_OK;
-}
-
 // Section timing with a reusable pool of CUDA events: 4 events per time step.
 struct StepEvents {
     std::vector<cudaEvent_t> ev;
@@ -286,7 +235,7 @@ static int iso_forward_streamed(const b2_iso_args *a, IsoPlan &p, FieldGeom g, D
     B2_CUDA(cudaStreamWaitEvent(S.up, ev_start, 0), B2_ERR_DEVICE);
     B2_CUDA(cudaStreamWaitEvent(S.down, ev_start, 0), B2_ERR_DEVICE);
 
-    const int t0_first = ((a->time_m % 3) + 3) % 3;
+    const int t0_first = slot(a->time_m, 3);
     if (decomposed) {
         // the first sub-launch exchanges the initial level's boundary planes through NCCL (like the first step of a
         // resident call): they must be on the device, all rows, before anything else
@@ -326,7 +275,7 @@ static int iso_forward_streamed(const b2_iso_args *a, IsoPlan &p, FieldGeom g, D
     if (rec.present) {
         const int r0 = std::max(a->time_m, 0), r1 = std::min(a->time_M, rec.nt - 1);
         if (r1 >= r0)
-            B2_CUDA(cudaMemsetAsync((float *)rec.data.d + (size_t)r0 * rec.npoint_total, 0,
+            B2_CUDA(cudaMemsetAsync((float *)rec.data->d + (size_t)r0 * rec.npoint_total, 0,
                                     (size_t)(r1 - r0 + 1) * rec.npoint_total * sizeof(float), cs), B2_ERR_MEMORY);
     }
 
@@ -370,7 +319,7 @@ static int iso_forward_streamed(const b2_iso_args *a, IsoPlan &p, FieldGeom g, D
             const int ra = std::max(0, ph * W - shift);
             if (ra >= rb) continue;
             const int time = a->time_m + s - 1;
-            const int t0 = ((time % 3) + 3) % 3, t1 = (((time + 1) % 3) + 3) % 3, t2 = (((time - 1) % 3) + 3) % 3;
+            const int t0 = slot(time, 3), t1 = slot(time + 1, 3), t2 = slot(time - 1, 3);
             float *f1 = p.u + (size_t)t1 * p.slot_elems;
             FieldGeom q = range_geom(ra, rb);
             if (dim == 0) {
@@ -433,69 +382,18 @@ extern "C" void b2_last_call_profile(double out[5]) {
     for (int i = 0; i < 5; ++i) out[i] = b2::g_last_profile[i];
 }
 
-extern "C" int b2_iso_forward(const struct b2_iso_args *a) {
-    if (!a || !a->u) { set_error("b2_iso_forward: NULL args"); return B2_ERR_INVALID; }
-    if (a->ndim != 2 && a->ndim != 3) { set_error("b2_iso_forward: ndim must be 2 or 3"); return B2_ERR_INVALID; }
-    if (a->radius < 1 || a->radius > B2_MAX_RADIUS || a->radius > a->space_order) {
-        set_error("b2_iso_forward: unsupported radius %d (space_order %d)", a->radius, a->space_order);
-        return B2_ERR_INVALID;
-    }
-    if (a->time_M < a->time_m) return B2_OK;
-    std::lock_guard<std::mutex> api_lock(api_mutex());
-    if (int rc0 = use_device(a->deviceid)) return rc0;
-    note_sweep_kernel("");
-
+static int iso_forward_body(const b2_iso_args *a, Staging &st, SnapStreamer &streamer,
+                            std::chrono::steady_clock::time_point call_t0) {
     const int nd = a->ndim;
     const int so = a->space_order;
     int rc = B2_OK;
 
-    DevArray u, damp, param, grad, usave, bornU, borndm, snap;
-    bool staged_grad = false, staged_usave = false, staged_bornU = false, staged_borndm = false;
-    bool staged_snap = false;
-    SnapStreamer streamer;
+    DevArray *u, *damp = nullptr, *param = nullptr, *grad = nullptr, *usave = nullptr, *bornU = nullptr,
+             *borndm = nullptr, *snap = nullptr;
+    DevArray snap_host;                           // host snapshots streamed out: described, not staged
     SparseDev src, rec;
     IsoPlan p;
     FieldGeom g;
-    bool staged_u = false, staged_damp = false, staged_param = false;
-    bool u_is_home = false;                       // the streamed loop already brought u back to the host
-    bool u_host_io = false;                       // caller-provided device buffer next to the host array (host_io)
-    auto call_t0 = std::chrono::steady_clock::now();
-    for (double &v : g_last_profile) v = 0.0;
-
-    auto cleanup = [&](int code) {
-        // copy back what the reference would copy back (u and rec), free staged copies
-        const auto d2h_t0 = std::chrono::steady_clock::now();
-        int r1 = staged_u ? stage_out(u, (code == B2_OK || code == B2_ERR_NAN) && !u_is_home) : B2_OK;
-        if (staged_u && u_host_io && !u_is_home && (code == B2_OK || code == B2_ERR_NAN)) {
-            cudaError_t ce = cudaMemcpyAsync(u.h, u.d, u.nbytes, cudaMemcpyDeviceToHost, stream());
-            if (ce == cudaSuccess) ce = cudaStreamSynchronize(stream());
-            if (ce != cudaSuccess) { set_error("b2_iso_forward: device -> host copy failed"); r1 = B2_ERR_MEMORY; }
-        }
-        g_last_profile[2] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - d2h_t0).count();
-        g_last_profile[3] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - call_t0).count();
-        if (staged_damp) stage_out(damp, false);
-        if (staged_param) stage_out(param, false);
-        if (staged_usave) stage_out(usave, false);
-        int r3 = staged_grad ? stage_out(grad, code == B2_OK) : B2_OK;
-        if (staged_snap) {
-            const int r5 = stage_out(snap, code == B2_OK || code == B2_ERR_NAN);
-            if (!r3) r3 = r5;
-        }
-        {
-            const int r6 = streamer.end();
-            if (!r3) r3 = r6;
-        }
-        if (staged_borndm) stage_out(borndm, false);
-        if (staged_bornU) {
-            const int r4 = stage_out(bornU, code == B2_OK || code == B2_ERR_NAN);
-            if (!r3) r3 = r4;
-        }
-        if (code == B2_OK && r3) return r3;
-        sparse_stage_out(src, false);
-        int r2 = sparse_stage_out(rec, code == B2_OK || code == B2_ERR_NAN);
-        if (code != B2_OK) return code;
-        return r1 ? r1 : r2;
-    };
 
     // A large host-staged wavefield is a candidate for the streamed time loop (copies overlapped with a
     // skewed sweep, iso_forward_streamed): its uploads are then issued chunk by chunk, not here. Whether the
@@ -514,101 +412,92 @@ extern "C" int b2_iso_forward(const struct b2_iso_args *a) {
             return false;
         return true;
     }();
-    call_t0 = std::chrono::steady_clock::now();
-    if ((rc = stage_in(a->u, nd + 1, u, !maybe_stream))) return cleanup(rc);
-    staged_u = true;
-    u_host_io = host_io;
-    if (a->damp) {
-        if ((rc = stage_in(a->damp, nd, damp, !maybe_stream))) return cleanup(rc);
-        staged_damp = true;
-    }
+    if ((rc = st.array(a->u, nd + 1, true, u, !maybe_stream))) return rc;
+    u->host_io = host_io;
+    if (a->damp && (rc = st.array(a->damp, nd, false, damp, !maybe_stream))) return rc;
     if (a->param_kind != B2_PARAM_SCALAR) {
-        if (!a->param) { set_error("b2_iso_forward: param array missing"); return cleanup(B2_ERR_INVALID); }
-        if ((rc = stage_in(a->param, nd, param, !maybe_stream))) return cleanup(rc);
-        staged_param = true;
+        if (!a->param) { set_error("b2_iso_forward: param array missing"); return B2_ERR_INVALID; }
+        if ((rc = st.array(a->param, nd, false, param, !maybe_stream))) return rc;
     }
-    if ((rc = sparse_stage_in(a->src, nd, src, true))) return cleanup(rc);
-    if ((rc = sparse_stage_in(a->rec, nd, rec, true))) return cleanup(rc);
+    if ((rc = sparse_stage_in(st, a->src, nd, false, src))) return rc;
+    if ((rc = sparse_stage_in(st, a->rec, nd, true, rec))) return rc;
     // the support of a sparse point reaches r cells beyond the iterated box: it must fit in the halo
     // (devito/operations/interpolators.py:28-37 `check_radius`)
     if ((src.present && src.r > so) || (rec.present && rec.r > so)) {
         set_error("b2_iso_forward: sparse radius %d exceeds the halo (space_order %d)",
                   src.present && src.r > so ? src.r : rec.r, so);
-        return cleanup(B2_ERR_INVALID);
+        return B2_ERR_INVALID;
     }
+    int gh = 0;
     if (a->grad || a->usave) {
         if (!a->grad || !a->usave || nd != 3) {
             set_error("b2_iso_forward: the imaging condition needs both grad and usave (3-D)");
-            return cleanup(B2_ERR_INVALID);
+            return B2_ERR_INVALID;
         }
-        if ((rc = stage_in(a->grad, 3, grad, true))) return cleanup(rc);
-        staged_grad = true;
-        if ((rc = stage_in(a->usave, 4, usave, true))) return cleanup(rc);
-        staged_usave = true;
+        if ((rc = st.array(a->grad, 3, true, grad))) return rc;
+        if ((rc = st.array(a->usave, 4, false, usave))) return rc;
+        // k_imaging reads usave with u's strides and writes grad inside its extents
+        if (grid_halo("b2_iso_forward", "usave", a->usave, *usave, 1, *u, 3, so, so) < 0 ||
+            (gh = grid_halo("b2_iso_forward", "grad", a->grad, *grad, 0, *u, 3, so)) < 0)
+            return B2_ERR_INVALID;
     }
 
     const bool born = a->born_U || a->born_dm;
+    int dmh = 0;
     if (born) {
         if (!a->born_U || !a->born_dm || nd != 3 || a->adjoint || a->grad || a->free_surface || a->ot4) {
             set_error("b2_iso_forward: Born modelling needs born_U and born_dm, 3-D, forward in time, and is "
                       "not combined with a free surface, OT4 or the imaging condition");
-            return cleanup(B2_ERR_INVALID);
+            return B2_ERR_INVALID;
         }
-        if ((rc = stage_in(a->born_U, 4, bornU, true))) return cleanup(rc);
-        staged_bornU = true;
-        if ((rc = stage_in(a->born_dm, 3, borndm, true))) return cleanup(rc);
-        staged_borndm = true;
+        if ((rc = st.array(a->born_U, 4, true, bornU))) return rc;
+        if ((rc = st.array(a->born_dm, 3, false, borndm))) return rc;
         for (int d = 0; d < 4; ++d)
-            if (bornU.size[d] != u.size[d]) {
+            if (bornU->size[d] != u->size[d]) {
                 set_error("b2_iso_forward: born_U must have the layout of u");
-                return cleanup(B2_ERR_INVALID);
+                return B2_ERR_INVALID;
             }
+        if ((dmh = grid_halo("b2_iso_forward", "born_dm", a->born_dm, *borndm, 0, *u, 3, so)) < 0) return B2_ERR_INVALID;
     }
 
     int snap_h = 0;
     if (a->snap) {
         if (a->snap_factor < 1 || a->adjoint) {
             set_error("b2_iso_forward: snapshots need snap_factor >= 1 and forward time stepping");
-            return cleanup(B2_ERR_INVALID);
+            return B2_ERR_INVALID;
         }
         const bool stream_out = !a->snap->dmap && a->snap->data && nd == 3 &&
                                 !(getenv("B2_SNAP_STREAM") && atoi(getenv("B2_SNAP_STREAM")) == 0);
         if (stream_out) {
             // describe the array without allocating it on the device
-            if (!a->snap->size) { set_error("b2_iso_forward: snapshot dataobj without `size`"); return cleanup(B2_ERR_INVALID); }
-            snap.ndim = nd + 1;
-            for (int d = 0; d <= nd; ++d) snap.size[d] = a->snap->size[d];
-            snap.h = a->snap->data;
-            snap.d = nullptr;
-        } else {
-            if ((rc = stage_in(a->snap, nd + 1, snap, true))) return cleanup(rc);
-            staged_snap = true;
+            if (!a->snap->size) { set_error("b2_iso_forward: snapshot dataobj without `size`"); return B2_ERR_INVALID; }
+            snap = &snap_host;
+            snap->ndim = nd + 1;
+            for (int d = 0; d <= nd; ++d) snap->size[d] = a->snap->size[d];
+            snap->h = a->snap->data;
+        } else if ((rc = st.array(a->snap, nd + 1, true, snap))) {
+            return rc;
         }
-        snap_h = a->snap->hsize ? a->snap->hsize[2] : (snap.size[1] - (u.size[1] - 2 * so)) / 2;
-        for (int d = 0; d < nd; ++d)
-            if (snap.size[d + 1] != u.size[d + 1] - 2 * so + 2 * snap_h) {
-                set_error("b2_iso_forward: snapshot extent %d on dim %d does not match the grid", snap.size[d + 1], d);
-                return cleanup(B2_ERR_INVALID);
-            }
-        if (a->time_m < 0 || a->time_M / a->snap_factor >= snap.size[0]) {
+        if ((snap_h = grid_halo("b2_iso_forward", "snapshot", a->snap, *snap, 1, *u, nd, so)) < 0) return B2_ERR_INVALID;
+        if (a->time_m < 0 || a->time_M / a->snap_factor >= snap->size[0]) {
             set_error("b2_iso_forward: time_M=%d needs %d snapshots, the array holds %d", a->time_M,
-                      a->time_M / a->snap_factor + 1, snap.size[0]);
-            return cleanup(B2_ERR_INVALID);
+                      a->time_M / a->snap_factor + 1, snap->size[0]);
+            return B2_ERR_INVALID;
         }
         if (stream_out) {
-            const size_t one = (size_t)snap.size[1] * snap.size[2] * snap.size[3];
-            if ((rc = streamer.begin(snap.h, one * snap.size[0] * sizeof(float), one))) return cleanup(rc);
+            const size_t one = (size_t)snap->size[1] * snap->size[2] * snap->size[3];
+            if ((rc = streamer.begin(snap->h, one * snap->size[0] * sizeof(float), one))) return rc;
         }
     }
 
     // ---- geometry in the internal 3-dim convention ----
     const int lo_in[3] = {a->x_m, a->y_m, a->z_m};
     const int hi_in[3] = {a->x_M, a->y_M, a->z_M};
-    p.tsize = u.size[0];
+    p.tsize = u->size[0];
     p.so = so;
     if (nd == 3) {
         for (int d = 0; d < 3; ++d) {
-            p.a[d] = u.size[d + 1];
+            p.a[d] = u->size[d + 1];
             p.n[d] = hi_in[d] - lo_in[d] + 1;
             p.o[d] = lo_in[d] + so;
             p.radius[d] = a->radius;
@@ -616,74 +505,67 @@ extern "C" int b2_iso_forward(const struct b2_iso_args *a) {
     } else {
         p.a[0] = 1; p.n[0] = 1; p.o[0] = 0; p.radius[0] = 0;
         for (int d = 0; d < 2; ++d) {
-            p.a[d + 1] = u.size[d + 1];
+            p.a[d + 1] = u->size[d + 1];
             p.n[d + 1] = hi_in[d] - lo_in[d] + 1;
             p.o[d + 1] = lo_in[d] + so;
             p.radius[d + 1] = a->radius;
         }
     }
     for (int d = 0; d < 3; ++d) {
-        if (p.n[d] <= 0) return cleanup(B2_OK);
+        if (p.n[d] <= 0) return B2_OK;
         const int rd = p.radius[d];
         if (p.o[d] - rd < 0 || p.o[d] + p.n[d] - 1 + rd >= p.a[d]) {
             set_error("b2_iso_forward: iteration range [%d,%d] + radius %d leaves the allocated "
                       "array (extent %d) on dim %d", lo_in[nd == 3 ? d : d - 1], hi_in[nd == 3 ? d : d - 1],
                       rd, p.a[d], d);
-            return cleanup(B2_ERR_INVALID);
+            return B2_ERR_INVALID;
         }
     }
     p.sy = p.a[2];
     p.sx = (long long)p.a[1] * p.a[2];
     p.slot_elems = (size_t)p.a[0] * p.a[1] * p.a[2];
-    p.u = (float *)u.d;
-    p.damp = a->damp ? (const float *)damp.d : nullptr;
-    p.param = a->param_kind != B2_PARAM_SCALAR ? (const float *)param.d : nullptr;
+    p.u = (float *)u->d;
+    p.damp = damp ? (const float *)damp->d : nullptr;
+    p.param = param ? (const float *)param->d : nullptr;
     p.param_kind = a->param_kind;
     p.vp = a->vp;
     p.dt = a->dt;
     for (int d = 0; d < nd; ++d) {
         const int di = nd == 3 ? d : d + 1;
-        if (!a->w[d]) { set_error("b2_iso_forward: weights for dim %d missing", d); return cleanup(B2_ERR_INVALID); }
+        if (!a->w[d]) { set_error("b2_iso_forward: weights for dim %d missing", d); return B2_ERR_INVALID; }
         for (int i = 0; i <= a->radius; ++i) p.w[di][i] = a->w[d][i];
     }
     p.ot4 = a->ot4 != 0;
     if (p.ot4 && (a->free_surface || a->grad)) {
         set_error("b2_iso_forward: OT4 is not combined with a free surface or the imaging condition in this version");
-        return cleanup(B2_ERR_INVALID);
+        return B2_ERR_INVALID;
     }
     p.defer_coef = maybe_stream || host_io;       // the arrays are not on the device yet
-    if ((rc = iso_plan_init(p, a->kernel))) return cleanup(rc);
-    const bool damp_io = staged_damp && (damp.owned || (host_io && a->damp->dmap && a->damp->data));
-    const bool param_io = staged_param && (param.owned || (host_io && a->param->dmap && a->param->data));
-    const bool streamed = maybe_stream && streamed_wanted(a, p, u, host_io);
+    if ((rc = iso_plan_init(p, a->kernel))) return rc;
+    const bool damp_io = damp && (damp->owned || (host_io && a->damp->dmap && a->damp->data));
+    const bool param_io = param && (param->owned || (host_io && a->param->dmap && a->param->data));
+    const bool streamed = maybe_stream && streamed_wanted(a, p, *u, host_io);
     if ((maybe_stream || host_io) && !streamed) {
         // not streaming after all: the classic order — whole arrays in, tabulate, loop, whole arrays out
-        DevArray *arrs[3] = {&u, damp_io ? &damp : nullptr, param_io ? &param : nullptr};
+        DevArray *arrs[3] = {u, damp_io ? damp : nullptr, param_io ? param : nullptr};
         for (DevArray *x : arrs)
             if (x && (x->owned || host_io))
                 if (cudaMemcpyAsync(x->d, x->h, x->nbytes, cudaMemcpyHostToDevice, stream()) != cudaSuccess) {
                     set_error("b2_iso_forward: host -> device copy failed");
-                    return cleanup(B2_ERR_MEMORY);
+                    return B2_ERR_MEMORY;
                 }
         p.defer_coef = false;
-        if (p.use_tma && (rc = iso_coef_tabulate_planes(p, 0, p.a[0]))) return cleanup(rc);
+        if (p.use_tma && (rc = iso_coef_tabulate_planes(p, 0, p.a[0]))) return rc;
     }
     // Born: a second plan for the linearised field (same geometry and coefficient tables, own tensor maps)
     IsoPlan pU = p;
-    int dmh = 0;
     if (born) {
-        pU.u = (float *)bornU.d;
-        if ((rc = iso_plan_init(pU, a->kernel))) return cleanup(rc);
-        dmh = a->born_dm->hsize ? a->born_dm->hsize[0] : (borndm.size[0] - (u.size[1] - 2 * so)) / 2;
-        for (int d = 0; d < 3; ++d)
-            if (borndm.size[d] != u.size[d + 1] - 2 * so + 2 * dmh) {
-                set_error("b2_iso_forward: born_dm extent %d on dim %d does not match the grid", borndm.size[d], d);
-                return cleanup(B2_ERR_INVALID);
-            }
+        pU.u = (float *)bornU->d;
+        if ((rc = iso_plan_init(pU, a->kernel))) return rc;
     }
     if (a->free_surface && p.o[2] != so) {
         set_error("b2_iso_forward: a free surface needs the vertical iteration to start at 0");
-        return cleanup(B2_ERR_INVALID);
+        return B2_ERR_INVALID;
     }
 
     g.sx = p.sx;
@@ -720,149 +602,135 @@ extern "C" int b2_iso_forward(const struct b2_iso_args *a) {
     // (free-surface rows are redone after the sweep and Born steps a second field: those use the copy path)
     const bool fused = p2p && halo_fused_ok(a->halo, p) && !a->free_surface && !born;
     IsoFuse fz;
-    if (fused && (rc = halo_fuse_desc(a->halo, p, fz))) return cleanup(rc);
+    if (fused && (rc = halo_fuse_desc(a->halo, p, fz))) return rc;
     if (a->halo && nd == 3 && (a->x_m != 0 || a->x_M != p.a[0] - 2 * so - 1)) {
         set_error("b2_iso_forward: the decomposed dimension must be iterated over the whole slab "
                   "(x_m=%d, x_M=%d, %d owned planes)", a->x_m, a->x_M, p.a[0] - 2 * so);
-        return cleanup(B2_ERR_INVALID);
+        return B2_ERR_INVALID;
     }
     if (a->halo) a->halo->reset_primed();           // first step of a call exchanges through NCCL
     const int dir = a->adjoint ? -1 : 1;
     // profile: [0] staging issued before the loop, [1] the loop (device clock)
     cudaEventRecord(ev_prof[0], stream());
     if (streamed) {
-        if ((rc = iso_forward_streamed(a, p, g, u, staged_damp ? &damp : nullptr, staged_param ? &param : nullptr, src, rec,
-                                       scalar_scale, dt2, damp_io, param_io)))
-            return cleanup(rc);
-        u_is_home = true;
+        if ((rc = iso_forward_streamed(a, p, g, *u, damp, param, src, rec, scalar_scale, dt2, damp_io, param_io)))
+            return rc;
+        u->written = false;                       // the loop has brought u home
         g_last_profile[4] = 1.0;
     }
     if (!streamed)
     for (int time = a->adjoint ? a->time_M : a->time_m; a->adjoint ? time >= a->time_m : time <= a->time_M;
          time += dir) {
-        const int t0 = ((time % T) + T) % T;
-        const int t1 = (((time + dir) % T) + T) % T;     // written
-        const int t2 = (((time - dir) % T) + T) % T;     // the other time level read
+        const int t0 = slot(time, T);
+        const int t1 = slot(time + dir, T);     // written
+        const int t2 = slot(time - dir, T);     // the other time level read
         const bool per_step_events = timing && (step_index++ % sample_stride == 0) && se.used + 4 <= 16384;
         if (per_step_events) { se.next(); ++nsampled; }
         if (fused) {
-            if ((rc = halo_step_iso_fused(a->halo, p, t0, t2, t1))) return cleanup(rc);
+            if ((rc = halo_step_iso_fused(a->halo, p, t0, t2, t1))) return rc;
             // the injection below must reach the copies of my boundary planes in the neighbours' halos
             g.peer_lo = fz.peer_lo; g.peer_hi = fz.peer_hi;
             g.off_lo = (long long)t1 * fz.slot_lo + (long long)(p.o[0] + fz.n_lo) * p.sx;
             g.off_hi = (long long)t1 * fz.slot_hi + (long long)(p.o[0] - p.n[0]) * p.sx;
             g.nown = p.n[0]; g.pw = p.radius[0];
         } else if (a->halo) {
-            if ((rc = halo_exchange_and_step_iso(a->halo, p, t0, t2, t1))) return cleanup(rc);
+            if ((rc = halo_exchange_and_step_iso(a->halo, p, t0, t2, t1))) return rc;
         } else {
-            if ((rc = iso_step(p, t0, t2, t1, 0, p.n[0]))) return cleanup(rc);
+            if ((rc = iso_step(p, t0, t2, t1, 0, p.n[0]))) return rc;
         }
-        if (a->free_surface && (rc = iso_fs_fix(p, t0, t2, t1, 0, p.n[0]))) return cleanup(rc);
+        if (a->free_surface && (rc = iso_fs_fix(p, t0, t2, t1, 0, p.n[0]))) return rc;
         if (per_step_events) se.next();
         float *f1 = p.u + (size_t)t1 * p.slot_elems;
         if ((rc = launch_inject(src, g, f1, nullptr, time, p.param_kind, p.param, scalar_scale, dt2)))
-            return cleanup(rc);
+            return rc;
         if (fused) {
             // the sweep stored the boundary planes, the injection patched them: release the flags
-            if ((rc = halo_fused_signal(a->halo, p.u))) return cleanup(rc);
-            if (a->rec_toff && rec.present && (rc = halo_p2p_wait(a->halo))) return cleanup(rc);
+            if ((rc = halo_fused_signal(a->halo, p.u))) return rc;
+            if (a->rec_toff && rec.present && (rc = halo_p2p_wait(a->halo))) return rc;
         } else if (p2p) {
             // boundary planes of u[t1] are final: store them into the neighbours' halos, signal
             if ((rc = halo_p2p_publish(a->halo, p.u, nullptr, p.slot_elems, t1, (size_t)p.sx, p.o[0], p.n[0],
                                        halo_width_iso(p))))
-                return cleanup(rc);
+                return rc;
             // receivers that sample the just-written time level may touch halo cells: those
             // arrive with the neighbours' stores of this same step
-            if (a->rec_toff && rec.present && (rc = halo_p2p_wait(a->halo))) return cleanup(rc);
+            if (a->rec_toff && rec.present && (rc = halo_p2p_wait(a->halo))) return rc;
         }
         if (born) {
             // eqn2 of the reference's Born operator comes after the source injection into u[t+1]
             if (a->halo) {
-                if ((rc = halo_exchange_and_step_iso(a->halo, pU, t0, t2, t1))) return cleanup(rc);
+                if ((rc = halo_exchange_and_step_iso(a->halo, pU, t0, t2, t1))) return rc;
             } else if ((rc = iso_step(pU, t0, t2, t1, 0, pU.n[0]))) {
-                return cleanup(rc);
+                return rc;
             }
-            if ((rc = iso_born_source(p, t0, t2, t1, pU.u + (size_t)t1 * p.slot_elems, (const float *)borndm.d,
-                                      (long long)borndm.size[1] * borndm.size[2], borndm.size[2],
+            if ((rc = iso_born_source(p, t0, t2, t1, pU.u + (size_t)t1 * p.slot_elems, (const float *)borndm->d,
+                                      (long long)borndm->size[1] * borndm->size[2], borndm->size[2],
                                       a->x_m + dmh, a->y_m + dmh, a->z_m + dmh)))
-                return cleanup(rc);
+                return rc;
             // the linearised field's boundary planes are final: publish them like u's
             if (a->halo && halo_p2p_active(a->halo, pU.u) &&
                 (rc = halo_p2p_publish(a->halo, pU.u, nullptr, pU.slot_elems, t1, (size_t)pU.sx, pU.o[0], pU.n[0],
                                        halo_width_iso(pU))))
-                return cleanup(rc);
+                return rc;
         }
         if (a->snap && time % a->snap_factor == 0) {
             // internal dims: a 2-D grid is (1, x, y), its snapshots (nsnaps, x, y)
-            const long long ssy = snap.size[nd];
-            const long long ssx = nd == 3 ? (long long)snap.size[2] * snap.size[3] : 0;
-            const size_t one = (size_t)(nd == 3 ? snap.size[1] : 1) * snap.size[nd - 1] * snap.size[nd];
+            const long long ssy = snap->size[nd];
+            const long long ssx = nd == 3 ? (long long)snap->size[2] * snap->size[3] : 0;
+            const size_t one = (size_t)(nd == 3 ? snap->size[1] : 1) * snap->size[nd - 1] * snap->size[nd];
             float *dst = nullptr;
             if (streamer.active) {
-                if ((rc = streamer.acquire(&dst))) return cleanup(rc);
+                if ((rc = streamer.acquire(&dst))) return rc;
             } else {
-                dst = (float *)snap.d + (size_t)(time / a->snap_factor) * one;
+                dst = (float *)snap->d + (size_t)(time / a->snap_factor) * one;
             }
             const int d0 = nd == 3 ? a->x_m + snap_h : 0;
             const int d1 = (nd == 3 ? a->y_m : a->x_m) + snap_h;
             const int d2 = (nd == 3 ? a->z_m : a->y_m) + snap_h;
-            if ((rc = iso_snapshot(p, a->snap_toff ? t1 : t0, dst, ssx, ssy, d0, d1, d2))) return cleanup(rc);
+            if ((rc = iso_snapshot(p, a->snap_toff ? t1 : t0, dst, ssx, ssy, d0, d1, d2))) return rc;
             if (streamer.active) {
                 const int dd[3] = {d0, d1, d2};
-                if ((rc = streamer.release(time / a->snap_factor, &snap.size[1], dd, p.n))) return cleanup(rc);
+                if ((rc = streamer.release(time / a->snap_factor, &snap->size[1], dd, p.n))) return rc;
             }
         }
         if (per_step_events) se.next();
         if (a->halo && !p2p && a->rec_toff && rec.present) {
             // NCCL path: receivers that sample the level just written may reach into the halo, which is only
             // exchanged at the start of the next step -- exchange it now (the peer paths wait on the flags instead)
-            if ((rc = halo_exchange_slot(a->halo, born ? pU : p, t1))) return cleanup(rc);
+            if ((rc = halo_exchange_slot(a->halo, born ? pU : p, t1))) return rc;
         }
         const float *fr = (born ? pU.u : p.u) + (size_t)(a->rec_toff ? t1 : t0) * p.slot_elems;
-        if ((rc = launch_interp(rec, g, fr, nullptr, time))) return cleanup(rc);
-        if (staged_grad) {
-            if (time < 0 || time >= usave.size[0]) {
-                set_error("b2_iso_forward: time=%d outside the saved wavefield (nt=%d)", time, usave.size[0]);
-                return cleanup(B2_ERR_INVALID);
+        if ((rc = launch_interp(rec, g, fr, nullptr, time))) return rc;
+        if (grad) {
+            if (time < 0 || time >= usave->size[0]) {
+                set_error("b2_iso_forward: time=%d outside the saved wavefield (nt=%d)", time, usave->size[0]);
+                return B2_ERR_INVALID;
             }
-            ImgK ik;
-            ik.us2 = ik.w0 = ik.w1 = ik.w2 = nullptr;
-            ik.grad = (float *)grad.d;
-            ik.us = (const float *)usave.d + (size_t)time * p.slot_elems;
-            ik.v0 = p.u + (size_t)t0 * p.slot_elems;
-            ik.v1 = p.u + (size_t)t1 * p.slot_elems;
-            ik.v2 = p.u + (size_t)t2 * p.slot_elems;
-            ik.sx = p.sx; ik.sy = p.sy;
-            ik.gsy = grad.size[2];
-            ik.gsx = (long long)grad.size[1] * grad.size[2];
-            const int gh = a->grad->hsize ? a->grad->hsize[0] : (grad.size[0] - (u.size[1] - 2 * so)) / 2;
-            ik.n0 = p.n[0]; ik.n1 = p.n[1]; ik.n2 = p.n[2];
-            ik.o0 = p.o[0]; ik.o1 = p.o[1]; ik.o2 = p.o[2];
-            ik.g0 = a->x_m + gh; ik.g1 = a->y_m + gh; ik.g2 = a->z_m + gh;
-            ik.inv_dt2 = 1.0f / (a->dt * a->dt);
-            if ((rc = launch_imaging(ik))) return cleanup(rc);
+            if ((rc = launch_imaging(p, *grad, gh, (const float *)usave->d + (size_t)time * p.slot_elems, p.u, nullptr,
+                                     nullptr, t0, t1, t2)))
+                return rc;
         }
         if (per_step_events) se.next();
         if (a->errctl && ((time - a->time_m) % 100 == 99 || time == (a->adjoint ? a->time_m : a->time_M))) {
             bool bad = false;
-            if ((rc = check_finite(f1, p.slot_elems, bad))) return cleanup(rc);
-            if (bad) { set_error("NaN/Inf detected in u at time=%d", time); return cleanup(B2_ERR_NAN); }
+            if ((rc = check_finite(f1, p.slot_elems, bad))) return rc;
+            if (bad) { set_error("NaN/Inf detected in u at time=%d", time); return B2_ERR_NAN; }
         }
     }
-    if (a->halo && (rc = halo_p2p_drain(a->halo))) return cleanup(rc);
+    if (a->halo && (rc = halo_p2p_drain(a->halo))) return rc;
     if (timing) cudaEventRecord(ev_tot[1], stream());
     cudaEventRecord(ev_prof[1], stream());
     if (streamed && a->errctl) {
         bool bad = false;
-        const int tl = (((a->time_M + 1) % T) + T) % T;
-        if ((rc = check_finite(p.u + (size_t)tl * p.slot_elems, p.slot_elems, bad))) return cleanup(rc);
-        if (bad) { set_error("NaN/Inf detected in u at time=%d", a->time_M); return cleanup(B2_ERR_NAN); }
+        const int tl = slot(a->time_M + 1, T);
+        if ((rc = check_finite(p.u + (size_t)tl * p.slot_elems, p.slot_elems, bad))) return rc;
+        if (bad) { set_error("NaN/Inf detected in u at time=%d", a->time_M); return B2_ERR_NAN; }
     }
 
     cudaError_t e = cudaStreamSynchronize(stream());
     if (e != cudaSuccess) {
         set_error("b2_iso_forward: device error: %s", cudaGetErrorString(e));
-        return cleanup(B2_ERR_LAUNCH);
+        return B2_ERR_LAUNCH;
     }
     {
         float ms = 0.f;
@@ -889,5 +757,31 @@ extern "C" int b2_iso_forward(const struct b2_iso_args *a) {
         a->timers->section1 += s1 * 1e-3;
         a->timers->section2 += s2 * 1e-3;
     }
-    return cleanup(B2_OK);
+    return B2_OK;
+}
+
+extern "C" int b2_iso_forward(const struct b2_iso_args *a) {
+    if (!a || !a->u) { set_error("b2_iso_forward: NULL args"); return B2_ERR_INVALID; }
+    if (a->ndim != 2 && a->ndim != 3) { set_error("b2_iso_forward: ndim must be 2 or 3"); return B2_ERR_INVALID; }
+    if (a->radius < 1 || a->radius > B2_MAX_RADIUS || a->radius > a->space_order) {
+        set_error("b2_iso_forward: unsupported radius %d (space_order %d)", a->radius, a->space_order);
+        return B2_ERR_INVALID;
+    }
+    if (a->time_M < a->time_m) return B2_OK;
+    std::lock_guard<std::mutex> api_lock(api_mutex());
+    if (int rc0 = use_device(a->deviceid)) return rc0;
+    note_sweep_kernel("");
+    for (double &v : g_last_profile) v = 0.0;
+    const auto call_t0 = std::chrono::steady_clock::now();
+    Staging st;
+    SnapStreamer streamer;
+    int rc = iso_forward_body(a, st, streamer, call_t0);
+    // profile: [2] the write-back (copies to the host, snapshot drain, release), [3] the whole call; host clock
+    const auto d2h_t0 = std::chrono::steady_clock::now();
+    rc = st.finish(rc);
+    const int rs = streamer.end();
+    const auto t1 = std::chrono::steady_clock::now();
+    g_last_profile[2] = std::chrono::duration<double, std::milli>(t1 - d2h_t0).count();
+    g_last_profile[3] = std::chrono::duration<double, std::milli>(t1 - call_t0).count();
+    return rc ? rc : rs;
 }

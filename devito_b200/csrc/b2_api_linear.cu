@@ -23,53 +23,29 @@ __global__ void __launch_bounds__(256) k_linear(LinK k) {
 
 }  // namespace b2
 
-extern "C" int b2_linear_forward(const struct b2_linear_args *a) {
-    if (!a || !a->f || !a->taps) { set_error("b2_linear_forward: NULL args"); return B2_ERR_INVALID; }
-    if (a->ndim < 1 || a->ndim > 3) { set_error("b2_linear_forward: ndim must be 1..3"); return B2_ERR_INVALID; }
-    if (a->ntaps < 1 || a->ntaps > B2_MAX_TAPS) {
-        set_error("b2_linear_forward: %d taps (1..%d supported)", a->ntaps, B2_MAX_TAPS);
-        return B2_ERR_INVALID;
-    }
-    if (a->wshift != 1 && a->wshift != -1) { set_error("b2_linear_forward: wshift must be +1 or -1"); return B2_ERR_INVALID; }
-    if (a->time_M < a->time_m) return B2_OK;
-    std::lock_guard<std::mutex> api_lock(api_mutex());
-    if (int rc0 = use_device(a->deviceid)) return rc0;
-
-    const int nd = a->ndim, h = a->halo;
-    DevArray f;
-    int rc = stage_in(a->f, nd + 1, f, true);
+static int linear_forward_body(const b2_linear_args *a, Staging &st) {
+    const int nd = a->ndim;
+    DevArray *f;
+    int rc = st.array(a->f, nd + 1, true, f);
     if (rc) return rc;
-    auto cleanup = [&](int code) {
-        const int r = stage_out(f, code == B2_OK);
-        return code != B2_OK ? code : r;
-    };
-    // internal 3-dim convention: leading dummy dims of extent 1 for 1-D / 2-D fields
-    int alloc[3] = {1, 1, 1}, lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0}, hal[3] = {0, 0, 0};
-    const int lo_in[3] = {a->x_m, a->y_m, a->z_m}, hi_in[3] = {a->x_M, a->y_M, a->z_M};
-    for (int d = 0; d < nd; ++d) {
-        const int di = 3 - nd + d;
-        alloc[di] = f.size[d + 1];
-        lo[di] = lo_in[d];
-        hi[di] = hi_in[d];
-        hal[di] = h;
-    }
-    const int T = f.size[0];
+    const Box3 b = box3(a, nd, &f->size[1], a->halo);
+    const int T = f->size[0];
     LinK k;
-    k.sy = alloc[2];
-    k.sx = (long long)alloc[1] * alloc[2];
-    const size_t slot = (size_t)alloc[0] * alloc[1] * alloc[2];
-    k.n0 = hi[0] - lo[0] + 1; k.n1 = hi[1] - lo[1] + 1; k.n2 = hi[2] - lo[2] + 1;
-    k.o0 = lo[0] + hal[0]; k.o1 = lo[1] + hal[1]; k.o2 = lo[2] + hal[2];
-    if (k.n0 <= 0 || k.n1 <= 0 || k.n2 <= 0) return cleanup(B2_OK);
+    k.sy = b.alloc[2];
+    k.sx = (long long)b.alloc[1] * b.alloc[2];
+    const size_t slot_len = (size_t)b.alloc[0] * b.alloc[1] * b.alloc[2];
+    k.n0 = b.hi[0] - b.lo[0] + 1; k.n1 = b.hi[1] - b.lo[1] + 1; k.n2 = b.hi[2] - b.lo[2] + 1;
+    k.o0 = b.lo[0] + b.hal[0]; k.o1 = b.lo[1] + b.hal[1]; k.o2 = b.lo[2] + b.hal[2];
+    if (k.n0 <= 0 || k.n1 <= 0 || k.n2 <= 0) return B2_OK;
     k.ntaps = a->ntaps;
     int shifts[4], nshift = 0;
     for (int i = 0; i < a->ntaps; ++i) {
         const b2_tap &t = a->taps[i];
-        if (t.tshift == a->wshift) { set_error("b2_linear_forward: a tap reads the level being written"); return cleanup(B2_ERR_INVALID); }
+        if (t.tshift == a->wshift) { set_error("b2_linear_forward: a tap reads the level being written"); return B2_ERR_INVALID; }
         int s = -1;
         for (int j = 0; j < nshift; ++j) if (shifts[j] == t.tshift) s = j;
         if (s < 0) {
-            if (nshift == 4) { set_error("b2_linear_forward: more than 4 time levels read"); return cleanup(B2_ERR_INVALID); }
+            if (nshift == 4) { set_error("b2_linear_forward: more than 4 time levels read"); return B2_ERR_INVALID; }
             shifts[nshift] = t.tshift;
             s = nshift++;
         }
@@ -78,9 +54,9 @@ extern "C" int b2_linear_forward(const struct b2_linear_args *a) {
         for (int d = 0; d < nd; ++d) {
             const int di = 3 - nd + d, o = t.off[d];
             // the read must stay inside the allocated array
-            if (lo[di] + hal[di] + o < 0 || hi[di] + hal[di] + o >= alloc[di]) {
+            if (b.lo[di] + b.hal[di] + o < 0 || b.hi[di] + b.hal[di] + o >= b.alloc[di]) {
                 set_error("b2_linear_forward: tap offset %d on dim %d leaves the allocated array", o, d);
-                return cleanup(B2_ERR_INVALID);
+                return B2_ERR_INVALID;
             }
             delta += (long long)o * (di == 0 ? k.sx : di == 1 ? k.sy : 1);
         }
@@ -89,7 +65,7 @@ extern "C" int b2_linear_forward(const struct b2_linear_args *a) {
     }
     if (T <= nshift) {   // every level read and the one written must be distinct slots
         set_error("b2_linear_forward: %d time slots cannot hold %d levels", T, nshift + 1);
-        return cleanup(B2_ERR_INVALID);
+        return B2_ERR_INVALID;
     }
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (a->timers) {
@@ -99,14 +75,13 @@ extern "C" int b2_linear_forward(const struct b2_linear_args *a) {
     }
     dim3 block(64, 4, 1);
     dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
-    float *base = (float *)f.d;
-    auto slot_of = [&](int time, int shift) { return (((time + shift) % T) + T) % T; };
+    float *base = (float *)f->d;
     // an update of `f.backward` (wshift = -1) runs from time_M down to time_m, like the reference's
     // backward-in-time loop (devito/ir/support/space.py: Backward direction)
     const int dirn = a->wshift;
     for (int time = dirn > 0 ? a->time_m : a->time_M; dirn > 0 ? time <= a->time_M : time >= a->time_m; time += dirn) {
-        k.out = base + (size_t)slot_of(time, a->wshift) * slot;
-        for (int j = 0; j < nshift; ++j) k.lvl[j] = base + (size_t)slot_of(time, shifts[j]) * slot;
+        k.out = base + (size_t)slot(time + a->wshift, T) * slot_len;
+        for (int j = 0; j < nshift; ++j) k.lvl[j] = base + (size_t)slot(time + shifts[j], T) * slot_len;
         for (int j = nshift; j < 4; ++j) k.lvl[j] = k.lvl[0];
         k_linear<<<grid, block, 0, stream()>>>(k);
         count_launch();
@@ -120,6 +95,21 @@ extern "C" int b2_linear_forward(const struct b2_linear_args *a) {
         cudaEventDestroy(e0);
         cudaEventDestroy(e1);
     }
-    if (e != cudaSuccess) { set_error("b2_linear_forward: %s", cudaGetErrorString(e)); return cleanup(B2_ERR_LAUNCH); }
-    return cleanup(B2_OK);
+    if (e != cudaSuccess) { set_error("b2_linear_forward: %s", cudaGetErrorString(e)); return B2_ERR_LAUNCH; }
+    return B2_OK;
+}
+
+extern "C" int b2_linear_forward(const struct b2_linear_args *a) {
+    if (!a || !a->f || !a->taps) { set_error("b2_linear_forward: NULL args"); return B2_ERR_INVALID; }
+    if (a->ndim < 1 || a->ndim > 3) { set_error("b2_linear_forward: ndim must be 1..3"); return B2_ERR_INVALID; }
+    if (a->ntaps < 1 || a->ntaps > B2_MAX_TAPS) {
+        set_error("b2_linear_forward: %d taps (1..%d supported)", a->ntaps, B2_MAX_TAPS);
+        return B2_ERR_INVALID;
+    }
+    if (a->wshift != 1 && a->wshift != -1) { set_error("b2_linear_forward: wshift must be +1 or -1"); return B2_ERR_INVALID; }
+    if (a->time_M < a->time_m) return B2_OK;
+    std::lock_guard<std::mutex> api_lock(api_mutex());
+    if (int rc0 = use_device(a->deviceid)) return rc0;
+    Staging st;
+    return st.finish(linear_forward_body(a, st));
 }

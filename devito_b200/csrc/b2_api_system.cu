@@ -49,6 +49,175 @@ __global__ void __launch_bounds__(256) k_system_stage(const __grid_constant__ Sy
 
 }  // namespace b2
 
+static int system_forward_body(const b2_system_args *a, Staging &staging) {
+    const int nd = a->ndim, h = a->halo;
+    std::vector<DevArray *> F(a->nfields), C(a->ncoefs), injp(a->ninject, nullptr);
+    std::vector<SparseDev> inj(a->ninject), itp(a->ninterp);
+    int rc = B2_OK;
+    for (int i = 0; i < a->nfields; ++i) {
+        if ((rc = staging.array(a->fields[i], nd + 1, true, F[i]))) return rc;
+        if (F[i]->size[0] < 1) { set_error("b2_system_forward: field %d has no time slot", i); return B2_ERR_INVALID; }
+        for (int d = 1; d <= nd; ++d)
+            if (F[i]->size[d] != F[0]->size[d]) { set_error("b2_system_forward: field %d has another shape", i); return B2_ERR_INVALID; }
+    }
+    const Box3 b = box3(a, nd, &F[0]->size[1], h);
+    const int *alloc = b.alloc, *lo = b.lo, *hi = b.hi, *hal = b.hal;
+    int calloc_[3] = {1, 1, 1};
+    for (int i = 0; i < a->ncoefs; ++i) {
+        if ((rc = staging.array(a->coefs[i], nd, false, C[i]))) return rc;
+        for (int d = 0; d < nd; ++d) {
+            const int di = 3 - nd + d;
+            if (i == 0) calloc_[di] = C[i]->size[d];
+            if (C[i]->size[d] != calloc_[di] || C[i]->size[d] != alloc[di] - 2 * hal[di]) {
+                set_error("b2_system_forward: coefficient array %d does not have the grid's shape", i);
+                return B2_ERR_INVALID;
+            }
+        }
+    }
+    for (int i = 0; i < a->ninject; ++i) {
+        if ((rc = sparse_stage_in(staging, a->inject[i].s, nd, false, inj[i]))) return rc;
+        if (a->inject[i].param_kind != B2_PARAM_SCALAR) {
+            if (!a->inject[i].param) { set_error("b2_system_forward: injection %d lacks its parameter array", i); return B2_ERR_INVALID; }
+            if ((rc = staging.array(a->inject[i].param, nd, false, injp[i]))) return rc;
+            for (int d = 0; d < nd; ++d)
+                if (injp[i]->size[d] != F[0]->size[d + 1]) {
+                    set_error("b2_system_forward: the parameter array of injection %d does not have the fields' layout", i);
+                    return B2_ERR_INVALID;
+                }
+        }
+    }
+    for (int i = 0; i < a->ninterp; ++i)
+        if ((rc = sparse_stage_in(staging, a->interp[i].s, nd, true, itp[i]))) return rc;
+
+    SysK k;
+    k.sy = alloc[2];
+    k.sx = (long long)alloc[1] * alloc[2];
+    k.csy = calloc_[2];
+    k.csx = (long long)calloc_[1] * calloc_[2];
+    const size_t slot_len = (size_t)alloc[0] * alloc[1] * alloc[2];
+    if (hi[0] < lo[0] || hi[1] < lo[1] || hi[2] < lo[2]) return B2_OK;
+    for (int i = 0; i < a->ncoefs; ++i) k.cf[i] = (const float *)C[i]->d;
+    for (int i = a->ncoefs; i < B2_SYS_MAX_COEFS; ++i) k.cf[i] = nullptr;
+    auto slot_of = [&](int f, int time, int shift) { return slot(time + shift, F[f]->size[0]); };
+
+    // validate the stages once
+    for (int s = 0; s < a->nstages; ++s) {
+        const b2_sys_stage &st = a->stages[s];
+        if (st.out_field < 0 || st.out_field >= a->nfields || st.ntaps < 1 || st.ntaps > B2_SYS_MAX_TAPS || !st.taps ||
+            st.ext < 0 || st.ext > h) {
+            set_error("b2_system_forward: stage %d is malformed (%d taps, at most %d; box widened by %d, at most %d)", s,
+                      st.ntaps, B2_SYS_MAX_TAPS, st.ext, h);
+            return B2_ERR_INVALID;
+        }
+        for (int i = 0; i < st.ntaps; ++i) {
+            const b2_sys_tap &t = st.taps[i];
+            if (t.field < 0 || t.field >= a->nfields || t.tshift < 0 || t.tshift > 1 || t.cfield >= a->ncoefs ||
+                (st.ext > 0 && t.cfield >= 0)) {
+                set_error("b2_system_forward: stage %d tap %d is malformed", s, i);
+                return B2_ERR_INVALID;
+            }
+            // the kernel reads and writes in place: a shifted read of the written level would race with the writes
+            if (t.field == st.out_field && slot_of(t.field, 0, t.tshift) == slot_of(t.field, 0, st.out_tshift) &&
+                (t.off[0] || t.off[1] || t.off[2])) {
+                set_error("b2_system_forward: stage %d reads shifted points of the level it writes", s);
+                return B2_ERR_INVALID;
+            }
+            for (int d = 0; d < nd; ++d) {
+                const int di = 3 - nd + d;
+                if (lo[di] - st.ext + hal[di] + t.off[d] < 0 || hi[di] + st.ext + hal[di] + t.off[d] >= alloc[di]) {
+                    set_error("b2_system_forward: stage %d tap offset %d on dim %d leaves the allocated array", s, t.off[d], d);
+                    return B2_ERR_INVALID;
+                }
+            }
+        }
+    }
+    FieldGeom g;
+    g.sx = k.sx; g.sy = k.sy; g.slot_elems = slot_len; g.so = h; g.ndim = nd;
+    for (int d = 0; d < nd; ++d) { g.lo[d] = lo[3 - nd + d]; g.hi[d] = hi[3 - nd + d]; }
+
+    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    double sec[3] = {0, 0, 0};
+    const bool timing = a->timers != nullptr;
+    if (timing) for (auto &e : ev) cudaEventCreate(&e);
+    dim3 block(64, 4, 1);
+    const int nsteps = a->time_M - a->time_m + 1;
+    const bool per_step = timing && nsteps <= 2048;
+    std::vector<cudaEvent_t> pool;
+    auto rec_ev = [&]() { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, stream()); pool.push_back(e); };
+    if (timing && !per_step) cudaEventRecord(ev[0], stream());
+    for (int time = a->time_m; time <= a->time_M; ++time) {
+        if (per_step) rec_ev();
+        for (int s = 0; s < a->nstages; ++s) {
+            const b2_sys_stage &st = a->stages[s];
+            // the box, widened by ext on the space axes (internal axis 0 of a 2-D grid is the dummy extent 1)
+            const int e0 = nd == 3 ? st.ext : 0, e = st.ext;
+            k.n0 = hi[0] - lo[0] + 1 + 2 * e0; k.n1 = hi[1] - lo[1] + 1 + 2 * e; k.n2 = hi[2] - lo[2] + 1 + 2 * e;
+            k.o0 = lo[0] - e0 + hal[0]; k.o1 = lo[1] - e + hal[1]; k.o2 = lo[2] - e + hal[2];
+            k.c0 = lo[0] - e0; k.c1 = lo[1] - e; k.c2 = lo[2] - e;       // unused when e > 0 (no cfield)
+            const dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
+            k.out = (float *)F[st.out_field]->d + (size_t)slot_of(st.out_field, time, st.out_tshift) * slot_len;
+            for (int f = 0; f < a->nfields; ++f)
+                for (int t = 0; t < 2; ++t)
+                    k.in[f][t] = (const float *)F[f]->d + (size_t)slot_of(f, time, t) * slot_len;
+            k.ntaps = st.ntaps;
+            for (int i = 0; i < st.ntaps; ++i) {
+                const b2_sys_tap &t = st.taps[i];
+                long long delta = 0;
+                for (int d = 0; d < nd; ++d) {
+                    const int di = 3 - nd + d;
+                    delta += (long long)t.off[d] * (di == 0 ? k.sx : di == 1 ? k.sy : 1);
+                }
+                k.fld[i] = (short)t.field; k.tsh[i] = (short)t.tshift; k.cfi[i] = (short)t.cfield;
+                k.delta[i] = (int)delta; k.coef[i] = t.coef;
+            }
+            k_system_stage<<<grid, block, 0, stream()>>>(k);
+            count_launch();
+        }
+        if (per_step) rec_ev();
+        for (int i = 0; i < a->ninject; ++i) {
+            const b2_sys_inject &q = a->inject[i];
+            float *f0 = (float *)F[q.fields[0]]->d + (size_t)slot_of(q.fields[0], time, q.tshift) * slot_len;
+            float *f1 = q.nfields > 1 ? (float *)F[q.fields[1]]->d + (size_t)slot_of(q.fields[1], time, q.tshift) * slot_len : nullptr;
+            // scale modes of k_inject: scalar | dt2 * param^2 | dt2 / param with dt2 := q.scale
+            const float *prm = q.param_kind != B2_PARAM_SCALAR ? (const float *)injp[i]->d : nullptr;
+            if ((rc = launch_inject(inj[i], g, f0, f1, time, q.param_kind, prm, q.scale, q.scale))) return rc;
+            if (q.nfields > 2) {
+                float *f2 = (float *)F[q.fields[2]]->d + (size_t)slot_of(q.fields[2], time, q.tshift) * slot_len;
+                if ((rc = launch_inject(inj[i], g, f2, nullptr, time, q.param_kind, prm, q.scale, q.scale))) return rc;
+            }
+        }
+        if (per_step) rec_ev();
+        for (int i = 0; i < a->ninterp; ++i) {
+            const b2_sys_interp &q = a->interp[i];
+            const float *f = (const float *)F[q.field]->d + (size_t)slot_of(q.field, time, q.tshift) * slot_len;
+            if ((rc = launch_interp(itp[i], g, f, nullptr, time))) return rc;
+        }
+        if (per_step) rec_ev();
+    }
+    if (timing && !per_step) cudaEventRecord(ev[1], stream());
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream());
+    if (timing) {
+        float ms = 0.f;
+        if (per_step) {
+            for (size_t i = 0; i + 3 < pool.size(); i += 4) {
+                if (cudaEventElapsedTime(&ms, pool[i], pool[i + 1]) == cudaSuccess) sec[0] += ms;
+                if (cudaEventElapsedTime(&ms, pool[i + 1], pool[i + 2]) == cudaSuccess) sec[1] += ms;
+                if (cudaEventElapsedTime(&ms, pool[i + 2], pool[i + 3]) == cudaSuccess) sec[2] += ms;
+            }
+        } else if (e == cudaSuccess && cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) {
+            sec[0] = ms;
+        }
+        a->timers->section0 += sec[0] * 1e-3;
+        a->timers->section1 += sec[1] * 1e-3;
+        a->timers->section2 += sec[2] * 1e-3;
+        for (auto &x : ev) cudaEventDestroy(x);
+        for (auto &x : pool) cudaEventDestroy(x);
+    }
+    if (e != cudaSuccess) { set_error("b2_system_forward: %s", cudaGetErrorString(e)); return B2_ERR_LAUNCH; }
+    return B2_OK;
+}
+
 extern "C" int b2_system_forward(const struct b2_system_args *a) {
     if (!a || !a->fields || !a->stages) { set_error("b2_system_forward: NULL args"); return B2_ERR_INVALID; }
     if (a->ndim != 2 && a->ndim != 3) { set_error("b2_system_forward: ndim must be 2 or 3"); return B2_ERR_INVALID; }
@@ -76,197 +245,6 @@ extern "C" int b2_system_forward(const struct b2_system_args *a) {
     if (a->time_M < a->time_m) return B2_OK;
     std::lock_guard<std::mutex> api_lock(api_mutex());
     if (int rc0 = use_device(a->deviceid)) return rc0;
-
-    const int nd = a->ndim, h = a->halo;
-    std::vector<DevArray> F(a->nfields), C(a->ncoefs);
-    std::vector<SparseDev> inj(a->ninject), itp(a->ninterp);
-    std::vector<DevArray> injp(a->ninject);
-    std::vector<char> injp_staged(a->ninject, 0);
-    int staged_f = 0, staged_c = 0;
-    int rc = B2_OK;
-    auto cleanup = [&](int code) {
-        int r = B2_OK;
-        for (int i = 0; i < staged_f; ++i) { const int q = stage_out(F[i], code == B2_OK); if (!r) r = q; }
-        for (int i = 0; i < staged_c; ++i) stage_out(C[i], false);
-        for (auto &s : inj) sparse_stage_out(s, false);
-        for (size_t i = 0; i < injp.size(); ++i) if (injp_staged[i]) stage_out(injp[i], false);
-        for (auto &s : itp) { const int q = sparse_stage_out(s, code == B2_OK); if (!r) r = q; }
-        return code != B2_OK ? code : r;
-    };
-    for (int i = 0; i < a->nfields; ++i) {
-        if ((rc = stage_in(a->fields[i], nd + 1, F[i], true))) return cleanup(rc);
-        ++staged_f;
-        if (F[i].size[0] < 1) { set_error("b2_system_forward: field %d has no time slot", i); return cleanup(B2_ERR_INVALID); }
-        for (int d = 1; d <= nd; ++d)
-            if (F[i].size[d] != F[0].size[d]) { set_error("b2_system_forward: field %d has another shape", i); return cleanup(B2_ERR_INVALID); }
-    }
-    // internal 3-dim convention (a 2-D grid is (1, x, y))
-    int alloc[3] = {1, 1, 1}, lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0}, hal[3] = {0, 0, 0};
-    const int lo_in[3] = {a->x_m, a->y_m, a->z_m}, hi_in[3] = {a->x_M, a->y_M, a->z_M};
-    for (int d = 0; d < nd; ++d) {
-        const int di = 3 - nd + d;
-        alloc[di] = F[0].size[d + 1];
-        lo[di] = lo_in[d];
-        hi[di] = hi_in[d];
-        hal[di] = h;
-    }
-    int calloc_[3] = {1, 1, 1};
-    for (int i = 0; i < a->ncoefs; ++i) {
-        if ((rc = stage_in(a->coefs[i], nd, C[i], true))) return cleanup(rc);
-        ++staged_c;
-        for (int d = 0; d < nd; ++d) {
-            const int di = 3 - nd + d;
-            if (i == 0) calloc_[di] = C[i].size[d];
-            if (C[i].size[d] != calloc_[di] || C[i].size[d] != alloc[di] - 2 * hal[di]) {
-                set_error("b2_system_forward: coefficient array %d does not have the grid's shape", i);
-                return cleanup(B2_ERR_INVALID);
-            }
-        }
-    }
-    for (int i = 0; i < a->ninject; ++i) {
-        if ((rc = sparse_stage_in(a->inject[i].s, nd, inj[i], true))) return cleanup(rc);
-        if (a->inject[i].param_kind != B2_PARAM_SCALAR) {
-            if (!a->inject[i].param) { set_error("b2_system_forward: injection %d lacks its parameter array", i); return cleanup(B2_ERR_INVALID); }
-            if ((rc = stage_in(a->inject[i].param, nd, injp[i], true))) return cleanup(rc);
-            injp_staged[i] = 1;
-            for (int d = 0; d < nd; ++d)
-                if (injp[i].size[d] != F[0].size[d + 1]) {
-                    set_error("b2_system_forward: the parameter array of injection %d does not have the fields' layout", i);
-                    return cleanup(B2_ERR_INVALID);
-                }
-        }
-    }
-    for (int i = 0; i < a->ninterp; ++i)
-        if ((rc = sparse_stage_in(a->interp[i].s, nd, itp[i], true))) return cleanup(rc);
-
-    SysK k;
-    k.sy = alloc[2];
-    k.sx = (long long)alloc[1] * alloc[2];
-    k.csy = calloc_[2];
-    k.csx = (long long)calloc_[1] * calloc_[2];
-    const size_t slot = (size_t)alloc[0] * alloc[1] * alloc[2];
-    if (hi[0] < lo[0] || hi[1] < lo[1] || hi[2] < lo[2]) return cleanup(B2_OK);
-    for (int i = 0; i < a->ncoefs; ++i) k.cf[i] = (const float *)C[i].d;
-    for (int i = a->ncoefs; i < B2_SYS_MAX_COEFS; ++i) k.cf[i] = nullptr;
-    auto slot_of = [&](int f, int time, int shift) {
-        const int T = F[f].size[0];
-        return (((time + shift) % T) + T) % T;
-    };
-
-    // validate the stages once
-    for (int s = 0; s < a->nstages; ++s) {
-        const b2_sys_stage &st = a->stages[s];
-        if (st.out_field < 0 || st.out_field >= a->nfields || st.ntaps < 1 || st.ntaps > B2_SYS_MAX_TAPS || !st.taps ||
-            st.ext < 0 || st.ext > h) {
-            set_error("b2_system_forward: stage %d is malformed (%d taps, at most %d; box widened by %d, at most %d)", s,
-                      st.ntaps, B2_SYS_MAX_TAPS, st.ext, h);
-            return cleanup(B2_ERR_INVALID);
-        }
-        for (int i = 0; i < st.ntaps; ++i) {
-            const b2_sys_tap &t = st.taps[i];
-            if (t.field < 0 || t.field >= a->nfields || t.tshift < 0 || t.tshift > 1 || t.cfield >= a->ncoefs ||
-                (st.ext > 0 && t.cfield >= 0)) {
-                set_error("b2_system_forward: stage %d tap %d is malformed", s, i);
-                return cleanup(B2_ERR_INVALID);
-            }
-            // the kernel reads and writes in place: a shifted read of the written level would race with the writes
-            if (t.field == st.out_field && slot_of(t.field, 0, t.tshift) == slot_of(t.field, 0, st.out_tshift) &&
-                (t.off[0] || t.off[1] || t.off[2])) {
-                set_error("b2_system_forward: stage %d reads shifted points of the level it writes", s);
-                return cleanup(B2_ERR_INVALID);
-            }
-            for (int d = 0; d < nd; ++d) {
-                const int di = 3 - nd + d;
-                if (lo[di] - st.ext + hal[di] + t.off[d] < 0 || hi[di] + st.ext + hal[di] + t.off[d] >= alloc[di]) {
-                    set_error("b2_system_forward: stage %d tap offset %d on dim %d leaves the allocated array", s, t.off[d], d);
-                    return cleanup(B2_ERR_INVALID);
-                }
-            }
-        }
-    }
-    FieldGeom g;
-    g.sx = k.sx; g.sy = k.sy; g.slot_elems = slot; g.so = h; g.ndim = nd;
-    for (int d = 0; d < nd; ++d) { g.lo[d] = lo_in[d]; g.hi[d] = hi_in[d]; }
-
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    double sec[3] = {0, 0, 0};
-    const bool timing = a->timers != nullptr;
-    if (timing) for (auto &e : ev) cudaEventCreate(&e);
-    dim3 block(64, 4, 1);
-    const int nsteps = a->time_M - a->time_m + 1;
-    const bool per_step = timing && nsteps <= 2048;
-    std::vector<cudaEvent_t> pool;
-    auto rec_ev = [&]() { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, stream()); pool.push_back(e); };
-    if (timing && !per_step) cudaEventRecord(ev[0], stream());
-    for (int time = a->time_m; time <= a->time_M; ++time) {
-        if (per_step) rec_ev();
-        for (int s = 0; s < a->nstages; ++s) {
-            const b2_sys_stage &st = a->stages[s];
-            // the box, widened by ext on the space axes (internal axis 0 of a 2-D grid is the dummy extent 1)
-            const int e0 = nd == 3 ? st.ext : 0, e = st.ext;
-            k.n0 = hi[0] - lo[0] + 1 + 2 * e0; k.n1 = hi[1] - lo[1] + 1 + 2 * e; k.n2 = hi[2] - lo[2] + 1 + 2 * e;
-            k.o0 = lo[0] - e0 + hal[0]; k.o1 = lo[1] - e + hal[1]; k.o2 = lo[2] - e + hal[2];
-            k.c0 = lo[0] - e0; k.c1 = lo[1] - e; k.c2 = lo[2] - e;       // unused when e > 0 (no cfield)
-            const dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
-            k.out = (float *)F[st.out_field].d + (size_t)slot_of(st.out_field, time, st.out_tshift) * slot;
-            for (int f = 0; f < a->nfields; ++f)
-                for (int t = 0; t < 2; ++t)
-                    k.in[f][t] = (const float *)F[f].d + (size_t)slot_of(f, time, t) * slot;
-            k.ntaps = st.ntaps;
-            for (int i = 0; i < st.ntaps; ++i) {
-                const b2_sys_tap &t = st.taps[i];
-                long long delta = 0;
-                for (int d = 0; d < nd; ++d) {
-                    const int di = 3 - nd + d;
-                    delta += (long long)t.off[d] * (di == 0 ? k.sx : di == 1 ? k.sy : 1);
-                }
-                k.fld[i] = (short)t.field; k.tsh[i] = (short)t.tshift; k.cfi[i] = (short)t.cfield;
-                k.delta[i] = (int)delta; k.coef[i] = t.coef;
-            }
-            k_system_stage<<<grid, block, 0, stream()>>>(k);
-            count_launch();
-        }
-        if (per_step) rec_ev();
-        for (int i = 0; i < a->ninject; ++i) {
-            const b2_sys_inject &q = a->inject[i];
-            float *f0 = (float *)F[q.fields[0]].d + (size_t)slot_of(q.fields[0], time, q.tshift) * slot;
-            float *f1 = q.nfields > 1 ? (float *)F[q.fields[1]].d + (size_t)slot_of(q.fields[1], time, q.tshift) * slot : nullptr;
-            // scale modes of k_inject: scalar | dt2 * param^2 | dt2 / param with dt2 := q.scale
-            const float *prm = q.param_kind != B2_PARAM_SCALAR ? (const float *)injp[i].d : nullptr;
-            if ((rc = launch_inject(inj[i], g, f0, f1, time, q.param_kind, prm, q.scale, q.scale))) return cleanup(rc);
-            if (q.nfields > 2) {
-                float *f2 = (float *)F[q.fields[2]].d + (size_t)slot_of(q.fields[2], time, q.tshift) * slot;
-                if ((rc = launch_inject(inj[i], g, f2, nullptr, time, q.param_kind, prm, q.scale, q.scale))) return cleanup(rc);
-            }
-        }
-        if (per_step) rec_ev();
-        for (int i = 0; i < a->ninterp; ++i) {
-            const b2_sys_interp &q = a->interp[i];
-            const float *f = (const float *)F[q.field].d + (size_t)slot_of(q.field, time, q.tshift) * slot;
-            if ((rc = launch_interp(itp[i], g, f, nullptr, time))) return cleanup(rc);
-        }
-        if (per_step) rec_ev();
-    }
-    if (timing && !per_step) cudaEventRecord(ev[1], stream());
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream());
-    if (timing) {
-        float ms = 0.f;
-        if (per_step) {
-            for (size_t i = 0; i + 3 < pool.size(); i += 4) {
-                if (cudaEventElapsedTime(&ms, pool[i], pool[i + 1]) == cudaSuccess) sec[0] += ms;
-                if (cudaEventElapsedTime(&ms, pool[i + 1], pool[i + 2]) == cudaSuccess) sec[1] += ms;
-                if (cudaEventElapsedTime(&ms, pool[i + 2], pool[i + 3]) == cudaSuccess) sec[2] += ms;
-            }
-        } else if (e == cudaSuccess && cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) {
-            sec[0] = ms;
-        }
-        a->timers->section0 += sec[0] * 1e-3;
-        a->timers->section1 += sec[1] * 1e-3;
-        a->timers->section2 += sec[2] * 1e-3;
-        for (auto &x : ev) cudaEventDestroy(x);
-        for (auto &x : pool) cudaEventDestroy(x);
-    }
-    if (e != cudaSuccess) { set_error("b2_system_forward: %s", cudaGetErrorString(e)); return cleanup(B2_ERR_LAUNCH); }
-    return cleanup(B2_OK);
+    Staging st;
+    return st.finish(system_forward_body(a, st));
 }

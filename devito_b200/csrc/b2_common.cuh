@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <cstring>
 #include <string>
+#include <deque>
 #include <mutex>
 #include "b200stencil.h"
 
@@ -87,21 +88,45 @@ inline int choose_chunk_len(long long sms, int tiles, int xcount, int prime, int
         }                                                                          \
     } while (0)
 
+// ring-buffer slot of time level `time` in an array of T slots
+inline int slot(int time, int T) { return ((time % T) + T) % T; }
+
 // A dense f32/i32 array made device-visible: either resident (dmap) or staged by us.
 struct DevArray {
     void *d = nullptr;       // device pointer
     void *h = nullptr;       // host pointer (may be null when resident)
     size_t nbytes = 0;
-    bool owned = false;      // we cudaMalloc'ed it -> copy back (if written) + free
+    bool owned = false;      // we allocated it: released when the call ends
+    bool written = false;    // the call writes it: copied back to `h` (see Staging::finish)
+    bool host_io = false;    // ... even though not owned: the caller's own device buffer next to its host array
     int ndim = 0;
     int size[4] = {1, 1, 1, 1};
 };
 
-// ndim: number of entries of obj->size to read
-int stage_in(const b2_dataobj *obj, int ndim, DevArray &out, bool copy_in);
-int stage_out(DevArray &a, bool copy_back);
+// The arrays one entry-point call makes device-visible. The deque keeps their addresses stable: plans point into them.
+class Staging {
+  public:
+    // Stages `obj` (`ndim` extents): resident arrays (dmap) are used in place, host arrays are copied in (copy_in)
+    // to a buffer of the staging pool. `out` is set even when this fails, and finish() releases what it holds.
+    int array(const b2_dataobj *obj, int ndim, bool written, DevArray *&out, bool copy_in = true);
+    // Ends the call: the written arrays go back to the host iff `code` is B2_OK or B2_ERR_NAN, every staged buffer
+    // is released whatever the code. Returns `code`, or the first copy-back error when `code` is B2_OK.
+    int finish(int code);
 
-// Imaging condition over the iterated box, after the step and its injection (k_imaging, b2_api_iso.cu):
+  private:
+    std::deque<DevArray> arrays_;
+};
+
+// The halo of `x`, an array of u's grid (u: (time, space...), halo so) after `lead` leading dims: `need` when
+// need >= 0 (the array must have u's space layout), else obj->hsize's, else inferred from the extents. Every space
+// extent must be the grid's plus twice that halo. Returns the halo, or -1 after set_error naming the array.
+int grid_halo(const char *who, const char *name, const b2_dataobj *obj, const DevArray &x, int lead,
+              const DevArray &u, int nd, int so, int need = -1);
+
+// NaN/Inf check of n floats (reference: errctl='max', passes/iet/errors.py:59-85); waits for the result
+int check_finite(const float *f, size_t n, bool &bad);
+
+// Imaging condition over the iterated box, after the step and its injection (k_imaging, b2_runtime.cu):
 // grad -= us * (v1 - 2 v0 + v2) / dt^2, and with us2 != nullptr also - us2 * (w1 - 2 w0 + w2) / dt^2 (the TTI
 // gradient's second pair). 24 B/point with one pair, 40 with two.
 struct ImgK {
@@ -120,12 +145,43 @@ struct ImgK {
 };
 int launch_imaging(const ImgK &k);
 
-// section timers: CUDA-event accumulation per section, flushed to b2_profiler at exit
-struct SectionTimer {
-    bool enabled = false;
-    cudaEvent_t ev[5];
-    void init(bool on);
-    void destroy();
+// The imaging condition over plan p's box (IsoPlan or TtiPlan) at time level slots t0 (centre), t1, t2 of the
+// wavefields f and f2 (f2, us2 null: one pair); `us` / `us2` are the saved wavefields at this time step, `gh` grad's halo.
+template <class Plan>
+int launch_imaging(const Plan &p, const DevArray &grad, int gh, const float *us, const float *f, const float *us2,
+                   const float *f2, int t0, int t1, int t2) {
+    auto at = [&](const float *x, int t) { return x ? x + (size_t)t * p.slot_elems : nullptr; };
+    ImgK k;
+    k.grad = (float *)grad.d;
+    k.us = us; k.v0 = at(f, t0); k.v1 = at(f, t1); k.v2 = at(f, t2);
+    k.us2 = us2; k.w0 = at(f2, t0); k.w1 = at(f2, t1); k.w2 = at(f2, t2);
+    k.sx = p.sx; k.sy = p.sy;
+    k.gsy = grad.size[2];
+    k.gsx = (long long)grad.size[1] * grad.size[2];
+    k.n0 = p.n[0]; k.n1 = p.n[1]; k.n2 = p.n[2];
+    k.o0 = p.o[0]; k.o1 = p.o[1]; k.o2 = p.o[2];
+    k.g0 = p.o[0] - p.so + gh; k.g1 = p.o[1] - p.so + gh; k.g2 = p.o[2] - p.so + gh;
+    k.inv_dt2 = 1.0f / (p.dt * p.dt);
+    return launch_imaging(k);
+}
+
+// The iteration box of a linear / system call (`a`: x_m .. z_M) in the internal 3-dim convention: a 1-D or 2-D
+// grid gets leading dummy dims of extent 1. `size` = the allocated space extents, `h` the halo.
+struct Box3 {
+    int alloc[3] = {1, 1, 1}, lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0}, hal[3] = {0, 0, 0};
 };
+template <class Args>
+Box3 box3(const Args *a, int nd, const int *size, int h) {
+    const int lo_in[3] = {a->x_m, a->y_m, a->z_m}, hi_in[3] = {a->x_M, a->y_M, a->z_M};
+    Box3 b;
+    for (int d = 0; d < nd; ++d) {
+        const int di = 3 - nd + d;
+        b.alloc[di] = size[d];
+        b.lo[di] = lo_in[d];
+        b.hi[di] = hi_in[d];
+        b.hal[di] = h;
+    }
+    return b;
+}
 
 }  // namespace b2

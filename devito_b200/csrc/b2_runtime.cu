@@ -160,43 +160,119 @@ static void pool_release(void *p, size_t nbytes) {
     cudaFree(p);
 }
 
-int stage_in(const b2_dataobj *obj, int ndim, DevArray &out, bool copy_in) {
+static unsigned long long g_staged_outstanding = 0;    // pool buffers Staging holds (b2_staging_outstanding)
+
+int Staging::array(const b2_dataobj *obj, int ndim, bool written, DevArray *&out, bool copy_in) {
+    DevArray &x = arrays_.emplace_back();
+    out = &x;
+    x.written = written;
     if (!obj) { set_error("stage_in: NULL dataobj"); return B2_ERR_INVALID; }
     if (!obj->size) { set_error("stage_in: dataobj without `size`"); return B2_ERR_INVALID; }
     for (int i = 0; i < ndim; ++i)
         if (obj->size[i] <= 0) { set_error("stage_in: non-positive extent %d on dim %d", obj->size[i], i); return B2_ERR_INVALID; }
-    out.ndim = ndim;
+    x.ndim = ndim;
     size_t n = 1;
-    for (int i = 0; i < ndim; ++i) { out.size[i] = obj->size[i]; n *= (size_t)obj->size[i]; }
-    out.nbytes = obj->nbytes ? (size_t)obj->nbytes : n * 4;
-    out.h = obj->data;
+    for (int i = 0; i < ndim; ++i) { x.size[i] = obj->size[i]; n *= (size_t)obj->size[i]; }
+    x.nbytes = obj->nbytes ? (size_t)obj->nbytes : n * 4;
+    x.h = obj->data;
     if (obj->dmap) {
-        out.d = obj->dmap;
-        out.owned = false;
+        x.d = obj->dmap;
         return B2_OK;
     }
     if (!obj->data) { set_error("stage_in: dataobj has neither data nor dmap"); return B2_ERR_INVALID; }
-    B2_CUDA(pool_alloc(&out.d, out.nbytes), B2_ERR_MEMORY);
-    out.owned = true;
+    B2_CUDA(pool_alloc(&x.d, x.nbytes), B2_ERR_MEMORY);
+    x.owned = true;
+    ++g_staged_outstanding;
     if (copy_in)
-        B2_CUDA(cudaMemcpyAsync(out.d, out.h, out.nbytes, cudaMemcpyHostToDevice, stream()),
+        B2_CUDA(cudaMemcpyAsync(x.d, x.h, x.nbytes, cudaMemcpyHostToDevice, stream()),
                 B2_ERR_MEMORY);
     return B2_OK;
 }
 
-int stage_out(DevArray &a, bool copy_back) {
-    if (!a.owned) return B2_OK;
-    int rc = B2_OK;
-    if (copy_back) {
-        cudaError_t e = cudaMemcpyAsync(a.h, a.d, a.nbytes, cudaMemcpyDeviceToHost, stream());
-        if (e == cudaSuccess) e = cudaStreamSynchronize(stream());
-        if (e != cudaSuccess) { set_error("stage_out: %s", cudaGetErrorString(e)); rc = B2_ERR_MEMORY; }
+int Staging::finish(int code) {
+    cudaError_t e = cudaSuccess;
+    if (code == B2_OK || code == B2_ERR_NAN)
+        for (const DevArray &x : arrays_)
+            if (x.written && (x.owned || x.host_io)) {
+                const cudaError_t c = cudaMemcpyAsync(x.h, x.d, x.nbytes, cudaMemcpyDeviceToHost, stream());
+                if (e == cudaSuccess) e = c;
+            }
+    // the copies above, and whatever kernels and copies in flight still use the buffers
+    const cudaError_t s = cudaStreamSynchronize(stream());
+    if (e == cudaSuccess) e = s;
+    for (DevArray &x : arrays_)
+        if (x.owned) {
+            pool_release(x.d, x.nbytes);
+            --g_staged_outstanding;
+        }
+    arrays_.clear();
+    if (code == B2_OK && e != cudaSuccess) {
+        set_error("stage_out: %s", cudaGetErrorString(e));
+        return B2_ERR_MEMORY;
     }
-    if (!copy_back) cudaStreamSynchronize(stream());   // pending async H2D/kernels still use it
-    pool_release(a.d, a.nbytes);
-    a.d = nullptr;
-    a.owned = false;
-    return rc;
+    return code;
+}
+
+int grid_halo(const char *who, const char *name, const b2_dataobj *obj, const DevArray &x, int lead,
+              const DevArray &u, int nd, int so, int need) {
+    const int n0 = u.size[1] - 2 * so;                   // the grid's extent on the first space dim
+    const int h = need >= 0 ? need : obj->hsize ? obj->hsize[2 * lead] : (x.size[lead] - n0) / 2;
+    for (int d = 0; d < nd; ++d)
+        if (h < 0 || x.size[lead + d] != u.size[d + 1] - 2 * so + 2 * h) {
+            set_error("%s: %s extent %d on dim %d does not match the grid (halo %d)", who, name, x.size[lead + d], d, h);
+            return -1;
+        }
+    return h;
+}
+
+__global__ void k_check_finite(const float *__restrict__ f, size_t n, int *flag) {
+    size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    bool bad = false;
+    for (; i < n; i += stride) bad |= !isfinite(f[i]);
+    if (bad) atomicOr(flag, 1);
+}
+
+int check_finite(const float *f, size_t n, bool &bad) {
+    static int *d_flag = nullptr;
+    if (!d_flag) B2_CUDA(cudaMalloc(&d_flag, sizeof(int)), B2_ERR_MEMORY);
+    B2_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), stream()), B2_ERR_MEMORY);
+    B2_SM_COUNT(sms);
+    k_check_finite<<<sms * 4, 256, 0, stream()>>>(f, n, d_flag);
+    count_launch();
+    int h = 0;
+    B2_CUDA(cudaMemcpyAsync(&h, d_flag, sizeof(int), cudaMemcpyDeviceToHost, stream()), B2_ERR_MEMORY);
+    B2_CUDA(cudaStreamSynchronize(stream()), B2_ERR_DEVICE);
+    bad = h != 0;
+    return B2_OK;
+}
+
+// Imaging condition (reference: `Inc(grad, -u * v.dt2)`, acoustic/operators.py:222; the TTI gradient's
+// `Inc(dm, -(u0 * du.dt2 + v0 * dv.dt2))`, tti/operators.py `JacobianAdjOperator`, with the second pair):
+// grad[p] -= usave[time][p] * (v[t+1][p] - 2 v[t][p] + v[t-1][p]) / dt^2 (+ the same of us2, w) over the iterated box.
+__global__ void __launch_bounds__(256) k_imaging(ImgK k) {
+    const int z = blockIdx.x * blockDim.x + threadIdx.x;
+    const int y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (z >= k.n2 || y >= k.n1) return;
+    for (int x = blockIdx.z; x < k.n0; x += gridDim.z) {
+        const long long i = (long long)(k.o0 + x) * k.sx + (long long)(k.o1 + y) * k.sy + (k.o2 + z);
+        const long long g = (long long)(k.g0 + x) * k.gsx + (long long)(k.g1 + y) * k.gsy + (k.g2 + z);
+        const float d2 = (k.v1[i] - 2.0f * k.v0[i] + k.v2[i]) * k.inv_dt2;
+        if (k.us2) {
+            const float e2 = (k.w1[i] - 2.0f * k.w0[i] + k.w2[i]) * k.inv_dt2;
+            k.grad[g] = k.grad[g] - fmaf(k.us[i], d2, k.us2[i] * e2);
+        } else {
+            k.grad[g] = k.grad[g] - k.us[i] * d2;
+        }
+    }
+}
+
+int launch_imaging(const ImgK &ik) {
+    dim3 blk(64, 4, 1), grd((ik.n2 + 63) / 64, (ik.n1 + 3) / 4, (unsigned)(ik.n0 < 65535 ? ik.n0 : 65535));
+    k_imaging<<<grd, blk, 0, stream()>>>(ik);
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
 }
 
 }  // namespace b2
@@ -287,6 +363,11 @@ void b2_set_stream(void *s) { g_user_stream = (cudaStream_t)s; }
 void b2_staging_cache_release(void) {
     std::lock_guard<std::mutex> lock(api_mutex());
     pool_drain_big();
+}
+
+unsigned long long b2_staging_outstanding(void) {
+    std::lock_guard<std::mutex> lock(api_mutex());
+    return g_staged_outstanding;
 }
 
 }  // extern "C"

@@ -137,16 +137,16 @@ static SparseK make_k(const SparseDev &s, const FieldGeom &g, bool injecting) {
     k.off_lo = g.off_lo; k.off_hi = g.off_hi;
     k.nown = g.nown;
     k.pw = injecting && s.ndim == 3 && (g.peer_lo || g.peer_hi) ? g.pw : 0;
-    k.data = (const float *)s.data.d;
-    k.gp = (const int *)s.gp.d;
+    k.data = (const float *)s.data->d;
+    k.gp = (const int *)s.gp->d;
     if (s.ndim == 3) {
-        k.w0 = (const float *)s.w[0].d;
-        k.w1 = (const float *)s.w[1].d;
-        k.w2 = (const float *)s.w[2].d;
+        k.w0 = (const float *)s.w[0]->d;
+        k.w1 = (const float *)s.w[1]->d;
+        k.w2 = (const float *)s.w[2]->d;
     } else {
         k.w0 = nullptr;
-        k.w1 = (const float *)s.w[0].d;
-        k.w2 = (const float *)s.w[1].d;
+        k.w1 = (const float *)s.w[0]->d;
+        k.w2 = (const float *)s.w[1]->d;
     }
     k.npoint_total = s.npoint_total;
     k.p_m = s.p_m;
@@ -167,38 +167,36 @@ static SparseK make_k(const SparseDev &s, const FieldGeom &g, bool injecting) {
     return k;
 }
 
-int sparse_stage_in(const b2_sparse *s, int ndim, SparseDev &out, bool copy_data_in) {
+int sparse_stage_in(Staging &st, const b2_sparse *s, int ndim, bool written, SparseDev &out) {
     out.present = false;
     if (!s) return B2_OK;
     if (s->p_M < s->p_m) return B2_OK;     // empty point range: nothing to do
     if (s->r < 1 || s->r > 8) { set_error("sparse: unsupported radius %d", s->r); return B2_ERR_INVALID; }
-    int rc;
-    if ((rc = stage_in(s->data, 2, out.data, copy_data_in))) return rc;
-    if ((rc = stage_in(s->gp, 2, out.gp, true))) return rc;
-    for (int d = 0; d < ndim; ++d) {
+    if (!s->data || !s->data->size || !s->gp) { set_error("sparse: missing traces or base cells"); return B2_ERR_INVALID; }
+    for (int d = 0; d < ndim; ++d)
         if (!s->w[d]) { set_error("sparse: missing weight table for dim %d", d); return B2_ERR_INVALID; }
-        if ((rc = stage_in(s->w[d], 2, out.w[d], true))) return rc;
+    if (s->p_m < 0 || s->p_M >= s->data->size[1]) {
+        set_error("sparse: point range [%d,%d] outside [0,%d)", s->p_m, s->p_M, s->data->size[1]);
+        return B2_ERR_INVALID;
     }
-    out.nt = out.data.size[0];
-    out.npoint_total = out.data.size[1];
+    DevArray *x;
+    int rc;
+    if ((rc = st.array(s->data, 2, written, x))) return rc;
+    out.data = x;
+    if ((rc = st.array(s->gp, 2, false, x))) return rc;
+    out.gp = x;
+    for (int d = 0; d < ndim; ++d) {
+        if ((rc = st.array(s->w[d], 2, false, x))) return rc;
+        out.w[d] = x;
+    }
+    out.nt = out.data->size[0];
+    out.npoint_total = out.data->size[1];
     out.p_m = s->p_m;
     out.p_M = s->p_M;
     out.r = s->r;
     out.ndim = ndim;
-    if (out.p_m < 0 || out.p_M >= out.npoint_total) {
-        set_error("sparse: point range [%d,%d] outside [0,%d)", out.p_m, out.p_M, out.npoint_total);
-        return B2_ERR_INVALID;
-    }
     out.present = true;
     return B2_OK;
-}
-
-int sparse_stage_out(SparseDev &s, bool copy_data_back) {
-    if (!s.present) return B2_OK;
-    int rc = stage_out(s.data, copy_data_back);
-    stage_out(s.gp, false);
-    for (int d = 0; d < s.ndim; ++d) stage_out(s.w[d], false);
-    return rc;
 }
 
 int launch_inject(const SparseDev &s, const FieldGeom &g, float *f0, float *f1, int time,
@@ -220,7 +218,7 @@ int launch_interp(const SparseDev &s, const FieldGeom &g, const float *f0, const
     SparseK k = make_k(s, g, false);
     const int warps = k.p_cnt;
     const int blocks = (warps * 32 + 127) / 128;
-    k_interp<<<blocks, 128, 0, stream()>>>(k, f0, f1, (float *)s.data.d, time, (g.restrict_x || g.restrict_y) ? 1 : 0);
+    k_interp<<<blocks, 128, 0, stream()>>>(k, f0, f1, (float *)s.data->d, time, (g.restrict_x || g.restrict_y) ? 1 : 0);
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
     return B2_OK;

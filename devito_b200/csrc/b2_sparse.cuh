@@ -6,7 +6,7 @@ namespace b2 {
 
 struct SparseDev {
     bool present = false;
-    DevArray data, gp, w[3];
+    const DevArray *data = nullptr, *gp = nullptr, *w[3] = {nullptr, nullptr, nullptr};   // held by a Staging
     int npoint_total = 0;   // second extent of data
     int nt = 0;
     int p_m = 0, p_M = -1;
@@ -38,8 +38,9 @@ struct FieldGeom {
     int nown = 0, pw = 0;
 };
 
-int sparse_stage_in(const b2_sparse *s, int ndim, SparseDev &out, bool copy_data_in);
-int sparse_stage_out(SparseDev &s, bool copy_data_back);
+// Checks the tables of `s` (radius, gp, the ndim weight tables, the point range against the traces) and only then
+// stages them into `st`; `written`: the traces are copied back (receivers). `out.present` stays false without points.
+int sparse_stage_in(Staging &st, const b2_sparse *s, int ndim, bool written, SparseDev &out);
 
 // u[cell] += w*w*w * src[time][p] * scale(cell) for up to two fields (TTI injects into u and v)
 // scale(cell) = dt^2 * vp^2 | dt^2 * vp[cell]^2 | dt^2 / m[cell]

@@ -1201,12 +1201,6 @@ int tti_plan_init(TtiPlan &p, int kernel) {
     return B2_OK;
 }
 
-void tti_plan_free(TtiPlan &p) {
-    p.gzu = p.gzv = nullptr;       // scratch is cached in the library
-    p.coefA = nullptr;
-    p.tCx = p.tCy = p.tCz = p.tE2 = p.tSD = p.tMD = nullptr;
-}
-
 int tti_plan_retarget(const TtiPlan &p, float *u, float *v, TtiPlan &out) {
     out = p;
     out.u = u;

@@ -42,7 +42,6 @@ struct TtiPlan {
 };
 
 int tti_plan_init(TtiPlan &p, int kernel);
-void tti_plan_free(TtiPlan &p);
 // A plan for a second field pair (u, v) of the same layout that shares p's tables, scratch and sweep variant: only the
 // tensor maps are rebuilt for the new pointers. Fails (210) when p is fused and the new pointers do not qualify.
 int tti_plan_retarget(const TtiPlan &p, float *u, float *v, TtiPlan &out);

@@ -45,7 +45,10 @@ extern "C" {
  * (devito/passes/iet/languages/openacc.py:245-247); here:
  *    dmap == NULL : the callee allocates device memory, copies `data` H2D on entry, copies
  *                   written arrays D2H on exit and frees (== reference `devicerm=1`);
- *    dmap != NULL : the array is device-resident at `dmap` (same layout); no copies.    */
+ *    dmap != NULL : the array is device-resident at `dmap` (same layout); no copies.
+ * Written arrays are copied back when the call returns 0 or 100 (NaN); on any other return code
+ * the host arrays are left untouched.  The device memory staged for a call is released on every
+ * return path (b2_staging_outstanding counts what is still held).                        */
 struct b2_dataobj {
     void *data;
     int *size;              /* allocated shape, ndim entries                               */
@@ -370,8 +373,11 @@ void  b2_set_stream(void *stream);
 /* Host-staged applies recycle their device staging buffers across calls (up to B2_STAGING_CACHE_GB,
  * default 24): release what is cached. */
 void  b2_staging_cache_release(void);
+/* Staging buffers that entry-point calls allocated and have not released yet: 0 between calls. */
+unsigned long long b2_staging_outstanding(void);
 /* Phase times (ms) of the last b2_iso_forward call on this process: [0] host->device staging issued
- * before the time loop, [1] time loop, [2] device->host after the loop, [3] whole call (device clock);
+ * before the time loop, [1] time loop, [2] write-back after the loop (device->host copies, snapshot drain,
+ * release of the staging buffers), [3] whole call (host clock);
  * [4] = 1 when the call ran the streamed (skewed, copy-overlapped) time loop. */
 void  b2_last_call_profile(double out[5]);
 

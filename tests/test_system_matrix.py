@@ -7,6 +7,7 @@
 * The synthetic systems of tests/system_cases.py, in three modes: host-staged, device-resident coefficients, and the
   taps shuffled after `Stage` sorted them by coefficient array (every tap reloads the cached coefficient).
 * Malformed calls: each returns B2_ERR_INVALID (210) and leaves the fields and traces untouched.
+* Every call, run or refused, releases every staging buffer it took (`b2_staging_outstanding`).
 
 The reference package is never read here.
 """
@@ -77,8 +78,10 @@ def _build(system, fields, coefs, mode, seed=0):
 
 
 def _execute(system, fields, coefs, lo, hi, tm, tM, mode):
+    from devito_b200 import _lib as L_
     ls, fobjs, F, cobjs, traces, keep = _build(system, fields, coefs, mode)
     ls.apply(fobjs, cobjs, lo, hi, tm, tM)
+    assert L_.lib().b2_staging_outstanding() == 0
     return F, traces
 
 
@@ -168,6 +171,7 @@ def _refused(system, fields, coefs, lo, hi, edit=None):
         edit(a)
     rc = L_.lib().b2_system_forward(ctypes.byref(a))
     assert rc == B2_ERR_INVALID, (rc, L_.lib().b2_last_error().decode())
+    assert L_.lib().b2_staging_outstanding() == 0
     assert all(np.array_equal(f, f0) for f, f0 in zip(F, F0))
     assert all(np.array_equal(traces[k], tr0[k]) for k in tr0)
     return L_.lib().b2_last_error().decode()
@@ -217,13 +221,20 @@ SPARSE_EDITS = {
     'param_kind_negative': _set_inject('param_kind', -1),
     'interp_field_high': lambda a: setattr(a.interp[0], 'field', 2),
     'interp_field_negative': lambda a: setattr(a.interp[0], 'field', -1),
+    # the sparse tables themselves, refused before any of them is staged
+    'interp_p_M_high': lambda a: setattr(a.interp[0].s.contents, 'p_M', 1),      # = npoint_total
+    'inject_no_weight_table': lambda a: a.inject[0].s.contents.w.__setitem__(1, None),
 }
+_SPARSE_MSG = {'interp_p_M_high': 'point range', 'inject_no_weight_table': 'weight table'}
 
 
 @pytest.mark.parametrize('edit', list(SPARSE_EDITS))
 def test_refuses_bad_sparse_indices(edit):
     msg = _refused(*_small(3), edit=SPARSE_EDITS[edit])
-    assert 'injection' in msg or 'interpolation' in msg
+    if edit in _SPARSE_MSG:
+        assert _SPARSE_MSG[edit] in msg
+    else:
+        assert 'injection' in msg or 'interpolation' in msg
 
 
 @pytest.mark.parametrize('side', [-1, 1])
