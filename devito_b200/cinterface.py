@@ -12,7 +12,7 @@ generated file: the SAME symbol with the SAME kind of signature —
                 const int deviceid, const int devicerm, struct profiler *timers)
 
 — which packs its arguments into `struct b2_iso_args` / `struct b2_tti_args` (include/b200stencil.h)
-and calls `b2_iso_forward` / `b2_tti_forward`. Functions and Constants come first in alphabetical
+(or `struct b2_sa_args`) and calls `b2_iso_forward` / `b2_tti_forward` (or `b2_sa_forward`). Functions and Constants come first in alphabetical
 order, then bounds, `dt`, sparse point ranges and time bounds, like the parameter order of the
 reference's printed samples (`damp_vec, dt, m_vec, ..., u_vec, x_M, x_m, ..., timers`;
 devito/ir/iet/utils.py:105-147). The finite-difference weights are literals in the file, as they are
@@ -114,6 +114,12 @@ def signature(plan, name, distributed=False):
             f = plan.get(key)
             if f is not None:
                 head.append(_Param(f.name, 'struct dataobj *restrict', f'{f.name}_vec'))
+    elif plan['kind'] == 'sa':
+        for kind, obj in (plan['b_role'], plan['vp_role']):
+            if kind == 'f':
+                head.append(_Param(obj.name, 'struct dataobj *restrict', f'{obj.name}_vec'))
+            elif kind == 'c':
+                head.append(_Param(obj.name, 'const float', obj.name))
     else:
         for n, c in plan['consts'].items():
             if getattr(c, 'is_Function', False) or hasattr(c, 'space_order'):
@@ -287,6 +293,41 @@ def _tti_body(plan, distributed):
     return L
 
 
+def _sa_body(plan, distributed):
+    nd = plan['grid'].dim
+    L = []
+    for d in range(nd):
+        L.append(_warray(f'c_{"xyz"[d]}', plan['c'][d]))
+    if plan['src'] is not None:
+        L.append(_sparse_block(plan['src'], nd, 'src_s'))
+    if plan['rec'] is not None:
+        L.append(_sparse_block(plan['rec'], nd, 'rec_s'))
+    L.append("  struct b2_profiler prof = {0.0, 0.0, 0.0, 0.0};")
+    L.append("  struct b2_sa_args a;")
+    L.append("  memset(&a, 0, sizeof(a));")
+    L.append(f"  a.ndim = {nd};")
+    L.append(f"  a.space_order = {plan['so']};")
+    L.append(f"  a.radius = {plan['R']};")
+    for d in range(nd):
+        L.append(f"  a.c[{d}] = c_{'xyz'[d]};")
+    L.append(f"  a.u = (struct b2_dataobj *){plan['u'].name}_vec;")
+    for key, (kind, obj) in (('b', plan['b_role']), ('vp', plan['vp_role'])):
+        if kind == 'f':
+            L.append(f"  a.{key} = (struct b2_dataobj *){obj.name}_vec;")
+            L.append(f"  a.{key}_value = 1.0f;")
+        elif kind == 'c':
+            L.append(f"  a.{key}_value = {obj.name};")
+        else:
+            L.append(f"  a.{key}_value = {_flit(obj)};")
+    if plan.get('damp') is not None:
+        L.append(f"  a.damp = (struct b2_dataobj *){plan['damp'].name}_vec;")
+    L.append("  a.dt = dt;")
+    _bounds(plan, L)
+    L.append(f"  a.adjoint = {1 if plan.get('adjoint') else 0};")
+    _tail(plan, 'b2_sa_forward', L, distributed)
+    return L
+
+
 def generate(plan, name, distributed=False):
     """(ccode, hcode) strings for a recognised operator."""
     params = signature(plan, name, distributed)
@@ -302,7 +343,7 @@ def generate(plan, name, distributed=False):
     if distributed:
         h.append("struct b2_halo_ctx;\n")
     h += [proto + ";", "", "#ifdef __cplusplus", "#undef restrict", "}", "#endif", "", f"#endif /* {guard} */", ""]
-    body = _iso_body(plan, distributed) if plan['kind'] == 'iso' else _tti_body(plan, distributed)
+    body = {'iso': _iso_body, 'tti': _tti_body, 'sa': _sa_body}[plan['kind']](plan, distributed)
     c = ['#include <math.h>', '#include <string.h>', f'#include "{name}.h"', '#include "b200stencil.h"', "",
          "/* `struct dataobj` and `struct b2_dataobj` have the same members in the same order */",
          "typedef char dataobj_layout_check[(sizeof(struct dataobj) == sizeof(struct b2_dataobj)) ? 1 : -1];",

@@ -85,6 +85,8 @@ k_inject(SparseK k, float *__restrict__ f0, float *__restrict__ f1, int time, in
             scale = dt2 * v * v;
         } else if (param_kind == B2_PARAM_M) {
             scale = dt2 / param[idx];
+        } else if (param_kind == B2_SCALE_TABLE) {
+            scale = param[idx];
         }
         const float val = w * sv * scale;
         atomicAdd(f0 + idx, val);

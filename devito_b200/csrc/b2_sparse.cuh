@@ -42,8 +42,12 @@ struct FieldGeom {
 // stages them into `st`; `written`: the traces are copied back (receivers). `out.present` stays false without points.
 int sparse_stage_in(Staging &st, const b2_sparse *s, int ndim, bool written, SparseDev &out);
 
+// Internal param_kind of launch_inject: the scale is a tabulated array in the field's layout, taken at the cell
+// (the self-adjoint update's C = dt^2 vp^2 / b). Not part of the C ABI.
+constexpr int B2_SCALE_TABLE = 3;
+
 // u[cell] += w*w*w * src[time][p] * scale(cell) for up to two fields (TTI injects into u and v)
-// scale(cell) = dt^2 * vp^2 | dt^2 * vp[cell]^2 | dt^2 / m[cell]
+// scale(cell) = dt^2 * vp^2 | dt^2 * vp[cell]^2 | dt^2 / m[cell] | param[cell] (B2_SCALE_TABLE)
 int launch_inject(const SparseDev &s, const FieldGeom &g, float *f0, float *f1, int time,
                   int param_kind, const float *param, float scalar_scale, float dt2);
 

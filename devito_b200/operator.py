@@ -133,6 +133,14 @@ def second_derivative_weights(space_order, h):
     return [w[R + k] / (float(h) ** 2) for k in range(R + 1)]
 
 
+def sa_weights(R, h):
+    """c_k / h, k = 1..R: the weights of `f.dx(x0=x+h/2)` at fd_order 2R (offsets -R+1 .. R about x + h/2) at
+    offset +k; the weight at offset -k+1 is -c_k (examples/seismic/self_adjoint/operators.py:50-62)."""
+    from fractions import Fraction
+    w = fd_weights(1, list(range(-R + 1, R + 1)), Fraction(1, 2))
+    return [w[R - 1 + k] / float(h) for k in range(1, R + 1)]
+
+
 def half_node_first_derivative_weights(space_order, h):
     """Weights of `f.dx(fd_order=so/2, x0=x+h/2)` for offsets (-R/2+1 .. R/2), R = so/2
     (devito/finite_differences/tools.py:289-297; tti/operators.py:88-102)."""
@@ -299,7 +307,15 @@ class Operator:
         if fss and (len(updates) != 1 or len(fss) != 1 or fss[0].field is not updates[0][0]):
             raise _Unrecognised("a free surface is only on the fast path for the single-field acoustic update")
         if len(updates) == 1:
-            plan = self._recognise_iso(updates[0], injs, itps)
+            try:
+                plan = self._recognise_iso(updates[0], injs, itps)
+            except _Unrecognised as iso_why:
+                if incs or fss or snaps:
+                    raise
+                try:
+                    return self._recognise_sa(updates[0], injs, itps)
+                except _Unrecognised as sa_why:
+                    raise _Unrecognised(f"{iso_why}; as the self-adjoint update: {sa_why}") from None
             if incs:
                 self._attach_imaging(plan, incs[0])
             plan['free_surface'] = bool(fss)
@@ -522,6 +538,168 @@ class Operator:
                 'dt': dtsym, 'src': None, 'rec': None, 'rec_toff': 0, 'adjoint': dirn == -1}
         self._attach_sparse(plan, injs, itps, [u], funcs, consts, syms, m_role)
         return plan
+
+    def _recognise_sa(self, update, injs, itps):
+        """The reference's self-adjoint variable-density visco-acoustic update (examples/seismic/self_adjoint/
+        operators.py:4-65 `iso_stencil`): u_next = dt^2 vp^2/b * sum_d (b u.d(x0=d+h/2)).d(x0=d-h/2)
+        + (2 - dt w) u + (dt w - 1) u_prev. The radius and weights follow from the support; the roles of the
+        parameter leaves (b, vp, w) are tried in turn, and each candidate is checked by comparing EVERY stencil
+        coefficient with `predict_sa` at probe values that vary linearly in space, a different gradient per
+        Function and axis, so that where b is sampled (node, half node, output point) changes the prediction."""
+        u, eq = update
+        grid = u.grid
+        nd = grid.dim
+        if nd not in (2, 3):
+            raise _Unrecognised("only 2-D/3-D grids")
+        so = u.space_order
+        terms = self._coeffs(eq.rhs, [u])
+        keyed = {}
+        for acc, coef in terms.items():
+            k = _space_offsets(acc, None)
+            if k is None:
+                raise _Unrecognised("non-affine wavefield access")
+            keyed[k] = coef
+        dirn = self._dirn
+        zero = (0,) * nd
+        reach = max((max(abs(o) for o in k[1]) for k in keyed), default=0)
+        if reach % 2 == 0:
+            raise _Unrecognised("support is not that of nested half-node first derivatives")
+        R = (reach + 1) // 2
+        if 2 * R > so or R > 8:
+            raise _Unrecognised(f"radius {2 * R - 1} does not fit the halo of space_order {so}")
+        star = {(0, zero), (-dirn, zero)}
+        for d in range(nd):
+            for s in range(-reach, reach + 1):
+                o = [0] * nd
+                o[d] = s
+                star.add((0, tuple(o)))
+        if set(keyed) != star:
+            raise _Unrecognised("stencil support is not the star of radius 2R-1 plus the centre of the other level")
+        funcs, consts, syms = self._leaves(keyed.values())
+        for a in funcs:
+            if getattr(a.function, 'is_TimeFunction', False):
+                raise _Unrecognised("a second wavefield in the coefficients")
+        dtsym = grid.stepping_dim.spacing
+        if dtsym.name not in {s.name for s in syms}:
+            raise _Unrecognised("no time spacing in the update")
+        known = {dtsym.name} | {sp.name for sp in grid.spacing_map}
+        for sym in syms:
+            if sym.name not in known:
+                raise _Unrecognised(f"unknown symbol {sym.name} in the update")
+        hs = self._spacing_values(grid)
+        c = [sa_weights(R, h) for h in hs]
+        fcands = [('f', a.function) for a in funcs]
+        ccands = [('c', cst) for cst in consts]
+        cands = fcands + ccands
+        rng = np.random.default_rng(2468)
+        probes = [self._sa_probe(rng, cands, grid) for _ in range(3)]
+        found = None
+        for b_role in cands:
+            for vp_role in cands:
+                if vp_role is b_role:
+                    continue
+                for w_role in [r for r in fcands if r is not b_role and r is not vp_role] + [None]:
+                    used = {id(r[1]) for r in (b_role, vp_role, w_role) if r is not None}
+                    if used != {id(r[1]) for r in cands}:
+                        continue
+                    if all(self._sa_matches(keyed, pr, b_role, vp_role, w_role, c, R, nd, dirn, dtsym)
+                           for pr in probes):
+                        found = (b_role, vp_role, w_role)
+                        break
+                if found:
+                    break
+            if found:
+                break
+        if found is None:
+            raise _Unrecognised("coefficients are not those of the self-adjoint update for any roles of "
+                                "b, vp and w/Q")
+        b_role, vp_role, w_role = found
+        plan = {'kind': 'sa', 'u': u, 'grid': grid, 'so': so, 'R': R, 'c': c,
+                'b_role': b_role, 'vp_role': vp_role, 'damp': w_role[1] if w_role else None,
+                'dt': dtsym, 'src': None, 'rec': None, 'rec_toff': 0, 'adjoint': dirn == -1}
+        self._attach_sa_sparse(plan, injs, itps, funcs, consts, syms)
+        return plan
+
+    def _sa_probe(self, rng, cands, grid):
+        """Probe values: a Function is base + grad . offset (linear in space), a Constant one number."""
+        vals = {}
+        for kind, obj in cands:
+            if kind == 'f':
+                vals[id(obj)] = (rng.uniform(1.0, 2.0), rng.uniform(-0.05, 0.05, size=grid.dim))
+            else:
+                vals[id(obj)] = (rng.uniform(0.5, 2.0), np.zeros(grid.dim))
+        dt = rng.uniform(0.5, 2.0)
+        spc = {sp.name: float(v) for sp, v in grid.spacing_map.items()}
+        spc[grid.stepping_dim.spacing.name] = dt
+
+        def value(obj, off):
+            base, g = vals[id(obj)]
+            return base + float(np.dot(g, off))
+
+        def leaf(n):
+            if n.is_Access:
+                k = _space_offsets(n, None)
+                return value(n.function, k[1] if k is not None else (0,) * grid.dim)
+            if n.is_Constant:
+                return value(n, (0,) * grid.dim)
+            return spc[n.name]           # _recognise_sa refused every other symbol
+        return value, leaf, dt
+
+    def _sa_matches(self, keyed, probe, b_role, vp_role, w_role, c, R, nd, dirn, dtsym):
+        value, leaf, dt = probe
+        got = {k: eval_scalar(v, leaf) for k, v in keyed.items()}
+        pred = predict_sa(c, R, nd, lambda off: value(b_role[1], off), value(vp_role[1], (0,) * nd),
+                          value(w_role[1], (0,) * nd) if w_role else 0.0, dt, dirn)
+        scale = max(abs(v) for v in pred.values())
+        return set(got) == set(pred) and all(abs(got[k] - pred[k]) <= 1e-9 * scale for k in pred)
+
+    def _attach_sa_sparse(self, plan, injs, itps, funcs, consts, syms):
+        """Injection `src * dt^2 * vp^2 / b` into the level written (operators.py:101, :149), checked at random
+        values; receivers / the adjoint source as for the acoustic update."""
+        grid, dtsym = plan['grid'], plan['dt']
+        if injs:
+            inj = injs[0]
+            sf = inj.sfunction
+            if not isinstance(sf, SparseTimeFunction) or sf.interpolation not in ('linear', 'sinc'):
+                raise _Unrecognised("unsupported sparse function for injection")
+            self._check_radius(sf, [plan['u']])
+            if [id(a.function) for a in inj.fields] != [id(plan['u'])]:
+                raise _Unrecognised("injection target differs from the updated field")
+            a, ex = inj.fields[0], inj.exprs[0]
+            k = _space_offsets(a, None)
+            if k is None or k[0] != self._dirn or any(k[1]):
+                raise _Unrecognised("injection must target the updated time level")
+            ex = ex.evaluate.subs(self._subs) if self._subs else ex.evaluate
+            f2, c2, s2 = self._leaves([ex])
+            if dtsym.name not in {s.name for s in s2}:
+                raise _Unrecognised("injected expression has no time spacing")
+            for sym in s2:
+                if sym.name != dtsym.name and sym.name not in {sp.name for sp in grid.spacing_map}:
+                    raise _Unrecognised(f"unknown symbol {sym.name} in the injected expression")
+            if not any(acc.function is sf for acc in f2):
+                raise _Unrecognised("injected expression does not contain the source")
+            rng = np.random.default_rng(8642)
+            roles = [plan['b_role'], plan['vp_role']]
+            known = {id(o) for _, o in roles} | {id(sf)}
+            if any(id(acc.function) not in known for acc in f2) or any(id(cc) not in known for cc in c2):
+                raise _Unrecognised("injected expression has parameters other than vp and b")
+            for _ in range(2):
+                vals = {i: rng.uniform(0.5, 2.0) for i in known}
+                dt = rng.uniform(0.5, 2.0)
+                spc = {sp.name: float(v) for sp, v in grid.spacing_map.items()}
+
+                def leaf(n):
+                    if n.is_Access:
+                        return vals[id(n.function)]
+                    if n.is_Constant:
+                        return vals[id(n)]
+                    return dt if n.name == dtsym.name else spc[n.name]
+                want = vals[id(sf)] * dt * dt * vals[id(plan['vp_role'][1])] ** 2 / vals[id(plan['b_role'][1])]
+                if abs(eval_scalar(ex, leaf) - want) > 1e-9 * abs(want):
+                    raise _Unrecognised("injected expression is not src*dt^2*vp^2/b")
+            plan['src'] = sf
+        if itps:
+            self._attach_sparse(plan, [], itps, [plan['u']], funcs, consts, syms, None)
 
     def _recognise_ot4(self, u, keyed, star, R):
         """The reference's 4th-order-in-time acoustic update (examples/seismic/acoustic/operators.py:
@@ -1195,7 +1373,7 @@ class Operator:
             taps = ', '.join(f"f[t{t:+d}]{list(o)}" for t, o, _ in p['taps'])
             return (f"/* Operator `{self.name}` -> libb200stencil.so::b2_linear_forward (sm_90a)\n"
                     f"   {p['u'].name}[t{p['wshift']:+d}] = sum_k c_k * ({taps}) */")
-        entry = 'b2_iso_forward' if p['kind'] == 'iso' else 'b2_tti_forward'
+        entry = {'iso': 'b2_iso_forward', 'tti': 'b2_tti_forward', 'sa': 'b2_sa_forward'}[p['kind']]
         head = (f"/* Operator `{self.name}` -> libb200stencil.so::{entry} (sm_90a)\n"
                 f"   space_order={p['so']} radius={p['R']} src={p['src'] and p['src'].name} "
                 f"rec={p['rec'] and p['rec'].name} rec_toff={p['rec_toff']}"
@@ -1212,7 +1390,8 @@ class Operator:
         if self._plan is None:
             raise InvalidOperator("interpreted operators have no C entry point")
         L = L_.load_library()
-        return {'iso': L.b2_iso_forward, 'tti': L.b2_tti_forward, 'linear': L.b2_linear_forward}[self._plan['kind']]
+        return {'iso': L.b2_iso_forward, 'tti': L.b2_tti_forward, 'sa': L.b2_sa_forward,
+                'linear': L.b2_linear_forward}[self._plan['kind']]
 
     def cinterface(self, force=False):
         """Write `<name>.c` / `<name>.h` under the JIT directory and return `(ccode, hcode)`
@@ -1245,6 +1424,8 @@ class Operator:
             out.append(p['damp'])
         if p['kind'] == 'iso':
             out.append(p['m_role'][1])
+        elif p['kind'] == 'sa':
+            out += [p['b_role'][1], p['vp_role'][1]]
         else:
             out.extend(p['consts'].values())
         out += [p.get('born_U'), p.get('born_du'), p.get('born_dv'), p.get('born_dm'), p.get('snap')]
@@ -1266,6 +1447,8 @@ class Operator:
             return self._apply_iso(**kwargs)
         if self._plan['kind'] == 'linear':
             return self._apply_linear(**kwargs)
+        if self._plan['kind'] == 'sa':
+            return self._apply_sa(**kwargs)
         return self._apply_tti(**kwargs)
 
     def arguments(self, **kwargs):
@@ -1468,6 +1651,22 @@ class Operator:
                 else:
                     sval = float(val.data if isinstance(val, Constant) else val)
                     args['vp'] = sval if kind.startswith('vp') else 1.0 / np.sqrt(sval)
+        elif p['kind'] == 'sa':
+            if grid.distributor.is_parallel:
+                raise InvalidArgument("the self-adjoint update does not run on a decomposed grid in this version")
+            for key in ('b', 'vp'):
+                kind, obj = p[key + '_role']
+                val = kwargs.pop(obj.name, obj)
+                if isinstance(val, L_.ForeignDataobj) and isinstance(obj, Function):
+                    val = self._foreign(obj, val)
+                elif isinstance(val, np.ndarray) and val.ndim and isinstance(obj, Function):
+                    val = self._shadow(obj, val, None)
+                if isinstance(val, Function):
+                    args['sa_' + key] = val
+                elif isinstance(val, np.ndarray) and val.ndim:
+                    raise InvalidArgument(f"an array `{obj.name}` must have the allocated shape of a Function")
+                else:
+                    args['sa_' + key] = float(val.data if isinstance(val, Constant) else val)
         else:
             args['tti_arrays'] = {}
             for n, c in p['consts'].items():
@@ -1756,6 +1955,9 @@ class Operator:
         if p['kind'] == 'linear':
             return float(2 * len(p['taps'])), 4.0 * (len({t for t, _, _ in p['taps']}) + 1)
         R, nd = p['R'], p['grid'].dim
+        if p['kind'] == 'sa':
+            # per axis 2R fluxes of R multiply-adds and a multiply, then R outer multiply-adds; the update 6
+            return float(nd * (2 * R * (2 * R + 1) + 2 * R) + 6), 24.0
         star = 1 + nd * R * 3                       # centre mul + per tap pair: add, multiply-add
         if p['kind'] == 'iso':
             arr = p['m_role'][0].endswith('_f')
@@ -1838,6 +2040,52 @@ class Operator:
         a.host_io = 1 if self._host_io else 0
         t0 = _time.perf_counter()
         rc = L.b2_iso_forward(ctypes.byref(a))
+        t_wall = _time.perf_counter() - t0
+        for fn in post + args['post']:
+            fn()
+        return self._finish(rc, L, timers, args, 1, t_wall)
+
+    def _apply_sa(self, **kwargs):
+        L = L_.lib()
+        args, hold = self._prepare(dict(kwargs))
+        p = self._plan
+        grid = p['grid']
+        nd = grid.dim
+        dev = self._device(args)
+        res = args['resident']
+        a = L_.SaArgs()
+        a.ndim = nd
+        a.space_order = p['so']
+        a.radius = p['R']
+        a.c = self._w_arrays(p['c'], hold)
+        a.u = self._field_obj(args['fields'][0], dev, res, hold, written=True).ptr
+        for key in ('b', 'vp'):
+            val = args['sa_' + key]
+            if isinstance(val, Function):
+                setattr(a, key, self._field_obj(val, dev, res, hold, so=p['so']).ptr)
+                setattr(a, key + '_value', 1.0)
+            else:
+                setattr(a, key + '_value', val)
+        a.damp = self._field_obj(args['damp'], dev, res, hold, so=p['so']).ptr if args['damp'] is not None else None
+        a.dt = args['dt']
+        lo, hi = args['lo'] + [0] * (3 - nd), args['hi'] + [0] * (3 - nd)
+        a.x_m, a.x_M, a.y_m, a.y_M, a.z_m, a.z_M = lo[0], hi[0], lo[1], hi[1], lo[2], hi[2]
+        a.time_m, a.time_M = args['time_m'], args['time_M']
+        s = self._sparse_obj(args['src'], grid, hold)
+        post = []
+        r = self._sparse_obj(args['rec'], grid, hold, written=True, post=post,
+                             trange=(args['time_m'], args['time_M']))
+        a.src = ctypes.pointer(s) if s is not None else None
+        a.rec = ctypes.pointer(r) if r is not None else None
+        a.rec_toff = p['rec_toff']
+        a.adjoint = 1 if p.get('adjoint') else 0
+        a.errctl = args['errctl']
+        a.deviceid = dev
+        a.kernel = args['kernel']
+        timers = L_.Profiler()
+        a.timers = ctypes.pointer(timers)
+        t0 = _time.perf_counter()
+        rc = L.b2_sa_forward(ctypes.byref(a))
         t_wall = _time.perf_counter() - t0
         for fn in post + args['post']:
             fn()
@@ -1992,6 +2240,32 @@ class Operator:
         for fn in post + args['post']:
             fn()
         return self._finish(rc, L, timers, args, 2, t_wall)
+
+
+# ---------------------------------------------------------------------------------------------
+# the stencil the self-adjoint kernels implement, as linear coefficients (float64) — used only by the recogniser
+# ---------------------------------------------------------------------------------------------
+def predict_sa(c, R, nd, bval, vp, w, dt, dirn):
+    """{(time_shift, offsets): coefficient} of u_next = C sum_d sum_k c_k (F_d(p+(k-1)) - F_d(p-k)) + (2 - dt w) u
+    + (dt w - 1) u_prev, F_d(q) = b(q) sum_i c_i (u(q+i) - u(q-i+1)), C = dt^2 vp^2 / b(p). `bval(offset)` is b at
+    that offset from the output point; vp and w are their values at the output point."""
+    zero = (0,) * nd
+    C = dt * dt * vp * vp / bval(zero)
+    out = {(0, zero): 2.0 - dt * w, (-dirn, zero): dt * w - 1.0}
+
+    def unit(d, o):
+        e = [0] * nd
+        e[d] = o
+        return tuple(e)
+    for d in range(nd):
+        for j in range(-R, R):
+            a = c[d][j] if j >= 0 else -c[d][-j - 1]
+            bq = bval(unit(d, j))
+            for i in range(1, R + 1):
+                for m, sgn in ((j + i, 1.0), (j - i + 1, -1.0)):
+                    key = (0, unit(d, m))
+                    out[key] = out.get(key, 0.0) + C * a * bq * sgn * c[d][i - 1]
+    return out
 
 
 # ---------------------------------------------------------------------------------------------

@@ -8,3 +8,6 @@ from .acoustic import ForwardOperator as AcousticForwardOperator  # noqa: F401
 from .acoustic import AdjointOperator as AcousticAdjointOperator  # noqa: F401
 from .tti import AnisotropicWaveSolver, kernel_centered  # noqa: F401
 from .tti import ForwardOperator as TTIForwardOperator  # noqa: F401
+from .self_adjoint import (SaIsoAcousticWaveSolver, IsoFwdOperator, IsoAdjOperator, setup_w_over_q,  # noqa: F401
+                           acoustic_sa_setup)
+from .self_adjoint import iso_stencil as sa_iso_stencil  # noqa: F401

@@ -217,6 +217,48 @@ struct b2_tti_args {
 };
 int b2_tti_forward(const struct b2_tti_args *a);
 
+/* ---- self-adjoint variable-density visco-acoustic modelling (replaces the generated `IsoFwdOperator` /
+ *      `IsoAdjOperator`, examples/seismic/self_adjoint/operators.py:4-160) ------------------------------------
+ * With R = radius and c_d[k-1] (k = 1..R) the weights of a first derivative at the half node, offsets -R+1 .. R
+ * about x + h/2, at offset +k (the weight at offset -k+1 is -c_d[k-1]), divided by h_d:
+ *   F_d(q)  = b(q) sum_k c_d[k-1] (u[t](q + k e_d) - u[t](q - (k-1) e_d))
+ *   u[t+1]  = dt^2 vp^2/b * sum_d sum_k c_d[k-1] (F_d(p + (k-1) e_d) - F_d(p - k e_d))
+ *             + (2 - dt w) u[t] + (dt w - 1) u[t-1]
+ * b sampled at the grid nodes q, vp, b and w = damp (w/Q) at p. Then u[t+1][cell] += w.w.w * src[t][p] * dt^2 vp^2/b
+ * at the cell, and rec[t][p] samples u[t + rec_toff]. With `adjoint` the same formula writes u[t-1] from u[t] and
+ * u[t+1], time runs from time_M down to time_m, `src` (the receiver data) is injected into u[t-1] with the same scale
+ * and `rec` (the adjoint source) samples u[t] (rec_toff 0) or u[t-1] (rec_toff != 0).
+ * Not combined with halo exchange or a free surface (210). kernel 0 runs the 2.5-D TMA sweep k_sa_tma<R> when the
+ * layout qualifies (3-D, radius 2 or 4, z extent and z start multiples of 4, 16-byte aligned arrays), else the
+ * one-thread-per-point kernel; kernel 2 on a layout that does not qualify returns 210.
+ * b2_last_sweep_kernel reports "sa_tma<R>" or "sa_generic", with "+adj" on adjoint calls. */
+struct b2_sa_args {
+    int ndim;                         /* 2 or 3                                                      */
+    int space_order;                  /* halo width of u / b / vp / damp                             */
+    int radius;                       /* R <= space_order/2 (the nested stencil reaches 2R-1 points)  */
+    const float *c[3];                /* per-dim weights incl. 1/h: c[d][0..radius-1]                */
+    struct b2_dataobj *u;             /* (tsize, x+2so, y+2so[, z+2so]); tsize 3 or nt (save=True)   */
+    struct b2_dataobj *b;             /* buoyancy array, or NULL -> b_value                          */
+    float b_value;
+    struct b2_dataobj *vp;            /* velocity array, or NULL -> vp_value                         */
+    float vp_value;
+    struct b2_dataobj *damp;          /* w/Q array, or NULL -> no attenuation                        */
+    float dt;
+    int x_m, x_M, y_m, y_M, z_m, z_M; /* for ndim==2 the z entries are ignored                       */
+    int time_m, time_M;
+    struct b2_sparse *src;            /* injected into the level written                             */
+    struct b2_sparse *rec;            /* samples u[t] (rec_toff 0) or the level written              */
+    int rec_toff;
+    int adjoint;
+    int errctl;                       /* !=0: NaN check every 100 steps -> return 100                */
+    int deviceid;
+    int kernel;                       /* 0 auto, 1 generic, 2 TMA (210 if the layout does not take it) */
+    b2_halo_ctx *halo;                /* must be NULL                                                */
+    int free_surface;                 /* must be 0                                                   */
+    struct b2_profiler *timers;       /* may be NULL; section0 accumulates the loop time             */
+};
+int b2_sa_forward(const struct b2_sa_args *a);
+
 /* ---- generic explicit update with constant coefficients --------------------------------------
  * Any Operator whose single equation is  f[t + wshift][p] = sum_k coef_k * f[t + tshift_k][p + off_k]
  * with coefficients that do not depend on position (Constants, spacings, dt) — e.g. the reference's
@@ -358,7 +400,8 @@ void   b2_kernel_timing_enable(int on);
  * "tti_fused<2>", "tti_ws<pf1>", "tti_arr_ct2<4>" (radius); "" if the call launched none. Several kernels are
  * selected at run time (layout checks, B2_* switches): this tells which one computed the answer. A TTI Born call
  * appends the path of its source term: "+born_v4" (float4 along z) or "+born_s" (one point per thread); a TTI
- * adjoint call appends "+adj" to the variant that ran its sweep. */
+ * adjoint call appends "+adj" to the variant that ran its sweep. b2_sa_forward reports "sa_tma<R>" or "sa_generic", with "+adj" on
+ * adjoint calls. */
 const char *b2_last_sweep_kernel(void);
 /* device memory helpers for hosts that do not use torch */
 void *b2_malloc_device(unsigned long nbytes, int deviceid);
