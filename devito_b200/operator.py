@@ -21,6 +21,7 @@ import ctypes
 import os
 import time as _time
 from collections import OrderedDict
+from typing import NamedTuple
 
 import numpy as np
 
@@ -156,6 +157,81 @@ class _Unrecognised(Exception):
 
 
 # ---------------------------------------------------------------------------------------------
+# the argument block of a wave operator's C entry point
+# ---------------------------------------------------------------------------------------------
+class Slot(NamedTuple):
+    """An array member of the block: the plan's object, whether the call writes it, whether it is re-laid
+    out to the wavefield's halo, and what an override must be (a key of `_OVERRIDE_KINDS`)."""
+    member: str
+    obj: object
+    written: bool
+    layout: bool
+    check: str
+
+
+class Param(NamedTuple):
+    """A parameter passed as the array `member` or as the scalar `scalar`. `obj` is the plan's Function or
+    Constant (None: always `unit`); the scalar is `unit` while the array is used. `slowness`: `obj` is
+    m = 1/vp^2, passed as the scalar 1/sqrt(m) or as a B2_PARAM_M array. `switch`: an override may turn an
+    array into a scalar and back."""
+    member: str
+    scalar: str
+    obj: object
+    unit: float
+    slowness: bool
+    switch: bool
+
+
+class Entry(NamedTuple):
+    """Everything `Operator.apply`, `Operator.parameters`, the C adapter (cinterface.py) and the reference
+    plugin (refplugin.py) need to know about the call of a recognised wave operator."""
+    symbol: str             # b2_<kind>_forward, taking a struct b2_<kind>_args
+    struct: type            # its ctypes mirror
+    flags: dict             # integer members fixed by the plan
+    weights: list           # (member, per-dimension weight lists)
+    arrays: list            # Slots, in the order they are marshalled
+    params: list            # Params
+    host_io: tuple          # members that may come with the caller's device buffer (struct b2_iso_args.host_io)
+
+
+_OVERRIDE_KINDS = {'wavefield': "a TimeFunction of the wavefield's space order on the same grid",
+                   'saved': "a saved TimeFunction (save=nt) of the wavefield's space order",
+                   'snapshot': "a saved TimeFunction on the same grid",
+                   'function': "a Function or an array of its allocated shape"}
+
+
+def wave_entry(p):
+    """The `Entry` of a recognised wave plan (kind 'iso', 'tti' or 'sa')."""
+    kind = p['kind']
+    slots = [('u', True, False, 'wavefield'), ('v', True, False, 'wavefield'), ('damp', False, True, 'function'),
+             ('snap', True, False, 'snapshot'), ('born_U', True, False, 'wavefield'),
+             ('born_du', True, False, 'wavefield'), ('born_dv', True, False, 'wavefield'),
+             ('born_dm', False, False, 'function'), ('grad', True, False, 'function'),
+             ('usave', False, False, 'saved'), ('vsave', False, False, 'saved')]
+    arrays = [Slot(m, p[m], w, lay, chk) for m, w, lay, chk in slots if p.get(m) is not None]
+    if kind == 'iso':
+        role, obj = p['m_role']
+        params = [Param('param', 'vp', obj, 1.0, role.startswith('m_'), True)]
+    elif kind == 'sa':
+        params = [Param(k, k + '_value', p[k + '_role'][1], 1.0, False, True) for k in ('b', 'vp')]
+    else:
+        params = [Param(n + '_arr', n, p['consts'].get(n), 1.0 if n == 'vp' else 0.0, False, False)
+                  for n in ('vp', 'epsilon', 'delta', 'theta', 'phi')]
+    flags = {'space_order': p['so'], 'radius': p['R'], 'adjoint': int(bool(p.get('adjoint'))),
+             'rec_toff': p['rec_toff']}
+    if kind != 'tti':
+        flags['ndim'] = p['grid'].dim
+    if kind == 'iso':
+        flags.update(free_surface=int(bool(p.get('free_surface'))), ot4=int(bool(p.get('ot4'))))
+        if p.get('snap') is not None:
+            flags.update(snap_factor=p['snap_factor'], snap_toff=p['snap_toff'])
+    weights = [(k, p[k]) for k in ('w', 'w2', 'w1', 'c') if k in p]
+    struct = {'iso': L_.IsoArgs, 'tti': L_.TtiArgs, 'sa': L_.SaArgs}[kind]
+    return Entry(f'b2_{kind}_forward', struct, flags, weights, arrays, params,
+                 ('u', 'damp', 'param') if kind == 'iso' else ())
+
+
+# ---------------------------------------------------------------------------------------------
 # the operator
 # ---------------------------------------------------------------------------------------------
 class Operator:
@@ -195,6 +271,7 @@ class Operator:
             warning(f"Operator `{name}` updates a second-order-in-time field but is not one of the schemes "
                     f"the CUDA path implements ({self._why_not}); it will run on the NumPy interpreter")
         self._interp = None if self._plan is not None else Interpreter(self._items, None, self._subs, name=name)
+        self._entry = wave_entry(self._plan) if self._plan is not None and self._plan['kind'] != 'linear' else None
         self._profiler_last = None
 
     def _looks_like_wave_propagation(self):
@@ -1373,8 +1450,7 @@ class Operator:
             taps = ', '.join(f"f[t{t:+d}]{list(o)}" for t, o, _ in p['taps'])
             return (f"/* Operator `{self.name}` -> libb200stencil.so::b2_linear_forward (sm_90a)\n"
                     f"   {p['u'].name}[t{p['wshift']:+d}] = sum_k c_k * ({taps}) */")
-        entry = {'iso': 'b2_iso_forward', 'tti': 'b2_tti_forward', 'sa': 'b2_sa_forward'}[p['kind']]
-        head = (f"/* Operator `{self.name}` -> libb200stencil.so::{entry} (sm_90a)\n"
+        head = (f"/* Operator `{self.name}` -> libb200stencil.so::{self._entry.symbol} (sm_90a)\n"
                 f"   space_order={p['so']} radius={p['R']} src={p['src'] and p['src'].name} "
                 f"rec={p['rec'] and p['rec'].name} rec_toff={p['rec_toff']}"
                 f"{' free_surface' if p.get('free_surface') else ''}{' OT4' if p.get('ot4') else ''} */\n")
@@ -1389,9 +1465,7 @@ class Operator:
         """The C-ABI entry point this operator calls (devito/operator/operator.py:857-869)."""
         if self._plan is None:
             raise InvalidOperator("interpreted operators have no C entry point")
-        L = L_.load_library()
-        return {'iso': L.b2_iso_forward, 'tti': L.b2_tti_forward, 'sa': L.b2_sa_forward,
-                'linear': L.b2_linear_forward}[self._plan['kind']]
+        return getattr(L_.load_library(), self._entry.symbol if self._entry else 'b2_linear_forward')
 
     def cinterface(self, force=False):
         """Write `<name>.c` / `<name>.h` under the JIT directory and return `(ccode, hcode)`
@@ -1419,19 +1493,7 @@ class Operator:
         if p['kind'] == 'linear':
             cs = {id(n): n for _, _, c in p['taps'] for n in c.preorder() if n.is_Constant}
             return (p['u'],) + tuple(cs.values())
-        out = [p['u']] + ([p['v']] if p['kind'] == 'tti' else [])
-        if p.get('damp') is not None:
-            out.append(p['damp'])
-        if p['kind'] == 'iso':
-            out.append(p['m_role'][1])
-        elif p['kind'] == 'sa':
-            out += [p['b_role'][1], p['vp_role'][1]]
-        else:
-            out.extend(p['consts'].values())
-        out += [p.get('born_U'), p.get('born_du'), p.get('born_dv'), p.get('born_dm'), p.get('snap')]
-        if p['kind'] == 'tti':
-            out += [p.get('grad'), p.get('usave'), p.get('vsave')]
-        out += [s for s in (p['src'], p['rec']) if s is not None]
+        out = [s.obj for s in self._entry.arrays] + [prm.obj for prm in self._entry.params] + [p['src'], p['rec']]
         return tuple(o for o in out if o is not None)
 
     # ------------------------------------------------------------------------------------------
@@ -1443,13 +1505,9 @@ class Operator:
     def apply(self, **kwargs):
         if self._plan is None:
             return self._apply_interp(**kwargs)
-        if self._plan['kind'] == 'iso':
-            return self._apply_iso(**kwargs)
         if self._plan['kind'] == 'linear':
             return self._apply_linear(**kwargs)
-        if self._plan['kind'] == 'sa':
-            return self._apply_sa(**kwargs)
-        return self._apply_tti(**kwargs)
+        return self._apply_wave(**kwargs)
 
     def arguments(self, **kwargs):
         if self._plan is None:
@@ -1578,115 +1636,61 @@ class Operator:
             post.append(writeback)
         return sh
 
+    @staticmethod
+    def _override_ok(check, f, so, grid):
+        """Whether `f` is what the kernel reads in a slot of this `check` (see `_OVERRIDE_KINDS`)."""
+        if check == 'function':
+            return isinstance(f, Function)
+        if not isinstance(f, TimeFunction):
+            return False
+        if check == 'wavefield':
+            return f.space_order == so and f.grid.shape == grid.shape
+        if check == 'saved':
+            return not f.is_buffered and f.space_order == so
+        return not f.is_buffered and f.grid.shape == grid.shape
+
+    def _resolve_param(self, kwargs, prm, so):
+        """A Function (passed as an array) or a float: the override by name of `prm.obj`, else `prm.obj`
+        itself. Without `prm.switch` the override keeps the kind the Operator was built with."""
+        obj = prm.obj
+        if obj is None:
+            return prm.unit
+        val = kwargs.pop(obj.name, obj)
+        if isinstance(obj, Function):
+            if isinstance(val, L_.ForeignDataobj):
+                val = self._foreign(obj, val)
+            elif isinstance(val, np.ndarray) and val.ndim:
+                val = self._shadow(obj, val, None)
+        if not prm.switch:
+            if isinstance(obj, Function) and (not isinstance(val, Function) or val.space_order != so):
+                raise InvalidArgument(f"`{obj.name}` must be overridden by a Function of the same space_order")
+            if not isinstance(obj, Function) and isinstance(val, Function):
+                raise InvalidArgument(f"array-valued `{obj.name}` needs an Operator built with a Function")
+        if isinstance(val, Function):
+            return val
+        if isinstance(val, np.ndarray) and val.ndim:
+            raise InvalidArgument(f"an array `{obj.name}` must have the allocated shape of a Function")
+        return float(val.data if isinstance(val, Constant) else val)
+
     def _prepare(self, kwargs):
-        p = self._plan
+        p, entry = self._plan, self._entry
         grid = p['grid']
-        nd = grid.dim
         args = OrderedDict()
         hold = []          # keep ctypes/ndarray objects alive during the call
         post = args['post'] = []     # run after the C call (write-back of ndarray overrides)
-        u = self._resolve(kwargs, p['u'], post)
-        fields = [u]
-        if p['kind'] == 'tti':
-            v = self._resolve(kwargs, p['v'], post)
-            fields.append(v)
-        for f in fields:
-            if not isinstance(f, TimeFunction) or f.space_order != p['so'] or f.grid.shape != grid.shape:
-                raise InvalidArgument(f"incompatible override for a wavefield")
-        args['fields'] = fields
-        damp = self._resolve(kwargs, p['damp'], post) if p.get('damp') is not None else None
-        if damp is not None and not isinstance(damp, Function):
-            raise InvalidArgument("`damp` override must be a Function")
-        args['damp'] = damp
-        args['snap'] = self._resolve(kwargs, p.get('snap'), post)
-        if args['snap'] is not None:
-            sn = args['snap']
-            if not isinstance(sn, TimeFunction) or sn.is_buffered or sn.grid.shape != grid.shape:
-                raise InvalidArgument("the snapshot override must be a saved TimeFunction on the same grid")
-        args['born_U'] = self._resolve(kwargs, p.get('born_U'), post)
-        args['born_du'] = self._resolve(kwargs, p.get('born_du'), post)
-        args['born_dv'] = self._resolve(kwargs, p.get('born_dv'), post)
-        args['born_dm'] = self._resolve(kwargs, p.get('born_dm'), post)
-        for key in ('born_du', 'born_dv'):
-            bu = args[key]
-            if bu is not None and (not isinstance(bu, TimeFunction) or bu.space_order != p['so'] or
-                                   bu.grid.shape != grid.shape):
-                raise InvalidArgument("incompatible override for a linearised wavefield")
-        if args['born_du'] is not None:
-            if not isinstance(args['born_dm'], Function):
-                raise InvalidArgument("`dm` must be a Function or an array of its allocated shape")
-            if grid.distributor.is_parallel:
-                raise InvalidArgument("TTI Born modelling does not run on a decomposed grid in this version")
-        if args['born_U'] is not None:
-            bu = args['born_U']
-            if not isinstance(bu, TimeFunction) or bu.space_order != p['so'] or bu.grid.shape != grid.shape:
-                raise InvalidArgument("incompatible override for the linearised wavefield")
-            if not isinstance(args['born_dm'], Function):
-                raise InvalidArgument("`dm` must be a Function or an array of its allocated shape")
-        args['grad'] = self._resolve(kwargs, p.get('grad'), post)
-        args['usave'] = self._resolve(kwargs, p.get('usave'), post)
-        args['vsave'] = self._resolve(kwargs, p.get('vsave'), post)
-        for us in (args['usave'], args['vsave']):
-            if us is not None and (not isinstance(us, TimeFunction) or us.is_buffered or us.space_order != p['so']):
-                raise InvalidArgument("the forward wavefield override must be a saved TimeFunction")
-        if p['kind'] == 'tti' and p.get('adjoint') and grid.distributor.is_parallel:
-            raise InvalidArgument("the TTI adjoint does not run on a decomposed grid in this version")
-        # parameters
-        if p['kind'] == 'iso':
-            kind, obj = p['m_role']
-            args['param_kind'] = B2_PARAM_SCALAR
-            args['param'] = None
-            args['vp'] = 1.0
-            if kind == 'one':
-                pass
-            else:
-                val = kwargs.pop(obj.name, obj)
-                if isinstance(val, L_.ForeignDataobj) and isinstance(obj, Function):
-                    val = self._foreign(obj, val)
-                elif isinstance(val, np.ndarray) and val.ndim and isinstance(obj, Function):
-                    val = self._shadow(obj, val, None)
-                if isinstance(val, Function):
-                    args['param'] = val
-                    args['param_kind'] = B2_PARAM_VP if kind.startswith('vp') else B2_PARAM_M
-                else:
-                    sval = float(val.data if isinstance(val, Constant) else val)
-                    args['vp'] = sval if kind.startswith('vp') else 1.0 / np.sqrt(sval)
-        elif p['kind'] == 'sa':
-            if grid.distributor.is_parallel:
+        for s in entry.arrays:
+            f = args[s.member] = self._resolve(kwargs, s.obj, post)
+            if not self._override_ok(s.check, f, p['so'], grid):
+                raise InvalidArgument(f"the override of `{s.obj.name}` must be {_OVERRIDE_KINDS[s.check]}")
+        args['fields'] = [args[m] for m in ('u', 'v') if m in args]
+        if grid.distributor.is_parallel:
+            if p['kind'] == 'sa':
                 raise InvalidArgument("the self-adjoint update does not run on a decomposed grid in this version")
-            for key in ('b', 'vp'):
-                kind, obj = p[key + '_role']
-                val = kwargs.pop(obj.name, obj)
-                if isinstance(val, L_.ForeignDataobj) and isinstance(obj, Function):
-                    val = self._foreign(obj, val)
-                elif isinstance(val, np.ndarray) and val.ndim and isinstance(obj, Function):
-                    val = self._shadow(obj, val, None)
-                if isinstance(val, Function):
-                    args['sa_' + key] = val
-                elif isinstance(val, np.ndarray) and val.ndim:
-                    raise InvalidArgument(f"an array `{obj.name}` must have the allocated shape of a Function")
-                else:
-                    args['sa_' + key] = float(val.data if isinstance(val, Constant) else val)
-        else:
-            args['tti_arrays'] = {}
-            for n, c in p['consts'].items():
-                val = kwargs.pop(n, c)
-                if isinstance(c, Function):
-                    if isinstance(val, L_.ForeignDataobj):
-                        val = self._foreign(c, val)
-                    elif isinstance(val, np.ndarray) and val.ndim:
-                        val = self._shadow(c, val, None)
-                    if not isinstance(val, Function) or val.space_order != p['so']:
-                        raise InvalidArgument(f"`{n}` must be overridden by a Function of the same space_order")
-                    args['tti_arrays'][n] = val
-                    args[n] = 0.0
-                else:
-                    if isinstance(val, Function):
-                        raise InvalidArgument(f"array-valued `{n}` needs an Operator built with a Function")
-                    args[n] = float(val.data if isinstance(val, Constant) else val)
-            args.setdefault('phi', 0.0)
-            if 'vp' in args['tti_arrays']:
-                args['vp'] = 1.0
+            if p['kind'] == 'tti' and p.get('adjoint'):
+                raise InvalidArgument("the TTI adjoint does not run on a decomposed grid in this version")
+            if 'born_du' in args:
+                raise InvalidArgument("TTI Born modelling does not run on a decomposed grid in this version")
+        args['params'] = [self._resolve_param(kwargs, prm, p['so']) for prm in entry.params]
         # spacing / dt
         dt = kwargs.pop('dt', None)
         if dt is None:
@@ -1720,11 +1724,8 @@ class Operator:
         args['src'], args['rec'] = src, rec
         # time range (devito/types/dimension.py:279-331)
         sized = [s for s in (src, rec) if s is not None]
-        sized += [f for f in fields if not f.is_buffered]
-        if args.get('usave') is not None:
-            sized.append(args['usave'])
-        if args.get('vsave') is not None:
-            sized.append(args['vsave'])
+        sized += [f for f in args['fields'] if not f.is_buffered]
+        sized += [args[s.member] for s in entry.arrays if s.check == 'saved']
         time_m = kwargs.pop('time_m', None)
         time_M = kwargs.pop('time_M', kwargs.pop('time', None))
         if time_m is None:
@@ -1767,11 +1768,9 @@ class Operator:
         return int(dev)
 
     @staticmethod
-    def _as_layout(fn, so, like):
-        """Host array of a parameter Function in the allocated layout of the wavefield
-        (halo `so`); parameters defined with a different space_order are re-padded."""
-        if fn.space_order == so:
-            return None
+    def _as_layout(fn, so):
+        """Host array of a parameter Function defined with another space_order, re-padded to the
+        allocated layout of the wavefield (halo `so`)."""
         src = fn.data_ro_with_halo
         h = fn.space_order
         dom = src[tuple(slice(h, src.shape[i] - h) for i in range(src.ndim))]
@@ -1784,7 +1783,8 @@ class Operator:
         return np.ascontiguousarray(out)
 
     def _field_obj(self, fn, dev, resident, hold, so=None, written=False, host_io_ok=False):
-        """b2_dataobj for a dense function: resident (dmap set) or host-staged."""
+        """(b2_dataobj for a dense function: resident (dmap set) or host-staged, whether it is host-staged
+        through the caller's device buffer (host_io))."""
         import torch
         fo = getattr(fn, '_foreign_obj', None)
         if fo is not None:
@@ -1793,9 +1793,9 @@ class Operator:
             if resident:
                 raise InvalidArgument("caller-built structs are host arrays: apply with resident=False")
             hold.append(fo)
-            return fo
+            return fo, False
         if so is not None and fn.space_order != so:
-            host = self._as_layout(fn, so, None)
+            host = self._as_layout(fn, so)
             hold.append(host)
             halo = tuple((0, 0) if d.is_Time else (so, so) for d in fn.dimensions)
             if resident:
@@ -1805,8 +1805,9 @@ class Operator:
             else:
                 ob = L_.make_dataobj(host=host, halo=halo)
             hold.append(ob)
-            return ob
+            return ob, False
         st = fn.storage
+        host_io = False
         if resident:
             dist_ = fn.grid.distributor if fn.grid is not None else None
             p2p_field = (written and dist_ is not None and dist_.is_parallel and distributed.p2p_enabled()
@@ -1833,11 +1834,11 @@ class Operator:
                 if getattr(fn, 'is_TimeFunction', False) and not st.p2p_registered:
                     distributed.register_field(st, fn.grid, dev)
                 ob = L_.make_dataobj(host=host, dev_ptr=t.data_ptr(), halo=fn.halo)
-                self._host_io = True
+                host_io = True
             else:
                 ob = L_.make_dataobj(host=host, halo=fn.halo)
         hold.append(ob)
-        return ob
+        return ob, host_io
 
     def _sparse_obj(self, sf, grid, hold, written=False, post=None, trange=None):
         """b2_sparse for a SparseTimeFunction. Under x-slab decomposition every rank holds all
@@ -1923,7 +1924,19 @@ class Operator:
         hold.extend([gp, ws, data, gpo, wos, s, host])
         return s
 
-    def _finish(self, rc, L, timers, args, nfields_pts, t_wall):
+    def _call(self, L, symbol, a, args, dev, post=()):
+        """Run entry point `symbol` on the filled argument block `a`, then the post-call hooks."""
+        a.deviceid = dev
+        timers = L_.Profiler()
+        a.timers = ctypes.pointer(timers)
+        t0 = _time.perf_counter()
+        rc = getattr(L, symbol)(ctypes.byref(a))
+        t_wall = _time.perf_counter() - t0
+        for fn in list(post) + args['post']:
+            fn()
+        return self._finish(rc, L, timers, args, t_wall)
+
+    def _finish(self, rc, L, timers, args, t_wall):
         if rc != 0:
             msg = L.b2_last_error().decode()
             if rc == 100:
@@ -1979,33 +1992,41 @@ class Operator:
             arr[i] = a.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
         return arr
 
-    def _apply_iso(self, **kwargs):
+    def _apply_wave(self, **kwargs):
         L = L_.lib()
         args, hold = self._prepare(dict(kwargs))
-        p = self._plan
+        p, entry = self._plan, self._entry
         grid = p['grid']
-        nd = grid.dim
         dev = self._device(args)
         res = args['resident']
-        a = L_.IsoArgs()
-        a.ndim = nd
-        a.space_order = p['so']
-        a.radius = p['R']
-        a.w = self._w_arrays(p['w'], hold)
-        u = args['fields'][0]
-        self._host_io = False
-        a.u = self._field_obj(u, dev, res, hold, written=True, host_io_ok=True).ptr
-        a.damp = (self._field_obj(args['damp'], dev, res, hold, so=p['so'], host_io_ok=True).ptr
-                  if args['damp'] is not None else None)
-        a.param_kind = args['param_kind']
-        a.param = (self._field_obj(args['param'], dev, res, hold, so=p['so'], host_io_ok=True).ptr
-                   if args['param'] is not None else None)
-        a.vp = args['vp']
+        a = entry.struct()
+        for k, v in entry.flags.items():
+            setattr(a, k, v)
+        for member, w in entry.weights:
+            setattr(a, member, self._w_arrays(w, hold))
+        host_io = False
+        for s in entry.arrays:
+            ob, hio = self._field_obj(args[s.member], dev, res, hold, so=p['so'] if s.layout else None,
+                                      written=s.written, host_io_ok=s.member in entry.host_io)
+            setattr(a, s.member, ob.ptr)
+            host_io |= hio
+        for prm, val in zip(entry.params, args['params']):
+            if isinstance(val, Function):
+                ob, hio = self._field_obj(val, dev, res, hold, so=p['so'], host_io_ok=prm.member in entry.host_io)
+                setattr(a, prm.member, ob.ptr)
+                setattr(a, prm.scalar, prm.unit)
+                host_io |= hio
+            else:
+                setattr(a, prm.scalar, 1.0 / np.sqrt(val) if prm.slowness else val)
+            if prm.member == 'param':
+                a.param_kind = (B2_PARAM_SCALAR if not isinstance(val, Function) else
+                                B2_PARAM_M if prm.slowness else B2_PARAM_VP)
+        if entry.host_io:
+            a.host_io = int(host_io)
         a.dt = args['dt']
-        lo, hi = args['lo'], args['hi']
-        a.x_m, a.x_M, a.y_m, a.y_M = lo[0], hi[0], lo[1], hi[1]
-        if nd == 3:
-            a.z_m, a.z_M = lo[2], hi[2]
+        for ax, lo, hi in zip('xyz', args['lo'], args['hi']):
+            setattr(a, ax + '_m', lo)
+            setattr(a, ax + '_M', hi)
         a.time_m, a.time_M = args['time_m'], args['time_M']
         s = self._sparse_obj(args['src'], grid, hold)
         post = []
@@ -2013,83 +2034,15 @@ class Operator:
                              trange=(args['time_m'], args['time_M']))
         a.src = ctypes.pointer(s) if s is not None else None
         a.rec = ctypes.pointer(r) if r is not None else None
-        a.rec_toff = p['rec_toff']
         a.errctl = args['errctl']
-        a.deviceid = dev
         a.kernel = args['kernel']
-        a.halo = distributed.halo_context(dev) if grid.distributor.is_parallel else None
-        timers = L_.Profiler()
-        a.timers = ctypes.pointer(timers)
-        a.adjoint = 1 if p.get('adjoint') else 0
-        a.free_surface = 1 if p.get('free_surface') else 0
-        a.ot4 = 1 if p.get('ot4') else 0
-        if args.get('snap') is not None:
-            a.snap = self._field_obj(args['snap'], dev, res, hold, written=True).ptr
-            a.snap_factor = p['snap_factor']
-            a.snap_toff = p['snap_toff']
-        if args.get('born_U') is not None:
-            a.born_U = self._field_obj(args['born_U'], dev, res, hold, written=True).ptr
-            a.born_dm = self._field_obj(args['born_dm'], dev, res, hold).ptr
-        if args.get('grad') is not None:
-            a.grad = self._field_obj(args['grad'], dev, res, hold, written=True).ptr
-            a.usave = self._field_obj(args['usave'], dev, res, hold).ptr
+        if grid.distributor.is_parallel:
+            a.halo = distributed.halo_context(dev)
         if p.get('inject_literal'):
             # injection used a literal dt**2 (not the `dt` symbol): it must agree with runtime dt
             if abs(p['inject_dt2'] - a.dt * a.dt) > 1e-5 * p['inject_dt2']:
                 raise InvalidArgument("literal dt in the injected expression differs from runtime dt")
-        a.host_io = 1 if self._host_io else 0
-        t0 = _time.perf_counter()
-        rc = L.b2_iso_forward(ctypes.byref(a))
-        t_wall = _time.perf_counter() - t0
-        for fn in post + args['post']:
-            fn()
-        return self._finish(rc, L, timers, args, 1, t_wall)
-
-    def _apply_sa(self, **kwargs):
-        L = L_.lib()
-        args, hold = self._prepare(dict(kwargs))
-        p = self._plan
-        grid = p['grid']
-        nd = grid.dim
-        dev = self._device(args)
-        res = args['resident']
-        a = L_.SaArgs()
-        a.ndim = nd
-        a.space_order = p['so']
-        a.radius = p['R']
-        a.c = self._w_arrays(p['c'], hold)
-        a.u = self._field_obj(args['fields'][0], dev, res, hold, written=True).ptr
-        for key in ('b', 'vp'):
-            val = args['sa_' + key]
-            if isinstance(val, Function):
-                setattr(a, key, self._field_obj(val, dev, res, hold, so=p['so']).ptr)
-                setattr(a, key + '_value', 1.0)
-            else:
-                setattr(a, key + '_value', val)
-        a.damp = self._field_obj(args['damp'], dev, res, hold, so=p['so']).ptr if args['damp'] is not None else None
-        a.dt = args['dt']
-        lo, hi = args['lo'] + [0] * (3 - nd), args['hi'] + [0] * (3 - nd)
-        a.x_m, a.x_M, a.y_m, a.y_M, a.z_m, a.z_M = lo[0], hi[0], lo[1], hi[1], lo[2], hi[2]
-        a.time_m, a.time_M = args['time_m'], args['time_M']
-        s = self._sparse_obj(args['src'], grid, hold)
-        post = []
-        r = self._sparse_obj(args['rec'], grid, hold, written=True, post=post,
-                             trange=(args['time_m'], args['time_M']))
-        a.src = ctypes.pointer(s) if s is not None else None
-        a.rec = ctypes.pointer(r) if r is not None else None
-        a.rec_toff = p['rec_toff']
-        a.adjoint = 1 if p.get('adjoint') else 0
-        a.errctl = args['errctl']
-        a.deviceid = dev
-        a.kernel = args['kernel']
-        timers = L_.Profiler()
-        a.timers = ctypes.pointer(timers)
-        t0 = _time.perf_counter()
-        rc = L.b2_sa_forward(ctypes.byref(a))
-        t_wall = _time.perf_counter() - t0
-        for fn in post + args['post']:
-            fn()
-        return self._finish(rc, L, timers, args, 1, t_wall)
+        return self._call(L, entry.symbol, a, args, dev, post)
 
     # -- generic constant-coefficient update ------------------------------------------------------
     def _prepare_linear(self, kwargs):
@@ -2164,7 +2117,7 @@ class Operator:
         hold = []
         a = L_.LinearArgs()
         a.ndim = nd
-        a.f = self._field_obj(args['fields'][0], dev, args['resident'], hold, written=True).ptr
+        a.f = self._field_obj(args['fields'][0], dev, args['resident'], hold, written=True)[0].ptr
         a.halo = p['so']
         taps = (L_.Tap * len(args['taps']))()
         for i, (t, o, c) in enumerate(args['taps']):
@@ -2178,68 +2131,7 @@ class Operator:
         lo, hi = args['lo'] + [0] * (3 - nd), args['hi'] + [0] * (3 - nd)
         a.x_m, a.x_M, a.y_m, a.y_M, a.z_m, a.z_M = lo[0], hi[0], lo[1], hi[1], lo[2], hi[2]
         a.time_m, a.time_M = args['time_m'], args['time_M']
-        a.deviceid = dev
-        timers = L_.Profiler()
-        a.timers = ctypes.pointer(timers)
-        t0 = _time.perf_counter()
-        rc = L.b2_linear_forward(ctypes.byref(a))
-        t_wall = _time.perf_counter() - t0
-        for fn in args['post']:
-            fn()
-        return self._finish(rc, L, timers, args, 1, t_wall)
-
-    def _apply_tti(self, **kwargs):
-        L = L_.lib()
-        args, hold = self._prepare(dict(kwargs))
-        p = self._plan
-        grid = p['grid']
-        dev = self._device(args)
-        res = args['resident']
-        a = L_.TtiArgs()
-        a.space_order = p['so']
-        a.radius = p['R']
-        a.w2 = self._w_arrays(p['w2'], hold)
-        a.w1 = self._w_arrays(p['w1'], hold)
-        u, v = args['fields']
-        a.u = self._field_obj(u, dev, res, hold, written=True).ptr
-        a.v = self._field_obj(v, dev, res, hold, written=True).ptr
-        a.damp = self._field_obj(args['damp'], dev, res, hold, so=p['so']).ptr if args['damp'] is not None else None
-        a.vp, a.epsilon, a.delta = args['vp'], args['epsilon'], args['delta']
-        a.theta, a.phi = args['theta'], args['phi']
-        for n, fn in args['tti_arrays'].items():
-            setattr(a, n + '_arr', self._field_obj(fn, dev, res, hold, so=p['so']).ptr)
-        a.dt = args['dt']
-        lo, hi = args['lo'], args['hi']
-        a.x_m, a.x_M, a.y_m, a.y_M, a.z_m, a.z_M = lo[0], hi[0], lo[1], hi[1], lo[2], hi[2]
-        a.time_m, a.time_M = args['time_m'], args['time_M']
-        s = self._sparse_obj(args['src'], grid, hold)
-        post = []
-        r = self._sparse_obj(args['rec'], grid, hold, written=True, post=post,
-                             trange=(args['time_m'], args['time_M']))
-        a.src = ctypes.pointer(s) if s is not None else None
-        a.rec = ctypes.pointer(r) if r is not None else None
-        a.rec_toff = p['rec_toff']
-        a.errctl = args['errctl']
-        a.deviceid = dev
-        a.kernel = args['kernel']
-        a.halo = distributed.halo_context(dev) if grid.distributor.is_parallel else None
-        if args.get('born_du') is not None:
-            a.born_du = self._field_obj(args['born_du'], dev, res, hold, written=True).ptr
-            a.born_dv = self._field_obj(args['born_dv'], dev, res, hold, written=True).ptr
-            a.born_dm = self._field_obj(args['born_dm'], dev, res, hold).ptr
-        a.adjoint = 1 if p.get('adjoint') else 0
-        if args.get('grad') is not None:
-            a.grad = self._field_obj(args['grad'], dev, res, hold, written=True).ptr
-            a.usave = self._field_obj(args['usave'], dev, res, hold).ptr
-            a.vsave = self._field_obj(args['vsave'], dev, res, hold).ptr
-        timers = L_.Profiler()
-        a.timers = ctypes.pointer(timers)
-        t0 = _time.perf_counter()
-        rc = L.b2_tti_forward(ctypes.byref(a))
-        t_wall = _time.perf_counter() - t0
-        for fn in post + args['post']:
-            fn()
-        return self._finish(rc, L, timers, args, 2, t_wall)
+        return self._call(L, 'b2_linear_forward', a, args, dev)
 
 
 # ---------------------------------------------------------------------------------------------

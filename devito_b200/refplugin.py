@@ -712,17 +712,12 @@ class B200CudaOperator(Cpu64AdvOmpOperator):
             hold.append(fo)
             return fo
 
-        fields = [p['u']] + ([p['v']] if p['kind'] == 'tti' else [])
-        for f in fields + [p.get(k) for k in ('damp', 'usave', 'grad', 'born_U', 'born_dm', 'snap')]:
-            if f is not None:
-                ov[f.name] = dataobj(f.name)
-        if p['kind'] == 'iso':
-            kind, obj = p['m_role']
-            if obj is not None:
-                ov[obj.name] = dataobj(obj.name) if kind.endswith('_f') else float(args[obj.name])
-        else:
-            for n, c in p['consts'].items():
-                ov[n] = dataobj(n) if hasattr(c, 'space_order') else float(args[n])
+        for s in shadow._entry.arrays:
+            ov[s.obj.name] = dataobj(s.obj.name)
+        for prm in shadow._entry.params:
+            if prm.obj is not None:
+                n = prm.obj.name
+                ov[n] = dataobj(n) if hasattr(prm.obj, 'space_order') else float(args[n])
         for key in ('src', 'rec'):
             sf = p.get(key)
             if sf is None:

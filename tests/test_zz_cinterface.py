@@ -78,7 +78,8 @@ def _build_against_stub(jitdir, name):
     tag = f'stub_{name}_{os.path.basename(jitdir)}'.replace('-', '_')
     # the entry points are renamed on both sides so that the real library, when another test has
     # already loaded it with RTLD_GLOBAL, cannot interpose them
-    ren = ['-Db2_iso_forward=double_b2_iso_forward', '-Db2_tti_forward=double_b2_tti_forward']
+    ren = ['-Db2_iso_forward=double_b2_iso_forward', '-Db2_tti_forward=double_b2_tti_forward',
+           '-Db2_sa_forward=double_b2_sa_forward']
     _cc(['-O1', '-shared', '-fPIC', '-Wall', '-Werror', '-I', INCLUDE] + ren + [STUB_SRC, '-o', f'lib{tag}.so'],
         jitdir)
     _cc(['-O1', '-shared', '-fPIC', '-Wall', '-Werror', '-I', INCLUDE, '-I', jitdir] + ren + [f'{name}.c',
