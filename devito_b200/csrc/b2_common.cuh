@@ -4,6 +4,7 @@
 #include <cuda.h>
 #include <cstdio>
 #include <cstdint>
+#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <deque>
@@ -76,6 +77,12 @@ inline int choose_chunk_len(long long sms, int tiles, int xcount, int prime, int
         if (cost < best - 1e-9) { best = cost; best_n = n; }
     }
     return (xcount + best_n - 1) / best_n;
+}
+
+// integer value of the environment variable `name` (read per call), or `dflt` when it is unset
+inline int env_int(const char *name, int dflt) {
+    const char *v = getenv(name);
+    return v ? atoi(v) : dflt;
 }
 
 #define B2_CUDA(call, code)                                                        \

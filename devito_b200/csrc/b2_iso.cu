@@ -465,11 +465,6 @@ template <> struct TileOf<4, true> { static constexpr int TY = 32, TZ4 = 16; };
 template <bool ARR> struct TileOf<6, ARR> { static constexpr int TY = 16, TZ4 = 16; };
 template <bool ARR> struct TileOf<8, ARR> { static constexpr int TY = 8, TZ4 = 16; };
 
-static int env_int(const char *name, int dflt) {
-    const char *v = getenv(name);
-    return v ? atoi(v) : dflt;
-}
-
 // scratch for the coefficient arrays, cached across calls (re-allocated when the size changes)
 static float *g_coef[3] = {nullptr, nullptr, nullptr};     // A, B (TMA path), W (OT4)
 static size_t g_coef_elems[3] = {0, 0, 0};

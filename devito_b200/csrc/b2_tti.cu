@@ -197,19 +197,17 @@ struct TtiFK {
     const float *__restrict__ tE2;
     const float *__restrict__ tSD;
     const float *__restrict__ tMD;
-    int ay, az;                // allocated extents of dims 1, 2 (bounds of the table reads on the extended tile)
-    int pfc;                   // != 0: prefetch next iteration's stage-A factor groups into L2
     int hint;                  // != 0: once-per-CTA table reads bypass L1 allocation
     // ADJ: the centre of the update, p[t] / r[t]; the tensor maps then cover the mixes of the adjoint plan
     const float *__restrict__ pc;
     const float *__restrict__ rc;
 };
 
-// D = how many batches the producer may run ahead of the slowest consumer (ring depths follow); CT = the array-
-// parameter variant that stages the rotation-factor tiles of stage A through shared memory by TMA (two planes of
-// three tables, paid for with one batch less of u / v prefetch)
-template <int R, int TY, int D = 3, int CT = 0>
+// ARR: the array-parameter sweep, which stages the rotation-factor tiles through shared memory by TMA (a ring of
+// three tables per plane, paid for with one batch less of u / v prefetch)
+template <int R, int TY, bool ARR = false>
 struct TtiCfg {
+    static constexpr int D = ARR ? 2 : 3;            // batches the producer may run ahead of the slowest consumer
     static constexpr int H = R / 2;
     static constexpr int TZ4 = 16, TZ = 64, RZ = 4;
     static constexpr int PR = TY + 2 * R;            // rows of a u/v plane box
@@ -225,32 +223,29 @@ struct TtiCfg {
     static constexpr int NCT = TY * TZ4;             // consumer threads
     static constexpr int NCW = NCT / 32;
     static constexpr int GGROUPS = (TY + R - 1) * (BZ / 4);   // float4 groups of the extended tile
-    // factor-tile ring: CT = 1 holds stage A's plane x+H-1 and the one in flight; CT = 2 also keeps the planes down to x
-    // for stage B (H live planes + the one in flight)
-    static constexpr int NCT_PLANES = CT == 0 ? 0 : (CT == 1 ? 2 : H + 1);
+    // factor-tile ring: stage A's plane x+H-1 and the planes down to x for stage B (H live planes + the one in flight)
+    static constexpr int NCT_PLANES = ARR ? H + 1 : 0;
     static constexpr size_t SMEM = (size_t)((NUU + NUV) * PLANE + (2 * NG + 3 * NCT_PLANES) * GPLANE) * 4 + 2 * NB * 8 + 128;
 };
 
 // ARR = true: array-valued vp / epsilon / delta / theta / phi (`layers-tti`). The rotation factors are sampled where
 // the reference samples them — at the Gz point inside Gz, at the shifted point in the outer derivative — from the
-// per-point tables of k_tti_tables, read through L1 (`ld.global.nc`): stage A loads cx, cy, cz of its float4 group,
-// stage B keeps cx of its own column in a register queue along x and loads cy of the R rows / cz of the z segment
-// around its four points; (1+2eps), sqrt(1+2delta), m/dt^2 and A come with u[t-1], v[t-1] at the top of the
-// iteration. 52 B/point instead of 28.
-// CT = true (needs ARR): cx, cy, cz of stage A's plane arrive by TMA with the u / v batch instead (boxes of the
-// extended tile, zero-filled outside the array), so stage A has no global loads at all.
+// per-point tables of k_tti_tables. cx, cy, cz of stage A's plane arrive by TMA with the u / v batch (boxes of the
+// extended tile, zero-filled outside the array) in a ring of R/2 + 1 planes, so stage A has no global loads at all;
+// stage B keeps cx of its own column in a register queue along x and reads cy of the R rows / cz of the z segment
+// around its four points from the ring's plane x. (1+2eps), sqrt(1+2delta), m/dt^2 and A come with u[t-1], v[t-1]
+// at the top of the iteration. 52 B/point instead of 28.
 // ADJ: the adjoint step. The tensor maps cover the mixes a = e2 p + sd r, b = sd p + r, combined with e2 = 1, sd = 0;
 // the centre of the time update is loaded from p[t], r[t] (with ARR in place of the e2 / sd tables, so the array
 // kernel moves the same bytes as the forward one).
-template <int R, int TY, bool ARR, int CT, bool ADJ = false>
+template <int R, int TY, bool ARR, bool ADJ = false>
 __global__ void __launch_bounds__(TY * 16 + 32, 1)
 k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_v,
             const __grid_constant__ CUtensorMap tm_cx, const __grid_constant__ CUtensorMap tm_cy,
             const __grid_constant__ CUtensorMap tm_cz, const TtiFK k) {
-    static_assert(!CT || ARR, "factor tiles exist only with array-valued parameters");
-    constexpr int D = CT ? 2 : 3;
-    constexpr int NCP = (CT == 0 ? 1 : (CT == 1 ? 2 : R / 2 + 1));   // planes of the factor-tile ring
-    using C = TtiCfg<R, TY, D, CT>;
+    using C = TtiCfg<R, TY, ARR>;
+    constexpr int D = C::D;
+    constexpr int NCP = ARR ? C::NCT_PLANES : 1;    // planes of the factor-tile ring
     constexpr int H = C::H, TZ = C::TZ, RZ = C::RZ, BZ = C::BZ, PR = C::PR, GR = C::GR;
     constexpr int NUU = C::NUU, NUV = C::NUV, NG = C::NG, NB = C::NB;
     constexpr int PLANE = C::PLANE, GPLANE = C::GPLANE, NCT = C::NCT, NCW = C::NCW;
@@ -261,7 +256,7 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     float *s_v = s_u + NUU * PLANE;
     float *s_gu = s_v + NUV * PLANE;
     float *s_gv = s_gu + NG * GPLANE;
-    float *s_c = s_gv + NG * GPLANE;                // CT: [plane mod NCP][cx, cy, cz][GPLANE]
+    float *s_c = s_gv + NG * GPLANE;                // ARR: [plane mod NCP][cx, cy, cz][GPLANE]
     uint64_t *full = reinterpret_cast<uint64_t *>(s_c + 3 * C::NCT_PLANES * GPLANE);
     uint64_t *empty = full + NB;
 
@@ -293,7 +288,7 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
             b2ptx::tma_prefetch_desc(&tm_v);
             // batch `it` carries u plane (x+R) and v plane (x+R-1) of iteration x = xs-PRE+it.
             // Its slots were last read in iteration it-3 (u plane x-3+R... see DESIGN.md §3.3).
-            if constexpr (CT) {
+            if constexpr (ARR) {
                 b2ptx::tma_prefetch_desc(&tm_cx);
                 b2ptx::tma_prefetch_desc(&tm_cy);
                 b2ptx::tma_prefetch_desc(&tm_cz);
@@ -307,9 +302,9 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
                 const int pu = x + R;                    // u plane index (relative to origin)
                 const int pv = x + R - 1;
                 const bool hv = pv >= xs - (R - 1);      // v planes below xs-R+1 are never used
-                // CT: factor tiles of stage A's plane x+H-1; their slot held plane x+H-1-NCP, last read (stage A with CT = 1,
-                // stage B with CT = 2) in iteration it-2
-                const bool hc = CT && (x + H - 1 >= xs - H);
+                // ARR: factor tiles of stage A's plane x+H-1; their slot held plane x+H-1-NCP, last read (by stage B) in
+                // iteration it-2
+                const bool hc = ARR && (x + H - 1 >= xs - H);
                 b2ptx::mbar_arrive_expect_tx(&full[it % NB], (uint32_t)(PR * BZ * 4) * (hv ? 2u : 1u) +
                                                                  (hc ? (uint32_t)(3 * C::GR * BZ * 4) : 0u));
                 b2ptx::tma_load_4d(s_u + ((pu % NUU + NUU) % NUU) * PLANE, &tm_u, &full[it % NB],
@@ -317,7 +312,7 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
                 if (hv)
                     b2ptx::tma_load_4d(s_v + ((pv % NUV + NUV) % NUV) * PLANE, &tm_v, &full[it % NB],
                                        k.oz + z0 - RZ, k.oy + y0 - R, k.ox + pv, k.slot0);
-                if constexpr (CT) {
+                if constexpr (ARR) {
                     if (hc) {
                         float *dst = s_c + (((x + H - 1) % NCP + NCP) % NCP) * 3 * GPLANE;
                         b2ptx::tma_load_4d(dst, &tm_cx, &full[it % NB], k.oz + z0 - RZ, k.oy + y0 - H, k.ox + x + H - 1, 0);
@@ -348,7 +343,6 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     // [-H, H-1], dealt round-robin; packed as poff | fv<<16 | has_left<<17 | has_right<<18 | valid<<19
     constexpr int NTASK = (2 * C::GGROUPS + NCT - 1) / NCT;
     int tdesc[NTASK];
-    int tcoff[(ARR && !CT) ? NTASK : 1];        // ARR without CT: offset of the group inside an x plane of the tables, -1 = outside the array
 #pragma unroll
     for (int t = 0; t < NTASK; ++t) {
         const int task = tid + t * NCT;
@@ -359,11 +353,6 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
         const int poff = (gr + R - H) * BZ + 4 * gc;
         tdesc[t] = poff | (fv ? 1 << 16 : 0) | (gc > 0 ? 1 << 17 : 0) | (gc < BZ / 4 - 1 ? 1 << 18 : 0) |
                    (valid ? 1 << 19 : 0);
-        if constexpr (ARR && !CT) {
-            const int ay_ = k.oy + y0 - H + gr, az_ = k.oz + z0 - RZ + 4 * gc;
-            tcoff[t] = (valid && ay_ >= 0 && ay_ < k.ay && az_ >= 0 && az_ + 4 <= k.az)
-                           ? (int)((long long)ay_ * k.sy + az_) : -1;
-        }
     }
     float4 cxq[ARR ? R : 1];           // ARR: cx of the own column at planes x-H .. x+H-1
     if constexpr (ARR) {
@@ -375,9 +364,9 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     // ring positions of plane x (updated incrementally; x starts at xs - PRE)
     int iu = ((xs - PRE) % NUU + NUU) % NUU, iv = ((xs - PRE) % NUV + NUV) % NUV,
         ig = ((xs - PRE) % NG + NG) % NG;
-    int ic = ((xs - PRE) % NCP + NCP) % NCP;        // CT: ring slot of factor plane x
+    int ic = ((xs - PRE) % NCP + NCP) % NCP;        // ARR: ring slot of factor plane x
     auto wrap = [](int v, int n) { return v >= n ? v - n : v; };
-    // per-point tables read once per CTA: optionally kept out of L1, which the row / segment reads of cy, cz reuse
+    // per-point tables read once per CTA: optionally kept out of L1
     const bool stream_hint = ARR && k.hint != 0;
     auto ldt = [&](const float *q) -> float4 {
         float4 r;
@@ -435,28 +424,11 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
                 }
                 pmd = ldt(k.tMD + gi);
             }
-            // stage A of the NEXT iteration reads cx, cy, cz of plane x+H for the first time: ask L2 for them now
-            if constexpr (!CT) {
-                if (k.pfc && x + H >= xs - H) {
-                    const long long cb = (long long)(k.ox + x + H) * k.sx;
-#pragma unroll
-                    for (int t = 0; t < NTASK; ++t)
-                        if (tcoff[t] >= 0 && !(tdesc[t] & (1 << 16))) {
-                            asm volatile("prefetch.global.L2 [%0];" ::"l"(k.tCx + cb + tcoff[t]));
-                            asm volatile("prefetch.global.L2 [%0];" ::"l"(k.tCy + cb + tcoff[t]));
-                            asm volatile("prefetch.global.L2 [%0];" ::"l"(k.tCz + cb + tcoff[t]));
-                        }
-                }
-            }
 #pragma unroll
             for (int i = 0; i < R - 1; ++i) cxq[i] = cxq[i + 1];
-            if constexpr (CT != 2) {
-                if (x + H - 1 >= xs - H && zcnt > 0)
-                    cxq[R - 1] = ldt(k.tCx + gi + (long long)(H - 1) * k.sx);
-            }
         }
         b2ptx::mbar_wait(&full[it % NB], (it / NB) & 1);
-        if constexpr (CT == 2) {                     // own column of the cx tile that just landed (plane x+H-1)
+        if constexpr (ARR) {                         // own column of the cx tile that just landed (plane x+H-1)
             if (x + H - 1 >= xs - H)
                 cxq[R - 1] = b2ptx::lds128(s_c + wrap(ic + H - 1, NCP) * 3 * GPLANE + my_goff);
         }
@@ -485,18 +457,11 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
                 const int poff = d & 0xffff;
                 float4 rr = make_float4(0, 0, 0, 0);
                 float4 c4x = rr, c4y = rr, c4z = rr, ry = rr, rz = rr;   // ARR: factors at the Gz point; D+y, D+z kept apart
-                if constexpr (CT) {
+                if constexpr (ARR) {
                     const float *cs = s_c + wrap(ic + H - 1, NCP) * 3 * GPLANE + poff - (R - H) * BZ;
                     c4x = b2ptx::lds128(cs);
                     c4y = b2ptx::lds128(cs + GPLANE);
                     c4z = b2ptx::lds128(cs + 2 * GPLANE);
-                } else if constexpr (ARR) {
-                    if (tcoff[t] >= 0) {
-                        const long long ci = (long long)(k.ox + x + H - 1) * k.sx + tcoff[t];
-                        c4x = __ldg(reinterpret_cast<const float4 *>(k.tCx + ci));
-                        c4y = __ldg(reinterpret_cast<const float4 *>(k.tCy + ci));
-                        c4z = __ldg(reinterpret_cast<const float4 *>(k.tCz + ci));
-                    }
                 }
 #pragma unroll
                 for (int j = 0; j < R; ++j) {                // x taps
@@ -538,7 +503,7 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
 
         // ---- stage B: output plane x ----
         if (x >= xs) {
-            if constexpr (ADJ && ARR && CT != 0) {   // in place of the e2 / sd tables; issued here, where registers are free
+            if constexpr (ADJ && ARR) {              // in place of the e2 / sd tables; issued here, where registers are free
                 if (zcnt > 0) {
                     pcn = ldt(k.pc + gi);
                     rcn = ldt(k.rc + gi);
@@ -547,7 +512,7 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
             // ARR: cy at the R rows and cz on the z segment around the four points, issued ahead of their use
             float4 cyq[ARR ? R : 1];
             float czr[ARR ? 12 : 1];
-            if constexpr (CT == 2) {               // plane x of the factor ring: rows y-H+j of cy, z segment of cz
+            if constexpr (ARR) {                   // plane x of the factor ring: rows y-H+j of cy, z segment of cz
                 const float *cb = s_c + ic * 3 * GPLANE + my_goff;
 #pragma unroll
                 for (int j = 0; j < R; ++j) cyq[j] = b2ptx::lds128(cb + GPLANE + (j - H) * BZ);
@@ -555,22 +520,6 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
                              r = b2ptx::lds128(cb + 2 * GPLANE + 4);
                 czr[0] = l.x; czr[1] = l.y; czr[2] = l.z; czr[3] = l.w; czr[4] = cc.x; czr[5] = cc.y; czr[6] = cc.z;
                 czr[7] = cc.w; czr[8] = r.x; czr[9] = r.y; czr[10] = r.z; czr[11] = r.w;
-            } else if constexpr (ARR) {
-                if (zcnt > 0) {
-#pragma unroll
-                    for (int j = 0; j < R; ++j)
-                        cyq[j] = __ldg(reinterpret_cast<const float4 *>(k.tCy + gi + (long long)(j - H) * k.sy));
-                    const float4 l = __ldg(reinterpret_cast<const float4 *>(k.tCz + gi - 4));
-                    const float4 cc = __ldg(reinterpret_cast<const float4 *>(k.tCz + gi));
-                    const float4 r = __ldg(reinterpret_cast<const float4 *>(k.tCz + gi + 4));
-                    czr[0] = l.x; czr[1] = l.y; czr[2] = l.z; czr[3] = l.w; czr[4] = cc.x; czr[5] = cc.y; czr[6] = cc.z;
-                    czr[7] = cc.w; czr[8] = r.x; czr[9] = r.y; czr[10] = r.z; czr[11] = r.w;
-                } else {
-#pragma unroll
-                    for (int j = 0; j < R; ++j) cyq[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                    for (int j = 0; j < 12; ++j) czr[j] = 0.f;
-                }
             }
             const float *cpl = s_u + iu * PLANE + my_off;   // u plane x, own column
             const float4 c = uq[R];
@@ -655,12 +604,6 @@ k_tti_fused(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
                         zv4.x = fmaf(w, av[o + 0], zv4.x); zv4.y = fmaf(w, av[o + 1], zv4.y);
                         zv4.z = fmaf(w, av[o + 2], zv4.z); zv4.w = fmaf(w, av[o + 3], zv4.w);
                     }
-                }
-            }
-            if constexpr (ADJ && ARR && CT == 0) {   // CT = 0 holds the factor queues longest: load just before use
-                if (zcnt > 0) {
-                    pcn = ldt(k.pc + gi);
-                    rcn = ldt(k.rc + gi);
                 }
             }
             float4 ou, ov;
@@ -1102,16 +1045,12 @@ constexpr int kTtiWsTY = 24;
 template <int R> struct TtiTile;
 template <> struct TtiTile<2> { static constexpr int TY = 32; };
 template <> struct TtiTile<4> { static constexpr int TY = 28; };
-// array-parameter variant: more live registers per thread (factor queue, per-point tables). Warps are allocated in
-// fours, so 22 rows (11 + 1 warps -> 168 registers) and 30 rows (15 + 1 warps -> 128) are the sizes below 16 / 20 warps
-template <int R> struct TtiTileArr;
-template <> struct TtiTileArr<2> { static constexpr int TY = 30; };
-template <> struct TtiTileArr<4> { static constexpr int TY = 22; };
-// ... and with the three-plane factor ring of CT = 2 (shared memory: 220 KB at 20 rows)
-template <int R> struct TtiTileArr2;
-template <> struct TtiTileArr2<2> { static constexpr int TY = 30; };
-template <> struct TtiTileArr2<4> { static constexpr int TY = 20; };
-static int env_int_tti(const char *name, int dflt);
+// array-parameter sweep: more live registers per thread (factor queue, per-point tables) and the factor ring in shared
+// memory. 30 rows at radius 2 (15 + 1 warps -> at most 128 registers); 20 rows at radius 4, the most whose rings fit in
+// shared memory (220 KB)
+template <int R> struct TtiArrTile;
+template <> struct TtiArrTile<2> { static constexpr int TY = 30; };
+template <> struct TtiArrTile<4> { static constexpr int TY = 20; };
 
 // scratch cached across calls
 // 0: A, 1-2: Gz(u), Gz(v) (two-pass), 3-8: per-point tables, 9-10: the adjoint's mixes
@@ -1139,10 +1078,10 @@ int tti_plan_init(TtiPlan &p, int kernel) {
     bool ok = (p.R == 2 || p.R == 4) && (p.a[2] % 4 == 0) && (p.o[2] % 4 == 0) &&
               ((uintptr_t)p.u % 16 == 0) && ((uintptr_t)p.v % 16 == 0) && (p.slot_elems % 4 == 0) &&
               p.n[1] >= 8 && p.n[2] >= 16;
-    // array-valued parameters: the fused kernel reads the per-point tables with 16-byte loads one group left and
-    // right of its points and with 32-bit in-plane offsets
+    // array-valued parameters: the fused kernel takes only layouts with at least one float4 group of halo in z and R
+    // rows in y on either side of the box, and planes of fewer than 2^31 points
     if (p.has_arrays)
-        ok = ok && env_int_tti("B2_TTI_ARR_FUSED", 1) != 0 && p.o[2] >= 4 && p.a[2] - (p.o[2] + p.n[2]) >= 4 &&
+        ok = ok && p.o[2] >= 4 && p.a[2] - (p.o[2] + p.n[2]) >= 4 &&
              p.o[1] >= p.R && p.a[1] - (p.o[1] + p.n[1]) >= p.R && (long long)p.a[1] * p.a[2] < (1ll << 31);
     if (kernel == 1) ok = false;
     if (kernel == 2 && !ok) {
@@ -1172,10 +1111,7 @@ int tti_plan_init(TtiPlan &p, int kernel) {
         if (p.arr_fused) {
             if ((rc = tables())) return rc;
             k_tti_coef_arr<<<sms * 8, 256, 0, stream()>>>(p.damp, p.tMD, inv_dt, p.coefA, p.slot_elems);
-            p.arr_ct = env_int_tti("B2_TTI_ARR_CT", 2);
-            if (p.arr_ct < 0 || p.arr_ct > 2) p.arr_ct = 2;
-            ty = p.arr_ct == 2 ? (p.R == 2 ? TtiTileArr2<2>::TY : TtiTileArr2<4>::TY)
-                               : (p.R == 2 ? TtiTileArr<2>::TY : TtiTileArr<4>::TY);
+            ty = p.R == 2 ? TtiArrTile<2>::TY : TtiArrTile<4>::TY;
         } else {
             const float md = (1.0f / (p.vp * p.vp)) * (1.0f / (p.dt * p.dt));
             k_tti_coef<<<sms * 8, 256, 0, stream()>>>(p.damp, md, inv_dt, p.coefA, p.slot_elems);
@@ -1186,9 +1122,7 @@ int tti_plan_init(TtiPlan &p, int kernel) {
         p.tm_rows = ty + 2 * p.R;
         if ((rc = tti_make_tmap(&p.tm_u, p.u, p.a, p.tsize, 72, ty + 2 * p.R))) return rc;
         if ((rc = tti_make_tmap(&p.tm_v, p.v, p.a, p.tsize, 72, ty + 2 * p.R))) return rc;
-        p.tm_cx = p.tm_cy = p.tm_cz = p.tm_u;
-        if (!p.arr_fused) p.arr_ct = 0;
-        if (p.arr_ct) {     // boxes of the Gz tile (TY + R rows) over the factor tables
+        if (p.arr_fused) {  // boxes of the Gz tile (TY + R rows) over the factor tables
             if ((rc = tti_make_tmap(&p.tm_cx, p.tCx, p.a, 1, 72, ty + p.R))) return rc;
             if ((rc = tti_make_tmap(&p.tm_cy, p.tCy, p.a, 1, 72, ty + p.R))) return rc;
             if ((rc = tti_make_tmap(&p.tm_cz, p.tCz, p.a, 1, 72, ty + p.R))) return rc;
@@ -1213,7 +1147,6 @@ int tti_plan_retarget(const TtiPlan &p, float *u, float *v, TtiPlan &out) {
     int rc;
     if ((rc = tti_make_tmap(&out.tm_u, u, p.a, p.tsize, 72, p.tm_rows))) return rc;
     if ((rc = tti_make_tmap(&out.tm_v, v, p.a, p.tsize, 72, p.tm_rows))) return rc;
-    if (!p.arr_ct) out.tm_cx = out.tm_cy = out.tm_cz = out.tm_u;
     return B2_OK;
 }
 
@@ -1231,7 +1164,6 @@ int tti_plan_adjoint(const TtiPlan &p, TtiPlan &out) {
         if (!p.arr_fused) out.tm_rows = (p.R == 2 ? TtiTile<2>::TY : TtiTile<4>::TY) + 2 * p.R;
         if ((rc = tti_make_tmap(&out.tm_u, a, p.a, 1, 72, out.tm_rows))) return rc;
         if ((rc = tti_make_tmap(&out.tm_v, b, p.a, 1, 72, out.tm_rows))) return rc;
-        if (!p.arr_ct) out.tm_cx = out.tm_cy = out.tm_cz = out.tm_u;
     }
     return B2_OK;
 }
@@ -1396,32 +1328,13 @@ int tti_adj_mix(const TtiPlan &pa, int slot0) {
     return B2_OK;
 }
 
-static int env_int_tti(const char *name, int dflt) {
-    const char *v = getenv(name);
-    return v ? atoi(v) : dflt;
-}
-
-// fused kernel with per-point parameter tables
+// The members of TtiFK that both fused launchers fill alike (zero elsewhere): the time levels, A, the layout, the x
+// range and its chunks, the tensor-map slot and the adjoint's centre. `ty`: rows of the kernel's yz-tile; `nblk`: the
+// CTAs to launch.
 template <int R>
-static int tti_launch_fused_arr(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount) {
-    constexpr int TY1 = TtiTileArr<R>::TY, TY2 = TtiTileArr2<R>::TY;
-    using C0 = TtiCfg<R, TY1, 3, 0>;
-    using C1 = TtiCfg<R, TY1, 2, 1>;
-    using C2 = TtiCfg<R, TY2, 2, 2>;
-    auto kern0 = p.adj ? k_tti_fused<R, TY1, true, 0, true> : k_tti_fused<R, TY1, true, 0>;
-    auto kern1 = p.adj ? k_tti_fused<R, TY1, true, 1, true> : k_tti_fused<R, TY1, true, 1>;
-    auto kern2 = p.adj ? k_tti_fused<R, TY2, true, 2, true> : k_tti_fused<R, TY2, true, 2>;
-    static_assert(C0::SMEM <= 232448 && C1::SMEM <= 232448 && C2::SMEM <= 232448, "shared memory per CTA");
-    static bool attr_set[2] = {false, false};
-    if (!attr_set[p.adj]) {
-        B2_CUDA(cudaFuncSetAttribute(kern0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C0::SMEM), B2_ERR_LAUNCH);
-        B2_CUDA(cudaFuncSetAttribute(kern1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C1::SMEM), B2_ERR_LAUNCH);
-        B2_CUDA(cudaFuncSetAttribute(kern2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2::SMEM), B2_ERR_LAUNCH);
-        attr_set[p.adj] = true;
-    }
-    const int TY = p.arr_ct == 2 ? TY2 : TY1;
-    using C = C0;      // TZ is common to the three configurations
-    TtiFK k;
+static int tti_fk_common(const TtiPlan &p, int ty, int slot0, int slotm, int slot1, int xlo, int xcount, TtiFK &k,
+                         unsigned &nblk) {
+    constexpr int TZ = TtiCfg<R, 1>::TZ;           // the same for every tile height
     memset(&k, 0, sizeof(k));
     k.u1 = p.u + (size_t)slot1 * p.slot_elems;
     k.v1 = p.v + (size_t)slot1 * p.slot_elems;
@@ -1435,56 +1348,63 @@ static int tti_launch_fused_arr(const TtiPlan &p, int slot0, int slotm, int slot
     k.ox = p.o[0];
     k.oy = p.o[1];
     k.oz = p.o[2];
-    k.ay = p.a[1];
-    k.az = p.a[2];
     k.xlo = xlo;
     k.xcount = xcount;
-    k.ntz = (p.n[2] + C::TZ - 1) / C::TZ;
-    k.nty = (p.n[1] + TY - 1) / TY;
-    int lx = env_int_tti("B2_TTI_LX", 0);
+    k.ntz = (p.n[2] + TZ - 1) / TZ;
+    k.nty = (p.n[1] + ty - 1) / ty;
+    int lx = env_int("B2_TTI_LX", 0);
     if (lx <= 0) {
         B2_SM_COUNT(sms);
         lx = choose_chunk_len(sms, k.ntz * k.nty, xcount, 2 * R, 32);
     }
     lx = std::min(lx, xcount);
     k.lx = lx;
-    const int ntx = (xcount + lx - 1) / lx;
+    nblk = (unsigned)(k.ntz * k.nty * ((xcount + lx - 1) / lx));
     k.slot0 = p.adj ? 0 : slot0;
-    if (p.adj) {
-        k.pc = p.u + (size_t)slot0 * p.slot_elems;
-        k.rc = p.v + (size_t)slot0 * p.slot_elems;
+    k.pc = p.adj ? p.u + (size_t)slot0 * p.slot_elems : nullptr;
+    k.rc = p.adj ? p.v + (size_t)slot0 * p.slot_elems : nullptr;
+    return B2_OK;
+}
+
+// fused kernel with per-point parameter tables
+template <int R>
+static int tti_launch_fused_arr(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount) {
+    constexpr int TY = TtiArrTile<R>::TY;
+    using C = TtiCfg<R, TY, true>;
+    auto kern = p.adj ? k_tti_fused<R, TY, true, true> : k_tti_fused<R, TY, true>;
+    static_assert(C::SMEM <= 232448, "shared memory per CTA");
+    static bool attr_set[2] = {false, false};
+    if (!attr_set[p.adj]) {
+        B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM), B2_ERR_LAUNCH);
+        attr_set[p.adj] = true;
     }
+    TtiFK k;
+    unsigned nblk;
+    int rc;
+    if ((rc = tti_fk_common<R>(p, TY, slot0, slotm, slot1, xlo, xcount, k, nblk))) return rc;
     k.tCx = p.tCx; k.tCy = p.tCy; k.tCz = p.tCz; k.tE2 = p.tE2; k.tSD = p.tSD; k.tMD = p.tMD;
-    k.pfc = env_int_tti("B2_TTI_ARR_PREFETCH", 1);
-    k.hint = env_int_tti("B2_TTI_ARR_HINT", 1);
+    k.hint = env_int("B2_TTI_ARR_HINT", 1);
     for (int i = 0; i <= R; ++i) { k.w2x[i] = p.w2[0][i]; k.w2y[i] = p.w2[1][i]; k.w2z[i] = p.w2[2][i]; }
     for (int i = 0; i < R; ++i) { k.w1x[i] = p.w1[0][i]; k.w1y[i] = p.w1[1][i]; k.w1z[i] = p.w1[2][i]; }
     timing_begin();
-    note_sweep_kernel("tti_arr_ct%d<%d>%s", p.arr_ct == 2 ? 2 : (p.arr_ct == 1 ? 1 : 0), R, p.adj ? "+adj" : "");
-    const unsigned nblk = (unsigned)(k.ntz * k.nty * ntx);
-    if (p.arr_ct == 2)
-        kern2<<<nblk, TY2 * 16 + 32, C2::SMEM, stream()>>>(p.tm_u, p.tm_v, p.tm_cx, p.tm_cy, p.tm_cz, k);
-    else if (p.arr_ct == 1)
-        kern1<<<nblk, TY1 * 16 + 32, C1::SMEM, stream()>>>(p.tm_u, p.tm_v, p.tm_cx, p.tm_cy, p.tm_cz, k);
-    else
-        kern0<<<nblk, TY1 * 16 + 32, C0::SMEM, stream()>>>(p.tm_u, p.tm_v, p.tm_cx, p.tm_cy, p.tm_cz, k);
+    note_sweep_kernel("tti_arr_ct2<%d>%s", R, p.adj ? "+adj" : "");
+    kern<<<nblk, TY * 16 + 32, C::SMEM, stream()>>>(p.tm_u, p.tm_v, p.tm_cx, p.tm_cy, p.tm_cz, k);
     timing_end();
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
     return B2_OK;
 }
 
-static bool tti_use_ws(int R) { return R == 4 && env_int_tti("B2_TTI_KERNEL", 3) == 3; }
+static bool tti_use_ws(int R) { return R == 4 && env_int("B2_TTI_KERNEL", 3) == 3; }
 template <int R>
 static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount) {
     // k_tti_ws is register-bound (DESIGN.md §3.5): with the centre loads of the adjoint it spills, so the adjoint
     // sweeps with k_tti_fused<4, .., ADJ>, which does not
     const bool ws = tti_use_ws(R) && !p.adj;
     constexpr int TYF = TtiTile<R>::TY;
-    const int TY = ws ? kTtiWsTY : TYF;
     using C = TtiCfg<R, TYF>;
     using CW = TtiWsCfg<kTtiWsTY>;
-    auto kern = p.adj ? k_tti_fused<R, TYF, false, 0, true> : k_tti_fused<R, TYF, false, 0>;
+    auto kern = p.adj ? k_tti_fused<R, TYF, false, true> : k_tti_fused<R, TYF, false>;
     auto kern_ws = k_tti_ws<kTtiWsTY>;
     static bool attr_set[2] = {false, false};
     if (!attr_set[p.adj]) {
@@ -1493,33 +1413,9 @@ static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, i
         attr_set[p.adj] = true;
     }
     TtiFK k;
-    k.u1 = p.u + (size_t)slot1 * p.slot_elems;
-    k.v1 = p.v + (size_t)slot1 * p.slot_elems;
-    k.um = p.u + (size_t)slotm * p.slot_elems;
-    k.vm = p.v + (size_t)slotm * p.slot_elems;
-    k.A = p.coefA;
-    k.sx = p.sx;
-    k.sy = p.sy;
-    k.ny = p.n[1];
-    k.nz = p.n[2];
-    k.ox = p.o[0];
-    k.oy = p.o[1];
-    k.oz = p.o[2];
-    k.xlo = xlo;
-    k.xcount = xcount;
-    k.ntz = (p.n[2] + C::TZ - 1) / C::TZ;
-    k.nty = (p.n[1] + TY - 1) / TY;
-    int lx = env_int_tti("B2_TTI_LX", 0);
-    if (lx <= 0) {
-        B2_SM_COUNT(sms);
-        lx = choose_chunk_len(sms, k.ntz * k.nty, xcount, 2 * R, 32);
-    }
-    lx = std::min(lx, xcount);
-    k.lx = lx;
-    const int ntx = (xcount + lx - 1) / lx;
-    k.slot0 = p.adj ? 0 : slot0;
-    k.pc = p.adj ? p.u + (size_t)slot0 * p.slot_elems : nullptr;
-    k.rc = p.adj ? p.v + (size_t)slot0 * p.slot_elems : nullptr;
+    unsigned nblk;
+    int rc;
+    if ((rc = tti_fk_common<R>(p, ws ? kTtiWsTY : TYF, slot0, slotm, slot1, xlo, xcount, k, nblk))) return rc;
     k.m_dt2 = (1.0f / (p.vp * p.vp)) * (1.0f / (p.dt * p.dt));
     const float st = sinf(p.theta), ct = cosf(p.theta), sp = sinf(p.phi), cp = cosf(p.phi);
     k.cx = st * cp;
@@ -1542,9 +1438,9 @@ static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, i
     if (ws) note_sweep_kernel("tti_ws<pf1>");
     else note_sweep_kernel("tti_fused<%d>%s", R, p.adj ? "+adj" : "");
     if (ws)
-        kern_ws<<<(unsigned)(k.ntz * k.nty * ntx), kTtiWsTY * 16 + 128, CW::SMEM, stream()>>>(p.tm_u, p.tm_v, k);
+        kern_ws<<<nblk, kTtiWsTY * 16 + 128, CW::SMEM, stream()>>>(p.tm_u, p.tm_v, k);
     else
-        kern<<<(unsigned)(k.ntz * k.nty * ntx), TYF * 16 + 32, C::SMEM, stream()>>>(p.tm_u, p.tm_v, p.tm_u, p.tm_u, p.tm_u, k);
+        kern<<<nblk, TYF * 16 + 32, C::SMEM, stream()>>>(p.tm_u, p.tm_v, p.tm_u, p.tm_u, p.tm_u, k);
     timing_end();
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);

@@ -25,8 +25,7 @@ struct TtiPlan {
     bool use_fused = false;
     bool arr_fused = false;      // fused kernel with per-point parameter tables (k_tti_fused<.., ARR = true>)
     CUtensorMap tm_u, tm_v;
-    CUtensorMap tm_cx, tm_cy, tm_cz;   // factor tables (arr_ct)
-    int arr_ct = 0;              // ... 1: stage-A factor tiles staged through shared memory by TMA; 2: stage B reads them too
+    CUtensorMap tm_cx, tm_cy, tm_cz;   // factor tables (arr_fused)
     float *coefA = nullptr;
     // array-valued parameters (device pointers, nullptr -> scalar)
     const float *vp_a = nullptr, *eps_a = nullptr, *delta_a = nullptr, *theta_a = nullptr, *phi_a = nullptr;

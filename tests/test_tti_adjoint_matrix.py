@@ -123,6 +123,9 @@ def _check(key, sweep, **kw):
         assert err < TOL, f"{n}: {err:.2e}"
 
 
+# variables the library does not read: set to what once selected other array-parameter sweeps, they change nothing
+STALE_ARR_ENV = {'B2_TTI_ARR_CT': '0', 'B2_TTI_ARR_PREFETCH': '0', 'B2_TTI_ARR_FUSED': '0'}
+
 VARIANTS = [
     # (so, arrays, environment, apply kernel=, sweep variant)
     (4, False, {}, 1, 'tti_two_pass+adj'),
@@ -131,13 +134,13 @@ VARIANTS = [
     (8, False, {'B2_TTI_KERNEL': '2'}, 0, 'tti_fused<4>+adj'),
     (8, False, {}, 0, 'tti_fused<4>+adj'),          # the forward runs k_tti_ws here
     (12, False, {}, 0, 'tti_two_pass+adj'),
-    (4, True, {'B2_TTI_ARR_CT': '0'}, 0, 'tti_arr_ct0<2>+adj'),
-    (4, True, {'B2_TTI_ARR_CT': '1'}, 0, 'tti_arr_ct1<2>+adj'),
-    (4, True, {'B2_TTI_ARR_CT': '2'}, 0, 'tti_arr_ct2<2>+adj'),
-    (8, True, {'B2_TTI_ARR_CT': '0'}, 0, 'tti_arr_ct0<4>+adj'),
-    (8, True, {'B2_TTI_ARR_CT': '1'}, 0, 'tti_arr_ct1<4>+adj'),
-    (8, True, {'B2_TTI_ARR_CT': '2'}, 0, 'tti_arr_ct2<4>+adj'),
-    (8, True, {'B2_TTI_ARR_FUSED': '0'}, 0, 'tti_two_pass+adj'),
+    (4, True, {}, 0, 'tti_arr_ct2<2>+adj'),
+    (8, True, {}, 0, 'tti_arr_ct2<4>+adj'),
+    (4, True, {'B2_TTI_ARR_HINT': '0'}, 0, 'tti_arr_ct2<2>+adj'),
+    (8, True, {'B2_TTI_ARR_HINT': '0'}, 0, 'tti_arr_ct2<4>+adj'),
+    (4, True, STALE_ARR_ENV, 0, 'tti_arr_ct2<2>+adj'),
+    (8, True, STALE_ARR_ENV, 0, 'tti_arr_ct2<4>+adj'),
+    (8, True, {}, 1, 'tti_two_pass+adj'),
     (12, True, {}, 0, 'tti_two_pass+adj'),
 ]
 
