@@ -135,7 +135,7 @@ _lib = None
 # every symbol include/b200stencil.h declares
 SYMBOLS = ['b2_iso_forward', 'b2_tti_forward', 'b2_sa_forward', 'b2_linear_forward', 'b2_system_forward', 'b2_nccl_unique_id', 'b2_halo_create',
            'b2_halo_destroy', 'b2_halo_update', 'b2_device_count', 'b2_last_error', 'b2_version',
-           'b2_launch_count', 'b2_last_sweep_kernel', 'b2_kernel_timing_reset', 'b2_kernel_timing_ms',
+           'b2_launch_count', 'b2_last_sweep_kernel', 'b2_last_iso_coef_reuse', 'b2_kernel_timing_reset', 'b2_kernel_timing_ms',
            'b2_kernel_timing_enable', 'b2_malloc_device', 'b2_free_device', 'b2_memcpy_h2d',
            'b2_memcpy_d2h', 'b2_memset_device', 'b2_synchronize', 'b2_set_stream',
            'b2_staging_cache_release', 'b2_staging_outstanding', 'b2_last_call_profile', 'b2_device_pci_bus_id',
@@ -181,6 +181,8 @@ def load_library():
     L.b2_launch_count.restype = c_ulonglong
     L.b2_last_sweep_kernel.argtypes = []
     L.b2_last_sweep_kernel.restype = c_char_p
+    L.b2_last_iso_coef_reuse.argtypes = []
+    L.b2_last_iso_coef_reuse.restype = c_int
     L.b2_kernel_timing_reset.restype = None
     L.b2_kernel_timing_ms.argtypes = [POINTER(c_int)]
     L.b2_kernel_timing_ms.restype = c_double

@@ -555,7 +555,7 @@ static int iso_forward_body(const b2_iso_args *a, Staging &st, SnapStreamer &str
                     return B2_ERR_MEMORY;
                 }
         p.defer_coef = false;
-        if (p.use_tma && (rc = iso_coef_tabulate_planes(p, 0, p.a[0]))) return rc;
+        if (p.use_tma && (rc = iso_coef_tabulate_all(p))) return rc;
     }
     // Born: a second plan for the linearised field (same geometry and coefficient tables, own tensor maps)
     IsoPlan pU = p;

@@ -17,12 +17,14 @@
 //                   consecutive z points (float4), keep the x-direction neighbours in a
 //                   register queue, read y/z neighbours from the shared plane, and write
 //                   u[t+1] with 16-byte coalesced stores. No tensor cores: the update is
-//                   HBM-bandwidth bound (16 B/point).
+//                   HBM-bandwidth bound (16 B/point; 12 B with a scalar vp on the x-planes whose
+//                   coefficient A repeats the pinned plane's, see IsoTK::reuse).
 #include "b2_iso.cuh"
 #include "b2_iso_point.cuh"
 #include "b2_ptx.cuh"
 #include <cstdlib>
 #include <algorithm>
+#include <vector>
 
 namespace b2 {
 
@@ -125,6 +127,11 @@ struct IsoTK {
     long long off_lo, off_hi;     // element offset of "my plane 0" inside the neighbour's array (output slot)
     const int *flag_lo, *flag_hi; // local flags the neighbours release (NULL: nothing to wait for)
     int want;                     // flag value that says "halos of u[t] are in place" (< 0: already ensured)
+    // ---- coefficient reuse (scalar parameter only; NULL: every A tile is streamed) ----
+    // reuse[x] = 1 (allocated plane index) when A on plane x equals A on plane pin_x bit for bit over the
+    // update box (IsoPlan::coef_reuse): the CTA then takes those planes' A from one tile pinned before the march.
+    const unsigned char *reuse;
+    int pin_x;
 };
 
 constexpr int ceil4(int v) { return (v + 3) / 4 * 4; }
@@ -149,8 +156,11 @@ struct IsoTmaCfg {
     static constexpr int TILE = TY * TZ;
     static constexpr int NCW = TY * TZ4 / 32;          // consumer warps
     static constexpr int NTILES = 2 + (PK != B2_PARAM_SCALAR ? 1 : 0);   // prev, A, [B]
-    static constexpr size_t SMEM =
-        (size_t)(NU * PLANE + NS * TILE * NTILES) * 4 + 2 * NU * 8 + 128;
+    // scalar parameter: the pinned A tile, its mbarrier and one reuse flag per tile-ring stage
+    static constexpr int PIN = PK == B2_PARAM_SCALAR ? TILE : 0;
+    static constexpr size_t SMEM = (size_t)(NU * PLANE + NS * TILE * NTILES + PIN) * 4 + 2 * NU * 8 +
+                                   (PK == B2_PARAM_SCALAR ? 8 + NS * 4 : 0) + 128;
+    static_assert(SMEM <= 227 * 1024, "k_iso_tma: shared memory over the 227 KB of one SM");
 };
 
 __device__ __forceinline__ float4 f4add(float4 a, float4 b) {
@@ -179,9 +189,13 @@ k_iso_tma(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUt
     float *s_u = reinterpret_cast<float *>(smem_raw);
     float *s_prev = s_u + NU * PLANE;
     float *s_a = s_prev + NS * TILE;
-    float *s_b = s_a + NS * TILE;
-    uint64_t *full = reinterpret_cast<uint64_t *>(s_b + (PK != B2_PARAM_SCALAR ? NS * TILE : 0));
+    float *s_b = s_a + NS * TILE;                 // array vp|m: the B ring
+    float *s_pin = s_b;                           // scalar: the pinned A tile (my_prev + 2 NS TILE)
+    uint64_t *full = reinterpret_cast<uint64_t *>(s_b + (PK != B2_PARAM_SCALAR ? NS * TILE : C::PIN));
     uint64_t *empty = full + NU;
+    uint64_t *pinbar = empty + NU;                            // scalar: the pinned tile's arrival
+    int *s_reused = reinterpret_cast<int *>(pinbar + 1);      // scalar: per tile stage, A is the pinned tile
+    const bool pin = PK == B2_PARAM_SCALAR && k.reuse != nullptr;
 
     int b = blockIdx.x;
     const int iz = b % k.ntz;
@@ -206,6 +220,7 @@ k_iso_tma(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUt
             b2ptx::mbar_init(&full[i], 1);
             b2ptx::mbar_init(&empty[i], NCW);
         }
+        if (PK == B2_PARAM_SCALAR) b2ptx::mbar_init(pinbar, 1);
         b2ptx::fence_mbar_init();
     }
     __syncthreads();
@@ -217,6 +232,10 @@ k_iso_tma(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUt
             b2ptx::tma_prefetch_desc(&tm_uc);
             b2ptx::tma_prefetch_desc(&tm_a);
             if (PK != B2_PARAM_SCALAR) b2ptx::tma_prefetch_desc(&tm_b);
+            if (pin) {
+                b2ptx::mbar_arrive_expect_tx(pinbar, TILE * 4);
+                b2ptx::tma_load_3d(s_pin, &tm_a, pinbar, k.oz + z0, k.oy + y0, k.pin_x);
+            }
             int slot = 0, round = 0, ss = 0;
             bool need_lo = k.want >= 0 && k.flag_lo != nullptr, need_hi = k.want >= 0 && k.flag_hi != nullptr;
             for (int j = 0; j < NP; ++j) {
@@ -235,17 +254,24 @@ k_iso_tma(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUt
                     b2ptx::fence_proxy_async_global();
                     need_hi = false;
                 }
+                const int xo = xj - dx * R;      // output plane of step s
+                bool reused = false;
                 uint32_t bytes = C::BY * BZ * 4;
-                if (s >= 0) bytes += TILE * 4 * C::NTILES;
+                if (s >= 0) {
+                    // the flag travels to the consumers with the stage: the arrive below releases it
+                    reused = pin && __ldg(k.reuse + k.ox + xo) != 0;
+                    if (PK == B2_PARAM_SCALAR) s_reused[ss] = reused;
+                    bytes += TILE * 4 * (C::NTILES - (reused ? 1 : 0));
+                }
                 b2ptx::mbar_arrive_expect_tx(&full[slot], bytes);
                 b2ptx::tma_load_4d(s_u + slot * PLANE, &tm_uh, &full[slot], k.oz + z0 - RZ,
                                    k.oy + y0 - R, k.ox + xj, k.slot0);
                 if (s >= 0) {
-                    const int xo = xj - dx * R;
                     b2ptx::tma_load_4d(s_prev + ss * TILE, &tm_uc, &full[slot], k.oz + z0,
                                        k.oy + y0, k.ox + xo, k.slotm);
-                    b2ptx::tma_load_3d(s_a + ss * TILE, &tm_a, &full[slot], k.oz + z0, k.oy + y0,
-                                       k.ox + xo);
+                    if (!reused)
+                        b2ptx::tma_load_3d(s_a + ss * TILE, &tm_a, &full[slot], k.oz + z0, k.oy + y0,
+                                           k.ox + xo);
                     if (PK != B2_PARAM_SCALAR)
                         b2ptx::tma_load_3d(s_b + ss * TILE, &tm_b, &full[slot], k.oz + z0,
                                            k.oy + y0, k.ox + xo);
@@ -274,6 +300,7 @@ k_iso_tma(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUt
     for (int i = 0; i < Q; ++i) q[i] = make_float4(0.f, 0.f, 0.f, 0.f);
 
     const float wc = k.wx[0] + k.wy[0] + k.wz[0];
+    if (pin) b2ptx::mbar_wait(pinbar, 0);
     uint32_t par = 0;               // parity of the u-ring round
     int ssoff = 0;                  // float offset of the tile-ring slot of output step j-2R
 
@@ -334,7 +361,9 @@ k_iso_tma(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUt
                     f4fma(acc, k.wx[i], f4add(q[(pc - i + Q) % Q], q[(pc + i) % Q]));
 
                 const float4 pv = b2ptx::lds128(my_prev + ssoff);
-                const float4 ca = b2ptx::lds128(my_prev + (NS * TILE) + ssoff);
+                int aoff = NS * TILE + ssoff;
+                if (PK == B2_PARAM_SCALAR && s_reused[ssoff / TILE]) aoff = 2 * NS * TILE;   // s_pin
+                const float4 ca = b2ptx::lds128(my_prev + aoff);
                 const float4 dcp = f4sub(c, pv);
                 float4 o;
                 if (PK == B2_PARAM_SCALAR) {
@@ -531,6 +560,72 @@ int iso_coef_tabulate_planes(const IsoPlan &p, int plane_lo, int plane_hi) {
     return B2_OK;
 }
 
+// A over the whole allocated array (scalar parameter), and the reuse flags of the planes in the update box: a warp
+// whose damp row segment differs in any bit from the pin plane's (inside the box's rows and columns) clears its
+// plane's flag. The pin plane (4 B/point once) stays in L2 while every plane compares against it.
+__global__ void __launch_bounds__(256)
+k_iso_coef_scan(const float *__restrict__ damp, float m_dt2, float inv_dt, float *__restrict__ A,
+                unsigned char *__restrict__ reuse, long long sx, int a0, int a1, int a2, int xpin, int xlo, int xhi,
+                int ylo, int yhi, int zlo, int zhi) {
+    const int z = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool zin = z < a2;
+    for (int x = blockIdx.z; x < a0; x += gridDim.z) {
+        const bool cmp = zin && x >= xlo && x < xhi && z >= zlo && z < zhi;
+        bool differ = false;
+        for (int y = blockIdx.y; y < a1; y += gridDim.y) {
+            if (!zin) continue;
+            const size_t row = (size_t)y * a2 + z;
+            const float d = damp[(size_t)x * (size_t)sx + row];
+            A[(size_t)x * (size_t)sx + row] = 1.0f / (m_dt2 + d * inv_dt);
+            if (cmp && y >= ylo && y < yhi)
+                differ |= __float_as_uint(d) != __float_as_uint(damp[(size_t)xpin * (size_t)sx + row]);
+        }
+        if (__any_sync(0xffffffffu, differ) && (threadIdx.x & 31) == 0) reuse[x] = 0;
+    }
+}
+
+// one byte per allocated x-plane, cached across calls; g_reuse_n: planes the last iso call flagged (0: none)
+static unsigned char *g_reuse = nullptr;
+static int g_reuse_cap = 0, g_reuse_n = 0;
+
+int iso_coef_tabulate_all(IsoPlan &p) {
+    if (p.param_kind != B2_PARAM_SCALAR) return iso_coef_tabulate_planes(p, 0, p.a[0]);
+    if (g_reuse_cap < p.a[0]) {
+        if (g_reuse) cudaFree(g_reuse);
+        g_reuse = nullptr;
+        g_reuse_cap = 0;
+        B2_CUDA(cudaMalloc(&g_reuse, (size_t)p.a[0]), B2_ERR_MEMORY);
+        g_reuse_cap = p.a[0];
+    }
+    // 1 on the planes of the update box, 0 elsewhere; the scan clears the planes that differ
+    B2_CUDA(cudaMemsetAsync(g_reuse, 0, (size_t)p.a[0], stream()), B2_ERR_LAUNCH);
+    B2_CUDA(cudaMemsetAsync(g_reuse + p.o[0], 1, (size_t)p.n[0], stream()), B2_ERR_LAUNCH);
+    const float inv_dt = 1.0f / p.dt, inv_dt2 = 1.0f / (p.dt * p.dt);
+    const float md = (1.0f / (p.vp * p.vp)) * inv_dt2;
+    dim3 block(256, 1, 1), grid((p.a[2] + 255) / 256, (unsigned)std::min(p.a[1], 64), (unsigned)std::min(p.a[0], 65535));
+    k_iso_coef_scan<<<grid, block, 0, stream()>>>(p.damp, md, inv_dt, p.coefA, g_reuse, p.sx, p.a[0], p.a[1], p.a[2],
+                                                  p.o[0] + p.n[0] / 2, p.o[0], p.o[0] + p.n[0], p.o[1],
+                                                  p.o[1] + p.n[1], p.o[2], p.o[2] + p.n[2]);
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    p.coef_reuse = g_reuse;
+    g_reuse_n = p.a[0];
+    return B2_OK;
+}
+
+int iso_coef_reuse_count() {
+    if (g_reuse_n <= 0) return 0;
+    std::vector<unsigned char> h((size_t)g_reuse_n);
+    if (cudaMemcpyAsync(h.data(), g_reuse, h.size(), cudaMemcpyDeviceToHost, stream()) != cudaSuccess ||
+        cudaStreamSynchronize(stream()) != cudaSuccess) {
+        set_error("b2_last_iso_coef_reuse: reading the flags back failed");
+        return -1;
+    }
+    int n = 0;
+    for (unsigned char f : h) n += f != 0;
+    return n;
+}
+
 static int iso_coef_tabulate(IsoPlan &p) {
     int rc;
     if ((rc = coef_buffer(0, p.slot_elems, &p.coefA))) return rc;
@@ -538,7 +633,7 @@ static int iso_coef_tabulate(IsoPlan &p) {
     if (p.param_kind != B2_PARAM_SCALAR)
         if ((rc = coef_buffer(1, p.slot_elems, &p.coefB))) return rc;
     if (p.defer_coef) return B2_OK;          // the caller tabulates plane ranges itself
-    return iso_coef_tabulate_planes(p, 0, p.a[0]);
+    return iso_coef_tabulate_all(p);
 }
 
 template <int R>
@@ -562,6 +657,8 @@ static int plan_tma(IsoPlan &p) {
 }
 
 int iso_plan_init(IsoPlan &p, int kernel) {
+    p.coef_reuse = nullptr;
+    g_reuse_n = 0;
     const int R = p.radius[2];
     bool ok = (p.radius[0] == R && p.radius[1] == R) && (R == 2 || R == 4 || R == 6 || R == 8);
     ok = ok && p.damp != nullptr;
@@ -659,6 +756,8 @@ static int launch_tma(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo
         k.flag_hi = fz->flag_hi;
         k.want = fz->want;
     }
+    k.reuse = PK == B2_PARAM_SCALAR ? p.coef_reuse : nullptr;
+    k.pin_x = p.o[0] + p.n[0] / 2;
     k.slot0 = slot0;
     k.slotm = slotm;
     k.m_dt2 = (1.0f / (p.vp * p.vp)) * (1.0f / (p.dt * p.dt));

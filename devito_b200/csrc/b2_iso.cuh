@@ -25,6 +25,10 @@ struct IsoPlan {
     CUtensorMap tm_uh, tm_uc, tm_damp, tm_par;   // tm_damp/tm_par map coefA/coefB
     float *coefA = nullptr, *coefB = nullptr;    // tabulated update coefficients (library scratch)
     bool defer_coef = false;                     // plan init only allocates them (streamed loop: per chunk)
+    // scalar parameter, whole table tabulated: one byte per allocated x-plane (library scratch, device), 1 where
+    // damp on the plane equals damp on the pin plane o[0] + n[0]/2 bit for bit over the update box, so that A
+    // does too. NULL otherwise: the sweep then streams every A tile.
+    const unsigned char *coef_reuse = nullptr;
     int lx = 0;
     // OT4 (b2_iso_args.ot4): generic two-pass path, W = lap(u)/m in library scratch
     bool ot4 = false;
@@ -48,6 +52,11 @@ int iso_plan_init(IsoPlan &p, int kernel);
 
 // (Re)tabulate the coefficient tables on the allocated x-planes [plane_lo, plane_hi).
 int iso_coef_tabulate_planes(const IsoPlan &p, int plane_lo, int plane_hi);
+// Tabulate the whole tables once damp and the parameter are on the device; with a scalar parameter also find
+// the planes whose A repeats the pin plane's (p.coef_reuse).
+int iso_coef_tabulate_all(IsoPlan &p);
+// Planes of the last iso call whose A came from the pinned tile (reads the flags back: synchronises the stream).
+int iso_coef_reuse_count();
 int iso_coef_tabulate_rows(const IsoPlan &p, int x0, int x1, int y0, int y1);
 
 // One time step over x in [xlo, xlo + xcount) (relative to the iteration origin):

@@ -3,6 +3,7 @@
 // copyout` placed by DeviceAwareDataManager, devito/passes/iet/definitions.py:636-671),
 // launch counter, kernel timing, small device-memory utilities.
 #include "b2_common.cuh"
+#include "b2_iso.cuh"
 #include <cstdarg>
 #include <cstdlib>
 #include <vector>
@@ -300,6 +301,8 @@ const char *b2_version(void) { return "b200stencil 0.1 (sm_90a)"; }
 unsigned long long b2_launch_count(void) { return g_launches; }
 
 const char *b2_last_sweep_kernel(void) { return g_sweep_kernel; }
+
+int b2_last_iso_coef_reuse(void) { return iso_coef_reuse_count(); }
 
 void b2_kernel_timing_enable(int on) { g_timing_on = on != 0; }
 

@@ -403,6 +403,12 @@ void   b2_kernel_timing_enable(int on);
  * adjoint call appends "+adj" to the variant that ran its sweep. b2_sa_forward reports "sa_tma<R>" or "sa_generic", with "+adj" on
  * adjoint calls. */
 const char *b2_last_sweep_kernel(void);
+/* number of x-planes of the last b2_iso_forward call whose update coefficient A = 1/(m/dt^2 + damp/dt) the
+ * TMA sweep took from the one tile it pins per CTA instead of streaming it: the planes of the update box whose
+ * damp equals, bit for bit over the box, the damp of the centre plane x_m + (x_M - x_m + 1)/2 (scalar vp only,
+ * whole table on the device before the time loop; 0 for the streamed loop, an array vp|m and the generic
+ * kernel). Reads the flags back from the device: synchronises the library stream. -1 on a device error. */
+int         b2_last_iso_coef_reuse(void);
 /* device memory helpers for hosts that do not use torch */
 void *b2_malloc_device(unsigned long nbytes, int deviceid);
 void  b2_free_device(void *p, int deviceid);

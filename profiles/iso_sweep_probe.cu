@@ -6,7 +6,8 @@
 // (u[t-1], A) with TMA on a full mbarrier, and the consumer threads store one TY x TZ tile of u[t+1] with
 // 16-byte stores, then release the stage. The stage ring has LEAD+1 stages, so the producer runs LEAD planes
 // ahead of the consumers, as the sweep's does. The consumers do no arithmetic: the stored value is the u[t-1]
-// tile, so the time is that of the memory system alone.
+// tile, so the time is that of the memory system alone. NT = 1 drops the A tile: the three-stream mix the sweep
+// moves on the planes whose A it takes from its pinned tile (b2_iso.cu::k_iso_tma).
 //
 // k_stream is a plain float4 read/write stream (grid-stride, one read and one write per element).
 #include <cuda.h>
@@ -36,7 +37,7 @@ struct Grid {
     int ntz, nty, ntx;
 };
 
-template <int TY, int TZ, int HY, int HZ, int LEAD>
+template <int TY, int TZ, int HY, int HZ, int LEAD, int NT>
 struct CopyCfg {
     static constexpr int BY = TY + 2 * HY, BZ = TZ + 2 * HZ;
     static constexpr int UBOX = (BY * BZ + 31) / 32 * 32;
@@ -44,18 +45,18 @@ struct CopyCfg {
     static constexpr int NST = LEAD + 1;
     static constexpr int NCT = TILE / 4 < 512 ? TILE / 4 : 512;      // consumer threads
     static constexpr int NCW = NCT / 32;
-    static constexpr size_t SMEM = (size_t)NST * (UBOX + 2 * TILE) * 4 + 2 * NST * 8 + 128;
+    static constexpr size_t SMEM = (size_t)NST * (UBOX + NT * TILE) * 4 + 2 * NST * 8 + 128;
 };
 
-template <int TY, int TZ, int HY, int HZ, int LEAD>
-__global__ void __launch_bounds__(CopyCfg<TY, TZ, HY, HZ, LEAD>::NCT + 32, 1)
+template <int TY, int TZ, int HY, int HZ, int LEAD, int NT>
+__global__ void __launch_bounds__(CopyCfg<TY, TZ, HY, HZ, LEAD, NT>::NCT + 32, 1)
 k_copy(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_um,
        const __grid_constant__ CUtensorMap tm_a, float *__restrict__ out, Grid g) {
-    using C = CopyCfg<TY, TZ, HY, HZ, LEAD>;
+    using C = CopyCfg<TY, TZ, HY, HZ, LEAD, NT>;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float *s_u = reinterpret_cast<float *>(smem_raw);
-    float *s_t = s_u + C::NST * C::UBOX;                        // per stage: u[t-1] tile, A tile
-    uint64_t *full = reinterpret_cast<uint64_t *>(s_t + C::NST * 2 * C::TILE);
+    float *s_t = s_u + C::NST * C::UBOX;                        // per stage: u[t-1] tile[, A tile]
+    uint64_t *full = reinterpret_cast<uint64_t *>(s_t + C::NST * NT * C::TILE);
     uint64_t *empty = full + C::NST;
 
     int b = blockIdx.x;
@@ -82,12 +83,12 @@ k_copy(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtenso
                 const int st = j % C::NST;
                 if (j >= C::NST) b2ptx::mbar_wait(&empty[st], ((j / C::NST) - 1) & 1);
                 const bool tiles = j >= 2 * R;
-                b2ptx::mbar_arrive_expect_tx(&full[st], (C::BY * C::BZ + (tiles ? 2 * C::TILE : 0)) * 4);
+                b2ptx::mbar_arrive_expect_tx(&full[st], (C::BY * C::BZ + (tiles ? NT * C::TILE : 0)) * 4);
                 b2ptx::tma_load_3d(s_u + st * C::UBOX, &tm_u, &full[st], z0 - HZ, y0 - HY, xs - R + j);
                 if (tiles) {
-                    float *t = s_t + st * 2 * C::TILE;
+                    float *t = s_t + st * NT * C::TILE;
                     b2ptx::tma_load_3d(t, &tm_um, &full[st], z0, y0, xs + j - 2 * R);
-                    b2ptx::tma_load_3d(t + C::TILE, &tm_a, &full[st], z0, y0, xs + j - 2 * R);
+                    if (NT == 2) b2ptx::tma_load_3d(t + C::TILE, &tm_a, &full[st], z0, y0, xs + j - 2 * R);
                 }
             }
         }
@@ -98,7 +99,7 @@ k_copy(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtenso
         const int st = j % C::NST;
         b2ptx::mbar_wait(&full[st], (j / C::NST) & 1);
         if (j >= 2 * R) {
-            const float *t = s_t + st * 2 * C::TILE;
+            const float *t = s_t + st * NT * C::TILE;
             float *op = out + (size_t)(xs + j - 2 * R) * A * A;
 #pragma unroll
             for (int f = tid; f < C::TILE / 4; f += C::NCT) {
@@ -143,10 +144,10 @@ static CUtensorMap tmap(const float *base, int bz, int by) {
 static float *g_u, *g_um, *g_a, *g_out;
 static const int kReps = 5;
 
-template <int TY, int TZ, int HY, int HZ, int LEAD>
+template <int TY, int TZ, int HY, int HZ, int LEAD, int NT = 2>
 static void run_copy(const char *name, bool first) {
-    using C = CopyCfg<TY, TZ, HY, HZ, LEAD>;
-    auto kern = k_copy<TY, TZ, HY, HZ, LEAD>;
+    using C = CopyCfg<TY, TZ, HY, HZ, LEAD, NT>;
+    auto kern = k_copy<TY, TZ, HY, HZ, LEAD, NT>;
     CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
     CUtensorMap tu = tmap(g_u, C::BZ, C::BY), tum = tmap(g_um, TZ, TY), ta = tmap(g_a, TZ, TY);
     Grid g{N / TZ, N / TY, N / LX};
@@ -165,10 +166,10 @@ static void run_copy(const char *name, bool first) {
     ms /= kReps;
     const double pts = (double)(g.ntz * TZ) * (g.nty * TY) * (g.ntx * LX);
     const double alg = 16.0 * pts;
-    const double moved = (double)grid * ((double)(LX + 2 * R) * C::BY * C::BZ * 4 + (double)LX * C::TILE * 4 * 3);
-    printf("%s{\"name\": \"%s\", \"u_box\": [%d, %d], \"tile\": [%d, %d], \"lead\": %d, \"smem\": %zu, "
+    const double moved = (double)grid * ((double)(LX + 2 * R) * C::BY * C::BZ * 4 + (double)LX * C::TILE * 4 * (NT + 1));
+    printf("%s{\"name\": \"%s\", \"u_box\": [%d, %d], \"tile\": [%d, %d], \"tiles_in\": %d, \"lead\": %d, \"smem\": %zu, "
            "\"ms\": %.4f, \"alg_gbs\": %.1f, \"moved_gbs\": %.1f, \"moved_per_alg\": %.4f}",
-           first ? "" : ", ", name, C::BY, C::BZ, TY, TZ, LEAD, C::SMEM, ms, alg / ms * 1e-6, moved / ms * 1e-6,
+           first ? "" : ", ", name, C::BY, C::BZ, TY, TZ, NT, LEAD, C::SMEM, ms, alg / ms * 1e-6, moved / ms * 1e-6,
            moved / alg);
     CK(cudaEventDestroy(e0));
     CK(cudaEventDestroy(e1));
@@ -202,6 +203,9 @@ int main() {
     run_copy<32, 64, 0, 0, 7>("nohalo_32x64", false);
     run_copy<16, 128, 0, 0, 4>("nohalo_16x128", false);
     run_copy<16, 128, 0, 0, 7>("nohalo_16x128", false);
+    // the sweep's 16 x 128 boxes with the A tile (16 B/point) and without it (the planes whose A is pinned, 12 B/point)
+    run_copy<16, 128, 4, 4, 4>("sweep_16x128", false);
+    run_copy<16, 128, 4, 4, 4, 1>("sweep_16x128_noA", false);
     printf("]");
 
     // plain read/write stream over 2 x 4.4 GB
