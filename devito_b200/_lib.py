@@ -71,7 +71,7 @@ class TtiArgs(Structure):
                 ('phi_arr', POINTER(Dataobj)),
                 ('born_du', POINTER(Dataobj)), ('born_dv', POINTER(Dataobj)), ('born_dm', POINTER(Dataobj)),
                 ('adjoint', c_int), ('grad', POINTER(Dataobj)), ('usave', POINTER(Dataobj)),
-                ('vsave', POINTER(Dataobj))]
+                ('vsave', POINTER(Dataobj)), ('ndim', c_int)]
 
 
 class SaArgs(Structure):

@@ -137,10 +137,9 @@ def _body(plan, distributed):
     """Fill `struct b2_<kind>_args` from the flat parameters and call the entry point."""
     entry = wave_entry(plan)
     nd = plan['grid'].dim
-    nw = 3 if plan['kind'] == 'tti' else nd
     L = []
     for member, w in entry.weights:
-        for d in range(nw):
+        for d in range(nd):
             L.append(_warray(f'{member}_{"xyz"[d]}', w[d]))
     if plan['src'] is not None:
         L.append(_sparse_block(plan['src'], nd, 'src_s'))
@@ -152,7 +151,7 @@ def _body(plan, distributed):
     for k, v in entry.flags.items():
         L.append(f"  a.{k} = {int(v)};")
     for member, _ in entry.weights:
-        for d in range(nw):
+        for d in range(nd):
             L.append(f"  a.{member}[{d}] = {member}_{'xyz'[d]};")
     for s in entry.arrays:
         L.append(f"  a.{s.member} = (struct b2_dataobj *){s.obj.name}_vec;")

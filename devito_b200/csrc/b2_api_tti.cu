@@ -15,7 +15,12 @@ using namespace b2;
 
 static int tti_forward_body(const b2_tti_args *a, Staging &st) {
     const int so = a->space_order;
+    const int nd = a->ndim == 2 ? 2 : 3;
     int rc = B2_OK;
+    if (nd == 2 && (a->phi != 0.f || a->phi_arr || a->halo)) {
+        set_error("b2_tti_forward: a 2-D call takes no azimuth (phi = 0, phi_arr NULL) and no halo exchange");
+        return B2_ERR_INVALID;
+    }
 
     DevArray *u, *v, *damp = nullptr, *parr[5] = {}, *bdu = nullptr, *bdv = nullptr, *bdm = nullptr, *grad = nullptr,
              *usave = nullptr, *vsave = nullptr;
@@ -23,13 +28,13 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
     TtiPlan p, pd, pa;
     FieldGeom g;
 
-    if ((rc = st.array(a->u, 4, true, u))) return rc;
-    if ((rc = st.array(a->v, 4, true, v))) return rc;
-    if (a->damp && (rc = st.array(a->damp, 3, false, damp))) return rc;
+    if ((rc = st.array(a->u, nd + 1, true, u))) return rc;
+    if ((rc = st.array(a->v, nd + 1, true, v))) return rc;
+    if (a->damp && (rc = st.array(a->damp, nd, false, damp))) return rc;
     {
         const b2_dataobj *pa[5] = {a->vp_arr, a->epsilon_arr, a->delta_arr, a->theta_arr, a->phi_arr};
         for (int i = 0; i < 5; ++i)
-            if (pa[i] && (rc = st.array(pa[i], 3, false, parr[i]))) return rc;
+            if (pa[i] && (rc = st.array(pa[i], nd, false, parr[i]))) return rc;
     }
     const bool born = a->born_du || a->born_dv || a->born_dm;
     int dmh = 0;
@@ -42,15 +47,15 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
             set_error("b2_tti_forward: Born modelling is not combined with halo exchange in this version");
             return B2_ERR_INVALID;
         }
-        if ((rc = st.array(a->born_du, 4, true, bdu))) return rc;
-        if ((rc = st.array(a->born_dv, 4, true, bdv))) return rc;
-        if ((rc = st.array(a->born_dm, 3, false, bdm))) return rc;
-        for (int d = 0; d < 4; ++d)
+        if ((rc = st.array(a->born_du, nd + 1, true, bdu))) return rc;
+        if ((rc = st.array(a->born_dv, nd + 1, true, bdv))) return rc;
+        if ((rc = st.array(a->born_dm, nd, false, bdm))) return rc;
+        for (int d = 0; d <= nd; ++d)
             if (bdu->size[d] != u->size[d] || bdv->size[d] != u->size[d]) {
                 set_error("b2_tti_forward: born_du and born_dv must have the layout of u");
                 return B2_ERR_INVALID;
             }
-        if ((dmh = grid_halo("b2_tti_forward", "born_dm", a->born_dm, *bdm, 0, *u, 3, so)) < 0) return B2_ERR_INVALID;
+        if ((dmh = grid_halo("b2_tti_forward", "born_dm", a->born_dm, *bdm, 0, *u, nd, so)) < 0) return B2_ERR_INVALID;
     }
     const bool adj = a->adjoint != 0;
     int gh = 0;
@@ -71,16 +76,16 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
             set_error("b2_tti_forward: the imaging condition runs with the adjoint only");
             return B2_ERR_INVALID;
         }
-        if ((rc = st.array(a->grad, 3, true, grad))) return rc;
-        if ((rc = st.array(a->usave, 4, false, usave))) return rc;
-        if ((rc = st.array(a->vsave, 4, false, vsave))) return rc;
-        if (grid_halo("b2_tti_forward", "usave", a->usave, *usave, 1, *u, 3, so, so) < 0 ||
-            grid_halo("b2_tti_forward", "vsave", a->vsave, *vsave, 1, *u, 3, so, so) < 0 ||
-            (gh = grid_halo("b2_tti_forward", "grad", a->grad, *grad, 0, *u, 3, so)) < 0)
+        if ((rc = st.array(a->grad, nd, true, grad))) return rc;
+        if ((rc = st.array(a->usave, nd + 1, false, usave))) return rc;
+        if ((rc = st.array(a->vsave, nd + 1, false, vsave))) return rc;
+        if (grid_halo("b2_tti_forward", "usave", a->usave, *usave, 1, *u, nd, so, so) < 0 ||
+            grid_halo("b2_tti_forward", "vsave", a->vsave, *vsave, 1, *u, nd, so, so) < 0 ||
+            (gh = grid_halo("b2_tti_forward", "grad", a->grad, *grad, 0, *u, nd, so)) < 0)
             return B2_ERR_INVALID;
     }
-    if ((rc = sparse_stage_in(st, a->src, 3, false, src))) return rc;
-    if ((rc = sparse_stage_in(st, a->rec, 3, true, rec))) return rc;
+    if ((rc = sparse_stage_in(st, a->src, nd, false, src))) return rc;
+    if ((rc = sparse_stage_in(st, a->rec, nd, true, rec))) return rc;
     // devito/operations/interpolators.py:28-37 `check_radius`
     if ((src.present && src.r > so) || (rec.present && rec.r > so)) {
         set_error("b2_tti_forward: sparse radius %d exceeds the halo (space_order %d)",
@@ -90,15 +95,21 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
 
     const int lo_in[3] = {a->x_m, a->y_m, a->z_m};
     const int hi_in[3] = {a->x_M, a->y_M, a->z_M};
+    p.ndim = nd;
     p.R = a->radius;
     p.so = so;
     p.tsize = u->size[0];
     for (int d = 0; d < 3; ++d) {
-        p.a[d] = u->size[d + 1];
-        p.n[d] = hi_in[d] - lo_in[d] + 1;
-        p.o[d] = lo_in[d] + so;
+        const int di = d - (3 - nd);          // the grid's dim, or < 0 for the dummy leading dim of a 2-D grid
+        if (di < 0) {
+            p.a[d] = 1; p.n[d] = 1; p.o[d] = 0;
+            continue;
+        }
+        p.a[d] = u->size[di + 1];
+        p.n[d] = hi_in[di] - lo_in[di] + 1;
+        p.o[d] = lo_in[di] + so;
         if (p.n[d] <= 0) return B2_OK;
-        if (v->size[d + 1] != p.a[d]) { set_error("b2_tti_forward: u and v shapes differ"); return B2_ERR_INVALID; }
+        if (v->size[di + 1] != p.a[d]) { set_error("b2_tti_forward: u and v shapes differ"); return B2_ERR_INVALID; }
         if (p.o[d] - p.R < 0 || p.o[d] + p.n[d] - 1 + p.R >= p.a[d]) {
             set_error("b2_tti_forward: iteration range + radius leaves the allocated array on dim %d", d);
             return B2_ERR_INVALID;
@@ -119,10 +130,11 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
     const float *pv[5];
     for (int i = 0; i < 5; ++i) pv[i] = parr[i] ? (const float *)parr[i]->d : nullptr;
     p.vp_a = pv[0]; p.eps_a = pv[1]; p.delta_a = pv[2]; p.theta_a = pv[3]; p.phi_a = pv[4];
-    for (int d = 0; d < 3; ++d) {
-        if (!a->w2[d] || !a->w1[d]) { set_error("b2_tti_forward: weights missing"); return B2_ERR_INVALID; }
-        for (int i = 0; i <= a->radius; ++i) p.w2[d][i] = a->w2[d][i];
-        for (int i = 0; i < a->radius; ++i) p.w1[d][i] = a->w1[d][i];
+    for (int di = 0; di < nd; ++di) {       // a 2-D plan's dummy dim keeps zero weights
+        const int d = di + 3 - nd;
+        if (!a->w2[di] || !a->w1[di]) { set_error("b2_tti_forward: weights missing"); return B2_ERR_INVALID; }
+        for (int i = 0; i <= a->radius; ++i) p.w2[d][i] = a->w2[di][i];
+        for (int i = 0; i < a->radius; ++i) p.w1[d][i] = a->w1[di][i];
     }
     {
         // both pairs run one sweep variant: a linearised pair that cannot take the fused kernel sends both to the
@@ -138,8 +150,13 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
     g.sy = p.sy;
     g.slot_elems = p.slot_elems;
     g.so = so;
-    g.ndim = 3;
-    for (int d = 0; d < 3; ++d) { g.lo[d] = lo_in[d]; g.hi[d] = hi_in[d]; }
+    g.ndim = nd;
+    for (int d = 0; d < nd; ++d) { g.lo[d] = lo_in[d]; g.hi[d] = hi_in[d]; }
+    DevArray grad3;                             // grad with the plan's (dummy, x, z) extents on a 2-D grid
+    if (grad) {
+        grad3 = *grad;
+        if (nd == 2) { grad3.size[0] = 1; grad3.size[1] = grad->size[0]; grad3.size[2] = grad->size[1]; }
+    }
     if (a->halo) { g.nb_lo = a->halo->rank > 0; g.nb_hi = a->halo->rank < a->halo->nranks - 1; }
 
     const float dt2 = a->dt * a->dt;
@@ -185,8 +202,8 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
         }
         if (born) {
             if ((rc = tti_step(pd, t0, t2, t1, 0, p.n[0]))) return rc;
-            if ((rc = tti_born_source(p, pd, t0, t2, t1, (const float *)bdm->d, (long long)bdm->size[1] * bdm->size[2],
-                                      bdm->size[2], dmh)))
+            if ((rc = tti_born_source(p, pd, t0, t2, t1, (const float *)bdm->d,
+                                      nd == 3 ? (long long)bdm->size[1] * bdm->size[2] : 0, bdm->size[nd - 1], dmh)))
                 return rc;
         }
         const size_t ro = (size_t)(a->rec_toff ? t1 : t0) * p.slot_elems;
@@ -198,7 +215,7 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
                           vsave->size[0]);
                 return B2_ERR_INVALID;
             }
-            if ((rc = launch_imaging(p, *grad, gh, (const float *)usave->d + (size_t)time * p.slot_elems, p.u,
+            if ((rc = launch_imaging(p, grad3, gh, (const float *)usave->d + (size_t)time * p.slot_elems, p.u,
                                      (const float *)vsave->d + (size_t)time * p.slot_elems, p.v, t0, t1, t2)))
                 return rc;
         }
@@ -229,6 +246,10 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
 
 extern "C" int b2_tti_forward(const struct b2_tti_args *a) {
     if (!a || !a->u || !a->v) { set_error("b2_tti_forward: NULL args"); return B2_ERR_INVALID; }
+    if (a->ndim != 0 && a->ndim != 2 && a->ndim != 3) {
+        set_error("b2_tti_forward: ndim must be 2 or 3 (0: 3)");
+        return B2_ERR_INVALID;
+    }
     if (a->time_M < a->time_m) return B2_OK;
     std::lock_guard<std::mutex> api_lock(api_mutex());
     if (int rc0 = use_device(a->deviceid)) return rc0;

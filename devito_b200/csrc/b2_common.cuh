@@ -167,7 +167,9 @@ int launch_imaging(const Plan &p, const DevArray &grad, int gh, const float *us,
     k.gsx = (long long)grad.size[1] * grad.size[2];
     k.n0 = p.n[0]; k.n1 = p.n[1]; k.n2 = p.n[2];
     k.o0 = p.o[0]; k.o1 = p.o[1]; k.o2 = p.o[2];
-    k.g0 = p.o[0] - p.so + gh; k.g1 = p.o[1] - p.so + gh; k.g2 = p.o[2] - p.so + gh;
+    // o[0] == 0 only on the dummy leading dim of a 2-D plan (a grid dim starts at its halo, so >= 1): index 0 there
+    k.g0 = p.o[0] == 0 ? 0 : p.o[0] - p.so + gh;
+    k.g1 = p.o[1] - p.so + gh; k.g2 = p.o[2] - p.so + gh;
     k.inv_dt2 = 1.0f / (p.dt * p.dt);
     return launch_imaging(k);
 }

@@ -36,8 +36,9 @@ struct TtiK {
     int n0, n1, n2;
     int o0, o1, o2;
     int R;
+    int rx;                    // taps on dim 0: R, or 0 on the dummy dim of a 2-D plan
     float m_dt2, inv_dt;
-    float cx, cy, cz;          // sin(th)cos(ph), sin(th)sin(ph), cos(th)
+    float cx, cy, cz;          // sin(th)cos(ph), sin(th)sin(ph), cos(th); 2-D: 0, sin(th), cos(th)
     float e2, sd;              // 1+2eps, sqrt(1+2delta)
     float w2[3][B2_MAX_RADIUS + 1];
     float w1[3][B2_MAX_RADIUS];
@@ -59,14 +60,15 @@ __global__ void __launch_bounds__(256)
 k_tti_tables(const float *__restrict__ vp, const float *__restrict__ eps, const float *__restrict__ delta,
              const float *__restrict__ theta, const float *__restrict__ phi, float vp_s, float eps_s,
              float delta_s, float theta_s, float phi_s, float inv_dt2, float *Cx, float *Cy, float *Cz,
-             float *E2, float *SD, float *MD, size_t n) {
+             float *E2, float *SD, float *MD, size_t n, int two_d) {
     size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     for (; i < n; i += stride) {
         const float th = theta ? theta[i] : theta_s, ph = phi ? phi[i] : phi_s;
         const float st = sinf(th), ct = cosf(th);
-        Cx[i] = st * cosf(ph);
-        Cy[i] = st * sinf(ph);
+        // 2-D (1, x, z): `Gzz_centered_2d`'s rotation (sin th, cos th) on the plan's dims 1, 2; no Cx
+        if (!two_d) Cx[i] = st * cosf(ph);
+        Cy[i] = two_d ? st : st * sinf(ph);
         Cz[i] = ct;
         E2[i] = 2.0f * (eps ? eps[i] : eps_s) + 1.0f;
         SD[i] = sqrtf(2.0f * (delta ? delta[i] : delta_s) + 1.0f);
@@ -77,19 +79,19 @@ k_tti_tables(const float *__restrict__ vp, const float *__restrict__ eps, const 
 
 // pass A: Gz over the box extended by [-R/2, R/2-1]
 __global__ void __launch_bounds__(256) k_tti_gz(TtiK k) {
-    const int h = k.R / 2;
+    const int h = k.R / 2, hx = k.rx / 2;
     const int z = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     if (z >= k.n2 + k.R || y >= k.n1 + k.R) return;
-    for (int x = blockIdx.z; x < k.n0 + k.R; x += gridDim.z) {
-        const long long idx = (long long)(k.o0 + x - h) * k.sx + (long long)(k.o1 + y - h) * k.sy + (k.o2 + z - h);
+    for (int x = blockIdx.z; x < k.n0 + k.rx; x += gridDim.z) {
+        const long long idx = (long long)(k.o0 + x - hx) * k.sx + (long long)(k.o1 + y - h) * k.sy + (k.o2 + z - h);
         float dxu = 0.f, dyu = 0.f, dzu = 0.f, dxv = 0.f, dyv = 0.f, dzv = 0.f;
         for (int j = 0; j < k.R; ++j) {
             const int off = j - h + 1;
-            dxu = fmaf(k.w1[0][j], k.u0[idx + off * k.sx], dxu);
+            if (k.rx) dxu = fmaf(k.w1[0][j], k.u0[idx + off * k.sx], dxu);
             dyu = fmaf(k.w1[1][j], k.u0[idx + off * k.sy], dyu);
             dzu = fmaf(k.w1[2][j], k.u0[idx + off], dzu);
-            dxv = fmaf(k.w1[0][j], k.v0[idx + off * k.sx], dxv);
+            if (k.rx) dxv = fmaf(k.w1[0][j], k.v0[idx + off * k.sx], dxv);
             dyv = fmaf(k.w1[1][j], k.v0[idx + off * k.sy], dyv);
             dzv = fmaf(k.w1[2][j], k.v0[idx + off], dzv);
         }
@@ -113,7 +115,7 @@ __global__ void __launch_bounds__(256) k_tti_update(TtiK k) {
         const float uc = k.u0[idx], vc = k.v0[idx];
         float lap = (k.w2[0][0] + k.w2[1][0] + k.w2[2][0]) * uc;
         for (int i = 1; i <= k.R; ++i) {
-            lap = fmaf(k.w2[0][i], k.u0[idx - i * k.sx] + k.u0[idx + i * k.sx], lap);
+            if (k.rx) lap = fmaf(k.w2[0][i], k.u0[idx - i * k.sx] + k.u0[idx + i * k.sx], lap);
             lap = fmaf(k.w2[1][i], k.u0[idx - i * k.sy] + k.u0[idx + i * k.sy], lap);
             lap = fmaf(k.w2[2][i], k.u0[idx - i] + k.u0[idx + i], lap);
         }
@@ -121,12 +123,12 @@ __global__ void __launch_bounds__(256) k_tti_update(TtiK k) {
         for (int j = 0; j < k.R; ++j) {
             const int off = j - h;
             const long long ix = idx + off * k.sx, iy = idx + off * k.sy, iz = idx + off;
-            const float cx = k.tCx ? k.tCx[ix] : k.cx, cy = k.tCy ? k.tCy[iy] : k.cy,
+            const float cx = !k.rx ? 0.f : k.tCx ? k.tCx[ix] : k.cx, cy = k.tCy ? k.tCy[iy] : k.cy,
                         cz = k.tCz ? k.tCz[iz] : k.cz;
-            gu = fmaf(cx * k.w1[0][j], k.gzu[ix], gu);
+            if (k.rx) gu = fmaf(cx * k.w1[0][j], k.gzu[ix], gu);
             gu = fmaf(cy * k.w1[1][j], k.gzu[iy], gu);
             gu = fmaf(cz * k.w1[2][j], k.gzu[iz], gu);
-            gv = fmaf(cx * k.w1[0][j], k.gzv[ix], gv);
+            if (k.rx) gv = fmaf(cx * k.w1[0][j], k.gzv[ix], gv);
             gv = fmaf(cy * k.w1[1][j], k.gzv[iy], gv);
             gv = fmaf(cz * k.w1[2][j], k.gzv[iz], gv);
         }
@@ -998,6 +1000,341 @@ k_tti_ws(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUten
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// 2-D single-pass sweep k_tti2d<R, ARR, ADJ> (radius 2 or 4): the 2-D reduction of k_tti_fused.
+// ------------------------------------------------------------------------------------------
+// A CTA owns a z-segment of TZ = 512 points (128 consumer threads, four consecutive z points each) and marches
+// along x over a chunk of rows. Per iteration (output row x):
+//   producer warp : TMA-loads the haloed rows u[t](x+R), v[t](x+R) (ARR: the sin / cos tables of row x+H-1) into
+//                   shared rings, D rows ahead of the consumers;
+//   stage A       : Gz(u), Gz(v) of row g = x+H-1 once, when its last input row has arrived: own columns from the
+//                   register queue of u and the shared v rows, the two halo groups of the segment by one lane of
+//                   each consumer warp; stored in a shared ring of H+1 rows and, for the own column, in register
+//                   queues of R rows;
+//   stage B       : the Laplacian (x-taps from the register queue of u, z-taps from the shared row), the outer
+//                   half-node derivatives of Gz (x from the register queues, z from the shared row), the coupled
+//                   update with A = 1/(m/dt^2 + damp/dt), 16-byte stores.
+// u[t] and v[t] come from HBM once per step apart from the 2R rows that prime each chunk and the halo columns of
+// each segment. Bytes per point: 28 with scalar parameters (u, v at t and t-1, A; u, v at t+1 written), 48 with
+// arrays (+ sin, cos, 1+2eps, sqrt(1+2delta), m/dt^2); the adjoint reads the two mixes and p, r at t in place of u,
+// v at t (and of the eps / delta tables): 36 and 48.
+template <int R, bool ARR>
+struct Tti2dCfg {
+    static constexpr int H = R / 2;
+    static constexpr int NC = 128;                   // consumer threads
+    static constexpr int TZ = 4 * NC;                // z points of a segment
+    static constexpr int RZ = 32;                    // halo columns on either side (128 B: TMA destinations aligned)
+    static constexpr int NBOX = 3, BOXZ = 192;       // TMA boxes of a row: <= 256 elements, 128-byte multiples
+    static constexpr int BZ = NBOX * BOXZ;           // = TZ + 2 RZ
+    static constexpr int D = ARR ? 3 : 4;            // batches the producer may run ahead of the slowest consumer
+    static constexpr int NU = R + D;                 // u / v rows x .. x+R, + (D-1) in flight
+    static constexpr int NCR = R + D - 1;            // ARR: factor rows x-H .. x+H-1, + (D-1) in flight
+    static constexpr int NG = H + 1;                 // Gz rows x .. x+H (stage A of x+1 writes x+H while B reads x)
+    static constexpr int NB = 4;                     // barrier ring (>= D)
+    static constexpr int MINB = R == 2 ? 3 : 2;      // CTAs per SM the registers must allow (R = 4: no spills)
+    static constexpr size_t SMEM = (size_t)(2 * NU + 2 * NG + (ARR ? 2 * NCR : 0)) * BZ * 4 + 2 * NB * 8;
+    static_assert(BZ == TZ + 2 * RZ && RZ >= 8 && NB >= D, "2-D TTI sweep layout");
+};
+
+struct Tti2dK {
+    float *__restrict__ u1;
+    float *__restrict__ v1;
+    const float *__restrict__ um;
+    const float *__restrict__ vm;
+    const float *__restrict__ A;
+    const float *__restrict__ tE2;     // ARR, forward
+    const float *__restrict__ tSD;
+    const float *__restrict__ tMD;     // ARR
+    const float *__restrict__ pc;      // ADJ: p[t], r[t] (the tensor maps cover the mixes)
+    const float *__restrict__ rc;
+    long long sr;                      // row stride (the allocated z extent)
+    int nx, nz, ox, oz;                // box extents and the array index of its first point
+    int lx, ntz, slot0;
+    float m_dt2, e2, sd;
+    float w2x[5], w2z[5];
+    float w1x[4], w1z[4];              // scalar: multiplied by sin(th) / cos(th); ARR: the raw weights
+};
+
+template <int N>
+__device__ __forceinline__ int ring_(int r) { return (r + 64 * N) % N; }      // rows >= -2R > -64 N
+
+template <int R, bool ARR, bool ADJ>
+__global__ void __launch_bounds__(Tti2dCfg<R, ARR>::NC + 32, Tti2dCfg<R, ARR>::MINB)
+k_tti2d(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_v,
+        const __grid_constant__ CUtensorMap tm_s, const __grid_constant__ CUtensorMap tm_c, const Tti2dK k) {
+    using C = Tti2dCfg<R, ARR>;
+    constexpr int H = C::H, NC = C::NC, TZ = C::TZ, RZ = C::RZ, BZ = C::BZ, D = C::D;
+    constexpr int NU = C::NU, NG = C::NG, NB = C::NB, NCW = NC / 32;
+    constexpr int NCR = ARR ? C::NCR : 1;
+    constexpr int PRE = 2 * R;                      // priming iterations before the first output row
+    constexpr uint32_t ROWB = (uint32_t)BZ * 4;
+
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    float *s_u = reinterpret_cast<float *>(smem_raw);
+    float *s_v = s_u + NU * BZ;
+    float *s_gu = s_v + NU * BZ;
+    float *s_gv = s_gu + NG * BZ;
+    float *s_c = s_gv + NG * BZ;                    // ARR: [row mod NCR][sin, cos][BZ]
+    uint64_t *full = reinterpret_cast<uint64_t *>(s_c + (ARR ? 2 * NCR * BZ : 0));
+    uint64_t *empty = full + NB;
+
+    const int iz = blockIdx.x % k.ntz;
+    const int z0 = iz * TZ;
+    const int xs = (blockIdx.x / k.ntz) * k.lx;
+    const int xe = min(xs + k.lx, k.nx);
+    const int NIT = (xe - xs) + PRE;                // iterations: x = xs - PRE + it
+
+    const int tid = threadIdx.x;
+    const int warp = tid >> 5, lane = tid & 31;
+
+    if (tid == 0) {
+        for (int i = 0; i < NB; ++i) {
+            b2ptx::mbar_init(&full[i], 1);
+            b2ptx::mbar_init(&empty[i], NCW);
+        }
+        b2ptx::fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp == NCW) {
+        if (lane == 0) {
+            b2ptx::tma_prefetch_desc(&tm_u);
+            b2ptx::tma_prefetch_desc(&tm_v);
+            if constexpr (ARR) {
+                b2ptx::tma_prefetch_desc(&tm_s);
+                b2ptx::tma_prefetch_desc(&tm_c);
+            }
+            for (int it = 0; it < NIT; ++it) {
+                const int x = xs - PRE + it;
+                if (it >= D) {
+                    const int w = it - D;
+                    b2ptx::mbar_wait(&empty[w % NB], (w / NB) & 1);
+                }
+                const int q = x + R;                        // u / v row of this batch
+                const bool hv = q >= xs - R + 1;            // v rows below xs-R+1 are never read
+                const int qc = x + H - 1;                   // ARR: factor row of stage A
+                const bool hc = ARR && qc >= xs - H;
+                b2ptx::mbar_arrive_expect_tx(&full[it % NB], ROWB * ((hv ? 2u : 1u) + (hc ? 2u : 0u)));
+                float *du = s_u + ring_<NU>(q) * BZ, *dv = s_v + ring_<NU>(q) * BZ;
+#pragma unroll
+                for (int b = 0; b < C::NBOX; ++b) {
+                    const int zc = k.oz + z0 - RZ + b * C::BOXZ;
+                    b2ptx::tma_load_4d(du + b * C::BOXZ, &tm_u, &full[it % NB], zc, k.ox + q, 0, k.slot0);
+                    if (hv) b2ptx::tma_load_4d(dv + b * C::BOXZ, &tm_v, &full[it % NB], zc, k.ox + q, 0, k.slot0);
+                    if constexpr (ARR) {
+                        if (hc) {
+                            float *dc = s_c + ring_<NCR>(qc) * 2 * BZ + b * C::BOXZ;
+                            b2ptx::tma_load_4d(dc, &tm_s, &full[it % NB], zc, k.ox + qc, 0, 0);
+                            b2ptx::tma_load_4d(dc + BZ, &tm_c, &full[it % NB], zc, k.ox + qc, 0, 0);
+                        }
+                    }
+                }
+            }
+        }
+        return;
+    }
+
+    // ---------------- consumers ----------------
+    const int gz = z0 + 4 * tid;
+    const int zcnt = min(max(k.nz - gz, 0), 4);
+    const int my = RZ + 4 * tid;                    // own column in a row
+    // halo group of this warp's lane 0: field (warp & 1: v), side (warp >> 1: right)
+    const int hoff = (warp >> 1) ? RZ + TZ : RZ - 4;
+    const bool hfv = warp & 1;
+
+    float4 uq[2 * R + 1];                           // u rows x-R .. x+R, own column
+    float4 gqu[R], gqv[R];                          // Gz(u), Gz(v) rows x-H .. x+H-1, own column
+#pragma unroll
+    for (int i = 0; i <= 2 * R; ++i) uq[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int i = 0; i < R; ++i) gqu[i] = gqv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    const float wc = k.w2x[0] + k.w2z[0];
+    long long gi = (long long)(k.ox + xs - PRE) * k.sr + (k.oz + gz);
+
+    auto zwin = [](const float *c, float (&o)[12]) {      // the z points c-4 .. c+7
+        const float4 l = b2ptx::lds128(c - 4), m = b2ptx::lds128(c), r = b2ptx::lds128(c + 4);
+        o[0] = l.x; o[1] = l.y; o[2] = l.z; o[3] = l.w; o[4] = m.x; o[5] = m.y;
+        o[6] = m.z; o[7] = m.w; o[8] = r.x; o[9] = r.y; o[10] = r.z; o[11] = r.w;
+    };
+    // Gz of four consecutive points: D+x from `xr` (rows g-H+1 .. g+H), D+z from the row window `zz` of row g,
+    // factors `fs` / `fc` at the points (ARR)
+    auto gz4 = [&](const float4 (&xr)[R], const float (&zz)[12], float4 fs, float4 fc) -> float4 {
+        float4 dx = make_float4(0.f, 0.f, 0.f, 0.f), dz = dx;
+#pragma unroll
+        for (int j = 0; j < R; ++j) f4fma_(dx, k.w1x[j], xr[j]);
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+            const int o = 4 + j - H + 1;
+            dz.x = fmaf(k.w1z[j], zz[o + 0], dz.x); dz.y = fmaf(k.w1z[j], zz[o + 1], dz.y);
+            dz.z = fmaf(k.w1z[j], zz[o + 2], dz.z); dz.w = fmaf(k.w1z[j], zz[o + 3], dz.w);
+        }
+        if constexpr (ARR)
+            return make_float4(tti2d_gz_point(fs.x, fc.x, dx.x, dz.x), tti2d_gz_point(fs.y, fc.y, dx.y, dz.y),
+                               tti2d_gz_point(fs.z, fc.z, dx.z, dz.z), tti2d_gz_point(fs.w, fc.w, dx.w, dz.w));
+        return make_float4(dx.x + dz.x, dx.y + dz.y, dx.z + dz.z, dx.w + dz.w);   // weights hold sin / cos
+    };
+    auto ldt = [](const float *q) -> float4 {            // streams read once: no L1 allocation
+        float4 r;
+        asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
+                     : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(q));
+        return r;
+    };
+    auto ld4 = [&](const float *q) -> float4 {
+        if (zcnt == 4) return ldt(q + gi);
+        float t[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int i = 0; i < zcnt; ++i) t[i] = q[gi + i];
+        return make_float4(t[0], t[1], t[2], t[3]);
+    };
+
+    for (int it = 0; it < NIT; ++it) {
+        const int x = xs - PRE + it;
+        const bool out = x >= xs && zcnt > 0;
+        // loads of the output row issued first, so that stages A and B hide their latency
+        float4 pu = make_float4(0.f, 0.f, 0.f, 0.f), pv = pu, pa = pu, pe2 = pu, psd = pu, pmd = pu, pcn = pu, rcn = pu;
+        if (out) {
+            pu = ld4(k.um);
+            pv = ld4(k.vm);
+            pa = ld4(k.A);
+            if constexpr (ADJ) {
+                pcn = ld4(k.pc);
+                rcn = ld4(k.rc);
+            }
+            if constexpr (ARR) {
+                if constexpr (!ADJ) {
+                    pe2 = ld4(k.tE2);
+                    psd = ld4(k.tSD);
+                }
+                pmd = ld4(k.tMD);
+            }
+        }
+        b2ptx::mbar_wait(&full[it % NB], (it / NB) & 1);
+        const int q = x + R;
+#pragma unroll
+        for (int i = 0; i < 2 * R; ++i) uq[i] = uq[i + 1];
+        uq[2 * R] = b2ptx::lds128(s_u + ring_<NU>(q) * BZ + my);
+
+        // ---- stage A: Gz at row g = x + H - 1 (inputs: rows x .. x+R-1) ----
+        const int g = x + H - 1;
+        if (g >= xs - H) {
+            const float *fs_row = ARR ? s_c + ring_<NCR>(g) * 2 * BZ : nullptr;
+            float zz[12];
+            float4 xr[R];
+            float4 fs = make_float4(0.f, 0.f, 0.f, 0.f), fc = fs;
+            // own column, u
+#pragma unroll
+            for (int j = 0; j < R; ++j) xr[j] = uq[R + j];
+            zwin(s_u + ring_<NU>(g) * BZ + my, zz);
+            if constexpr (ARR) {
+                fs = b2ptx::lds128(fs_row + my);
+                fc = b2ptx::lds128(fs_row + BZ + my);
+            }
+            const float4 gu = gz4(xr, zz, fs, fc);
+            // own column, v
+#pragma unroll
+            for (int j = 0; j < R; ++j) xr[j] = b2ptx::lds128(s_v + ring_<NU>(x + j) * BZ + my);
+            zwin(s_v + ring_<NU>(g) * BZ + my, zz);
+            const float4 gv = gz4(xr, zz, fs, fc);
+            *reinterpret_cast<float4 *>(s_gu + ring_<NG>(g) * BZ + my) = gu;
+            *reinterpret_cast<float4 *>(s_gv + ring_<NG>(g) * BZ + my) = gv;
+#pragma unroll
+            for (int i = 0; i < R - 1; ++i) {
+                gqu[i] = gqu[i + 1];
+                gqv[i] = gqv[i + 1];
+            }
+            gqu[R - 1] = gu;
+            gqv[R - 1] = gv;
+            // the segment's halo groups: one per consumer warp
+            if (lane == 0) {
+                const float *ring = hfv ? s_v : s_u;
+#pragma unroll
+                for (int j = 0; j < R; ++j) xr[j] = b2ptx::lds128(ring + ring_<NU>(x + j) * BZ + hoff);
+                zwin(ring + ring_<NU>(g) * BZ + hoff, zz);     // inside the row: RZ >= 8
+                if constexpr (ARR) {
+                    fs = b2ptx::lds128(fs_row + hoff);
+                    fc = b2ptx::lds128(fs_row + BZ + hoff);
+                }
+                *reinterpret_cast<float4 *>((hfv ? s_gv : s_gu) + ring_<NG>(g) * BZ + hoff) = gz4(xr, zz, fs, fc);
+            }
+        }
+        // Gz of row x written by every consumer warp must be visible before its z neighbours are read
+        asm volatile("bar.sync 1, %0;" ::"n"(NC) : "memory");
+
+        // ---- stage B: output row x ----
+        if (x >= xs) {
+            const float4 c = uq[R];
+            const float4 vcn = b2ptx::lds128(s_v + ring_<NU>(x) * BZ + my);
+            float zr[12];
+            zwin(s_u + ring_<NU>(x) * BZ + my, zr);
+            float4 lap = make_float4(wc * c.x, wc * c.y, wc * c.z, wc * c.w);
+#pragma unroll
+            for (int i = 1; i <= R; ++i) {
+                lap.x = fmaf(k.w2z[i], zr[4 - i] + zr[4 + i], lap.x);
+                lap.y = fmaf(k.w2z[i], zr[5 - i] + zr[5 + i], lap.y);
+                lap.z = fmaf(k.w2z[i], zr[6 - i] + zr[6 + i], lap.z);
+                lap.w = fmaf(k.w2z[i], zr[7 - i] + zr[7 + i], lap.w);
+            }
+#pragma unroll
+            for (int i = 1; i <= R; ++i) {
+                const float4 a = uq[R - i], bb = uq[R + i];
+                lap.x = fmaf(k.w2x[i], a.x + bb.x, lap.x); lap.y = fmaf(k.w2x[i], a.y + bb.y, lap.y);
+                lap.z = fmaf(k.w2x[i], a.z + bb.z, lap.z); lap.w = fmaf(k.w2x[i], a.w + bb.w, lap.w);
+            }
+            // Gzz(u), Gzz(v): outer half-node derivatives of (factor * Gz) at offsets -H .. H-1
+            float4 zu4 = make_float4(0.f, 0.f, 0.f, 0.f), zv4 = zu4;
+#pragma unroll
+            for (int j = 0; j < R; ++j) {                       // x: rows x-H+j, sin(th) at those rows
+                float4 w = make_float4(k.w1x[j], k.w1x[j], k.w1x[j], k.w1x[j]);
+                if constexpr (ARR) {
+                    const float4 f = b2ptx::lds128(s_c + ring_<NCR>(x - H + j) * 2 * BZ + my);
+                    w = make_float4(f.x * k.w1x[j], f.y * k.w1x[j], f.z * k.w1x[j], f.w * k.w1x[j]);
+                }
+                zu4.x = fmaf(w.x, gqu[j].x, zu4.x); zu4.y = fmaf(w.y, gqu[j].y, zu4.y);
+                zu4.z = fmaf(w.z, gqu[j].z, zu4.z); zu4.w = fmaf(w.w, gqu[j].w, zu4.w);
+                zv4.x = fmaf(w.x, gqv[j].x, zv4.x); zv4.y = fmaf(w.y, gqv[j].y, zv4.y);
+                zv4.z = fmaf(w.z, gqv[j].z, zv4.z); zv4.w = fmaf(w.w, gqv[j].w, zv4.w);
+            }
+            {                                                   // z: row x, cos(th) at z+j-H
+                float au[12], av[12], cz[12];
+                zwin(s_gu + ring_<NG>(x) * BZ + my, au);
+                zwin(s_gv + ring_<NG>(x) * BZ + my, av);
+                if constexpr (ARR) zwin(s_c + ring_<NCR>(x) * 2 * BZ + BZ + my, cz);
+#pragma unroll
+                for (int j = 0; j < R; ++j) {
+                    const int o = 4 + j - H;
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const float w = ARR ? cz[o + e] * k.w1z[j] : k.w1z[j];
+                        float &ru = e == 0 ? zu4.x : e == 1 ? zu4.y : e == 2 ? zu4.z : zu4.w;
+                        float &rv = e == 0 ? zv4.x : e == 1 ? zv4.y : e == 2 ? zv4.z : zv4.w;
+                        ru = fmaf(w, au[o + e], ru);
+                        rv = fmaf(w, av[o + e], rv);
+                    }
+                }
+            }
+            float4 ou, ov;
+#define B2_TTI2D_UPD(F)                                                                                      \
+            if constexpr (ADJ)                                                                                   \
+                tti_update_adj_point(lap.F, zu4.F, zv4.F, pcn.F, rcn.F, pu.F, pv.F, pa.F, ARR ? pmd.F : k.m_dt2, \
+                                     ou.F, ov.F);                                                                \
+            else                                                                                                 \
+                tti_update_point(lap.F, zu4.F, zv4.F, c.F, vcn.F, pu.F, pv.F, pa.F, ARR ? pmd.F : k.m_dt2,       \
+                                 ARR ? pe2.F : k.e2, ARR ? psd.F : k.sd, ou.F, ov.F);
+            B2_TTI2D_UPD(x) B2_TTI2D_UPD(y) B2_TTI2D_UPD(z) B2_TTI2D_UPD(w)
+#undef B2_TTI2D_UPD
+            if (zcnt == 4) {
+                *reinterpret_cast<float4 *>(k.u1 + gi) = ou;
+                *reinterpret_cast<float4 *>(k.v1 + gi) = ov;
+            } else if (zcnt > 0) {
+                const float tu[4] = {ou.x, ou.y, ou.z, ou.w}, tv[4] = {ov.x, ov.y, ov.z, ov.w};
+                for (int i = 0; i < zcnt; ++i) { k.u1[gi + i] = tu[i]; k.v1[gi + i] = tv[i]; }
+            }
+        }
+        __syncwarp();
+        if (lane == 0) b2ptx::mbar_arrive(&empty[it % NB]);
+        gi += k.sr;
+    }
+}
+
 __global__ void __launch_bounds__(256)
 k_tti_coef_arr(const float *__restrict__ damp, const float *__restrict__ md, float inv_dt, float *__restrict__ A, size_t n) {
     size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
@@ -1068,6 +1405,63 @@ static int tti_scratch(int which, size_t elems, float **out) {
     return B2_OK;
 }
 
+// the per-point tables of k_tti_tables (array-valued parameters)
+static int tti_tables(TtiPlan &p) {
+    int rc;
+    B2_SM_COUNT(sms);
+    float **t[6] = {&p.tCx, &p.tCy, &p.tCz, &p.tE2, &p.tSD, &p.tMD};
+    for (int i = p.ndim == 2; i < 6; ++i)      // a 2-D plan has no rotation factor on its dummy dim: tCx stays NULL
+        if ((rc = tti_scratch(3 + i, p.slot_elems, t[i]))) return rc;
+    k_tti_tables<<<sms * 8, 256, 0, stream()>>>(p.vp_a, p.eps_a, p.delta_a, p.theta_a, p.phi_a, p.vp, p.epsilon,
+                                                 p.delta, p.theta, p.phi, 1.0f / (p.dt * p.dt), p.tCx, p.tCy, p.tCz,
+                                                 p.tE2, p.tSD, p.tMD, p.slot_elems, p.ndim == 2);
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
+}
+
+// tensor maps of the 2-D sweep over the field pair (u, v) of `tsize` slots: boxes of one row segment
+static int tti2d_maps(const TtiPlan &p, const float *u, const float *v, int tsize, TtiPlan &out) {
+    constexpr int BOXZ = Tti2dCfg<2, false>::BOXZ;
+    int rc;
+    if ((rc = tti_make_tmap(&out.tm_u, u, p.a, tsize, BOXZ, 1))) return rc;
+    return tti_make_tmap(&out.tm_v, v, p.a, tsize, BOXZ, 1);
+}
+
+static int tti_plan_init_2d(TtiPlan &p, int kernel) {
+    const bool ok = kernel != 1 && (p.R == 2 || p.R == 4) && p.a[2] % 4 == 0 && p.o[2] % 4 == 0 &&
+                    (uintptr_t)p.u % 16 == 0 && (uintptr_t)p.v % 16 == 0;
+    if (kernel == 2 && !ok) {
+        set_error("tti: 2-D single-pass kernel forced but layout does not qualify (radius=%d, z extent %d and "
+                  "z start %d must be multiples of 4, u and v 16-byte aligned)", p.R, p.a[2], p.o[2]);
+        return B2_ERR_INVALID;
+    }
+    p.use_2d = ok;
+    int rc;
+    if (p.has_arrays && (rc = tti_tables(p))) return rc;
+    if (!ok) {
+        if ((rc = tti_scratch(1, p.slot_elems, &p.gzu))) return rc;
+        return tti_scratch(2, p.slot_elems, &p.gzv);
+    }
+    if ((rc = tti_scratch(0, p.slot_elems, &p.coefA))) return rc;
+    B2_SM_COUNT(sms);
+    const float inv_dt = 1.0f / p.dt;
+    if (p.has_arrays)
+        k_tti_coef_arr<<<sms * 8, 256, 0, stream()>>>(p.damp, p.tMD, inv_dt, p.coefA, p.slot_elems);
+    else
+        k_tti_coef<<<sms * 8, 256, 0, stream()>>>(p.damp, (1.0f / (p.vp * p.vp)) * (inv_dt * inv_dt), inv_dt,
+                                                  p.coefA, p.slot_elems);
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    if ((rc = tti2d_maps(p, p.u, p.v, p.tsize, p))) return rc;
+    if (p.has_arrays) {       // sin(th), cos(th) of `Gzz_centered_2d`
+        constexpr int BOXZ = Tti2dCfg<2, false>::BOXZ;
+        if ((rc = tti_make_tmap(&p.tm_cy, p.tCy, p.a, 1, BOXZ, 1))) return rc;
+        if ((rc = tti_make_tmap(&p.tm_cz, p.tCz, p.a, 1, BOXZ, 1))) return rc;
+    }
+    return B2_OK;
+}
+
 int tti_plan_init(TtiPlan &p, int kernel) {
     p.kernel = kernel;
     if (p.R % 2 != 0 || p.R < 2 || p.R > B2_MAX_RADIUS) {
@@ -1075,6 +1469,7 @@ int tti_plan_init(TtiPlan &p, int kernel) {
         return B2_ERR_INVALID;
     }
     p.has_arrays = p.vp_a || p.eps_a || p.delta_a || p.theta_a || p.phi_a;
+    if (p.ndim == 2) return tti_plan_init_2d(p, kernel);
     bool ok = (p.R == 2 || p.R == 4) && (p.a[2] % 4 == 0) && (p.o[2] % 4 == 0) &&
               ((uintptr_t)p.u % 16 == 0) && ((uintptr_t)p.v % 16 == 0) && (p.slot_elems % 4 == 0) &&
               p.n[1] >= 8 && p.n[2] >= 16;
@@ -1092,18 +1487,7 @@ int tti_plan_init(TtiPlan &p, int kernel) {
     p.arr_fused = ok && p.has_arrays;
     int rc;
     B2_SM_COUNT(sms);
-    auto tables = [&]() -> int {
-        float **t[6] = {&p.tCx, &p.tCy, &p.tCz, &p.tE2, &p.tSD, &p.tMD};
-        for (int i = 0; i < 6; ++i)
-            if ((rc = tti_scratch(3 + i, p.slot_elems, t[i]))) return rc;
-        k_tti_tables<<<sms * 8, 256, 0, stream()>>>(p.vp_a, p.eps_a, p.delta_a, p.theta_a, p.phi_a, p.vp,
-                                                     p.epsilon, p.delta, p.theta, p.phi,
-                                                     1.0f / (p.dt * p.dt), p.tCx, p.tCy, p.tCz, p.tE2,
-                                                     p.tSD, p.tMD, p.slot_elems);
-        count_launch();
-        B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
-        return B2_OK;
-    };
+    auto tables = [&]() -> int { return tti_tables(p); };
     if (ok) {
         if ((rc = tti_scratch(0, p.slot_elems, &p.coefA))) return rc;
         const float inv_dt = 1.0f / p.dt;
@@ -1139,12 +1523,13 @@ int tti_plan_retarget(const TtiPlan &p, float *u, float *v, TtiPlan &out) {
     out = p;
     out.u = u;
     out.v = v;
-    if (!p.use_fused) return B2_OK;
+    if (!p.use_fused && !p.use_2d) return B2_OK;
     if ((uintptr_t)u % 16 != 0 || (uintptr_t)v % 16 != 0) {
         set_error("tti: the second field pair is not 16-byte aligned, so it cannot run the fused kernel of the first");
         return B2_ERR_INVALID;
     }
     int rc;
+    if (p.use_2d) return tti2d_maps(p, u, v, p.tsize, out);
     if ((rc = tti_make_tmap(&out.tm_u, u, p.a, p.tsize, 72, p.tm_rows))) return rc;
     if ((rc = tti_make_tmap(&out.tm_v, v, p.a, p.tsize, 72, p.tm_rows))) return rc;
     return B2_OK;
@@ -1159,6 +1544,7 @@ int tti_plan_adjoint(const TtiPlan &p, TtiPlan &out) {
     out.ma = a;
     out.mb = b;
     out.adj = true;
+    if (p.use_2d) return tti2d_maps(p, a, b, 1, out);
     if (p.use_fused) {      // one slot each (cudaMalloc'ed, so 16-byte aligned): the sweep reads slot 0 of the maps
         // the scalar so=8 adjoint sweeps with k_tti_fused<4> where the forward takes k_tti_ws (its own tile height)
         if (!p.arr_fused) out.tm_rows = (p.R == 2 ? TtiTile<2>::TY : TtiTile<4>::TY) + 2 * p.R;
@@ -1240,8 +1626,9 @@ int tti_born_source(const TtiPlan &p, const TtiPlan &pd, int slot0, int slotm, i
     k.du1 = pd.u + (size_t)slot1 * p.slot_elems;
     k.dv1 = pd.v + (size_t)slot1 * p.slot_elems;
     // the fused plans tabulated A; the two-pass plans have m/dt^2 per point only with array parameters
-    k.A = p.use_fused ? p.coefA : nullptr;
-    k.tMD = p.use_fused ? nullptr : p.tMD;
+    const bool tabA = p.use_fused || p.use_2d;
+    k.A = tabA ? p.coefA : nullptr;
+    k.tMD = tabA ? nullptr : p.tMD;
     k.damp = p.damp;
     k.dm = dm;
     k.sx = p.sx;
@@ -1250,7 +1637,8 @@ int tti_born_source(const TtiPlan &p, const TtiPlan &pd, int slot0, int slotm, i
     k.dsy = dsy;
     k.n0 = p.n[0]; k.n1 = p.n[1]; k.n2 = p.n[2];
     k.o0 = p.o[0]; k.o1 = p.o[1]; k.o2 = p.o[2];
-    k.dg0 = p.o[0] - p.so + dmh; k.dg1 = p.o[1] - p.so + dmh; k.dg2 = p.o[2] - p.so + dmh;
+    k.dg0 = p.ndim == 2 ? 0 : p.o[0] - p.so + dmh;      // 2-D: dim 0 is the plan's dummy dim
+    k.dg1 = p.o[1] - p.so + dmh; k.dg2 = p.o[2] - p.so + dmh;
     k.inv_dt = 1.0f / p.dt;
     k.inv_dt2 = 1.0f / (p.dt * p.dt);
     k.m_dt2 = (1.0f / (p.vp * p.vp)) * k.inv_dt2;
@@ -1447,8 +1835,61 @@ static int tti_launch_fused(const TtiPlan &p, int slot0, int slotm, int slot1, i
     return B2_OK;
 }
 
+// the 2-D single-pass sweep over the plan's rows (grid x), every z-segment
+template <int R, bool ARR>
+static int tti2d_launch(const TtiPlan &p, int slot0, int slotm, int slot1) {
+    using C = Tti2dCfg<R, ARR>;
+    auto kern = p.adj ? k_tti2d<R, ARR, true> : k_tti2d<R, ARR, false>;
+    static bool attr_set[2] = {false, false};
+    static int occ[2] = {0, 0};
+    if (!attr_set[p.adj]) {
+        B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM), B2_ERR_LAUNCH);
+        B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[p.adj], kern, C::NC + 32, C::SMEM), B2_ERR_LAUNCH);
+        attr_set[p.adj] = true;
+    }
+    Tti2dK k;
+    memset(&k, 0, sizeof(k));
+    k.u1 = p.u + (size_t)slot1 * p.slot_elems;
+    k.v1 = p.v + (size_t)slot1 * p.slot_elems;
+    k.um = p.u + (size_t)slotm * p.slot_elems;
+    k.vm = p.v + (size_t)slotm * p.slot_elems;
+    k.A = p.coefA;
+    if (ARR) { k.tE2 = p.tE2; k.tSD = p.tSD; k.tMD = p.tMD; }
+    k.pc = p.adj ? p.u + (size_t)slot0 * p.slot_elems : nullptr;
+    k.rc = p.adj ? p.v + (size_t)slot0 * p.slot_elems : nullptr;
+    k.slot0 = p.adj ? 0 : slot0;
+    k.sr = p.sy;
+    k.nx = p.n[1];
+    k.nz = p.n[2];
+    k.ox = p.o[1];
+    k.oz = p.o[2];
+    k.ntz = (k.nz + C::TZ - 1) / C::TZ;
+    B2_SM_COUNT(sms);
+    k.lx = std::min(choose_chunk_len((long long)sms * std::max(occ[p.adj], 1), k.ntz, k.nx, 2 * R, 32), k.nx);
+    const unsigned nblk = (unsigned)(k.ntz * ((k.nx + k.lx - 1) / k.lx));
+    k.m_dt2 = (1.0f / (p.vp * p.vp)) * (1.0f / (p.dt * p.dt));
+    k.e2 = 1.0f + 2.0f * p.epsilon;
+    k.sd = sqrtf(1.0f + 2.0f * p.delta);
+    const float st = ARR ? 1.f : sinf(p.theta), ct = ARR ? 1.f : cosf(p.theta);
+    for (int i = 0; i <= R; ++i) { k.w2x[i] = p.w2[1][i]; k.w2z[i] = p.w2[2][i]; }
+    for (int i = 0; i < R; ++i) { k.w1x[i] = st * p.w1[1][i]; k.w1z[i] = ct * p.w1[2][i]; }
+    timing_begin();
+    note_sweep_kernel("tti2d%s<%d>%s", ARR ? "_arr" : "", R, p.adj ? "+adj" : "");
+    kern<<<nblk, C::NC + 32, C::SMEM, stream()>>>(p.tm_u, p.tm_v, ARR ? p.tm_cy : p.tm_u, ARR ? p.tm_cz : p.tm_u, k);
+    timing_end();
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
+}
+
 int tti_step(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount) {
     if (xcount <= 0) return B2_OK;
+    if (p.use_2d) {
+        if (p.R == 2) return p.has_arrays ? tti2d_launch<2, true>(p, slot0, slotm, slot1)
+                                          : tti2d_launch<2, false>(p, slot0, slotm, slot1);
+        return p.has_arrays ? tti2d_launch<4, true>(p, slot0, slotm, slot1)
+                            : tti2d_launch<4, false>(p, slot0, slotm, slot1);
+    }
     if (p.arr_fused)
         return p.R == 2 ? tti_launch_fused_arr<2>(p, slot0, slotm, slot1, xlo, xcount)
                         : tti_launch_fused_arr<4>(p, slot0, slotm, slot1, xlo, xcount);
@@ -1476,19 +1917,24 @@ int tti_step(const TtiPlan &p, int slot0, int slotm, int slot1, int xlo, int xco
     k.o1 = p.o[1];
     k.o2 = p.o[2];
     k.R = p.R;
+    k.rx = p.ndim == 2 ? 0 : p.R;
     k.inv_dt = 1.0f / p.dt;
     k.m_dt2 = (1.0f / (p.vp * p.vp)) * (1.0f / (p.dt * p.dt));
     const float st = sinf(p.theta), ct = cosf(p.theta), sp = sinf(p.phi), cp = cosf(p.phi);
     k.cx = st * cp;
     k.cy = st * sp;
     k.cz = ct;
+    if (p.ndim == 2) {
+        k.cx = 0.f;
+        k.cy = st;
+    }
     k.e2 = 1.0f + 2.0f * p.epsilon;
     k.sd = sqrtf(1.0f + 2.0f * p.delta);
     memcpy(k.w2, p.w2, sizeof(k.w2));
     memcpy(k.w1, p.w1, sizeof(k.w1));
     k.tCx = p.tCx; k.tCy = p.tCy; k.tCz = p.tCz; k.tE2 = p.tE2; k.tSD = p.tSD; k.tMD = p.tMD;
     dim3 block(64, 4, 1);
-    dim3 gridA((k.n2 + k.R + 63) / 64, (k.n1 + k.R + 3) / 4, (unsigned)std::min(xcount + k.R, 65535));
+    dim3 gridA((k.n2 + k.R + 63) / 64, (k.n1 + k.R + 3) / 4, (unsigned)std::min(xcount + k.rx, 65535));
     timing_begin();
     note_sweep_kernel("tti_two_pass%s", p.adj ? "+adj" : "");
     k_tti_gz<<<gridA, block, 0, stream()>>>(k);

@@ -4,7 +4,10 @@
 
 namespace b2 {
 
+// A 2-D grid (x, z) is planned as (1, x, z): extent 1 and no stencil taps on the leading dim, rotation factors
+// (0, sin theta, cos theta). Its sweeps march along the grid's x, the plan's dim 1.
 struct TtiPlan {
+    int ndim = 3;                // 2 or 3
     int R = 4;                   // radius = space_order/2 (even)
     int so = 8;
     int a[3] = {1, 1, 1};
@@ -33,6 +36,7 @@ struct TtiPlan {
     float *tCx = nullptr, *tCy = nullptr, *tCz = nullptr, *tE2 = nullptr, *tSD = nullptr, *tMD = nullptr;
     bool has_arrays = false;
     int tm_rows = 0;             // rows of the u / v tensor-map boxes (fused plans)
+    bool use_2d = false;         // 2-D single-pass sweep k_tti2d (tm_u / tm_v: row boxes; ARR: tm_cy / tm_cz)
     // adjoint plan (tti_plan_adjoint): the sweep's stencil inputs are the one-slot mixes ma = e2 p + sd r and
     // mb = sd p + r (library scratch, tm_u / tm_v cover them), combined with (1, 0); u / v stay p / r, whose level
     // slot0 gives the centre of the update, slotm the previous level and slot1 the level written

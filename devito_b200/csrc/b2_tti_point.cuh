@@ -1,5 +1,5 @@
-// One-point forms of the centred-TTI Born source term (k_tti_born_src, b2_tti.cu) and of the adjoint's field mix
-// (k_tti_adj_mix).
+// One-point forms of the centred-TTI Born source term (k_tti_born_src, b2_tti.cu), of the adjoint's field mix
+// (k_tti_adj_mix) and of the 2-D sweep's Gz and time update (k_tti2d).
 //
 // `__host__ __device__` like b2_iso_point.cuh, so that tests/support/emu_points.cu can loop the SAME body on the
 // CPU and compare it with the float64 reference without a GPU.
@@ -72,6 +72,30 @@ B2_HD void tti_born_point(const TtiBK &k, int x, int y, int z) {
 B2_HD void tti_adj_mix_point(float e2, float sd, float p, float r, float &a, float &b) {
     a = fmaf(e2, p, sd * r);
     b = fmaf(sd, p, r);
+}
+
+// The 2-D sweep k_tti2d (b2_tti.cu), one point at a time. With D+x f, D+z f the half-node first derivatives at the Gz
+// point and s, c = sin(theta), cos(theta) there, Gz = s D+x f + c D+z f (`Gzz_centered_2d`).
+B2_HD float tti2d_gz_point(float s, float c, float dxf, float dzf) { return fmaf(c, dzf, s * dxf); }
+
+// The time update of the forward pair from lap(u), Gzz(u), Gzz(v) at the point, the centre u, v at t, the level t-1
+// (um, vm), A = 1/(m/dt^2 + damp/dt) and md = m/dt^2: H0 = e2 (lap - Gzz u) + sd Gzz v, Hz = sd (lap - Gzz u) + Gzz v,
+// f[t+1] = f + A (md (f - f[t-1]) + H) -- the reference's (md (2 f - f[t-1]) + damp/dt f + H) / (md + damp/dt).
+B2_HD void tti_update_point(float lap, float gzzu, float gzzv, float uc, float vc, float um, float vm, float A,
+                            float md, float e2, float sd, float &ou, float &ov) {
+    const float gh = lap - gzzu;
+    const float H0 = fmaf(e2, gh, sd * gzzv);
+    const float Hz = fmaf(sd, gh, gzzv);
+    ou = fmaf(A, fmaf(md, uc - um, H0), uc);
+    ov = fmaf(A, fmaf(md, vc - vm, Hz), vc);
+}
+
+// The adjoint pair: lap / gzza of the mix a = e2 p + sd r, gzzb of b = sd p + r (tti_adj_mix_point), the centre p, r at
+// t and the level t+1 (pm, rm): H0 = lap(a) - Gzz(a), Hz = Gzz(b), f[t-1] = f + A (md (f - f[t+1]) + H).
+B2_HD void tti_update_adj_point(float lapa, float gzza, float gzzb, float pc, float rc, float pm, float rm, float A,
+                                float md, float &op, float &orr) {
+    op = fmaf(A, fmaf(md, pc - pm, lapa - gzza), pc);
+    orr = fmaf(A, fmaf(md, rc - rm, gzzb), rc);
 }
 
 }  // namespace b2

@@ -218,9 +218,7 @@ def wave_entry(p):
         params = [Param(n + '_arr', n, p['consts'].get(n), 1.0 if n == 'vp' else 0.0, False, False)
                   for n in ('vp', 'epsilon', 'delta', 'theta', 'phi')]
     flags = {'space_order': p['so'], 'radius': p['R'], 'adjoint': int(bool(p.get('adjoint'))),
-             'rec_toff': p['rec_toff']}
-    if kind != 'tti':
-        flags['ndim'] = p['grid'].dim
+             'rec_toff': p['rec_toff'], 'ndim': p['grid'].dim}
     if kind == 'iso':
         flags.update(free_surface=int(bool(p.get('free_surface'))), ot4=int(bool(p.get('ot4'))))
         if p.get('snap') is not None:
@@ -1203,8 +1201,9 @@ class Operator:
     def _recognise_tti(self, updates, injs, itps, adjoint=False):
         (u, equ), (v, eqv) = updates
         grid = u.grid
-        if grid.dim != 3 or v.grid is not grid:
-            raise _Unrecognised("TTI fast path is 3-D only")
+        nd = grid.dim
+        if nd not in (2, 3) or v.grid is not grid:
+            raise _Unrecognised("TTI fast path needs a 2-D or 3-D grid shared by both fields")
         so = u.space_order
         if so != v.space_order or so % 4 or so // 2 > 8:
             raise _Unrecognised(f"TTI needs space_order multiple of 4 (got {so})")
@@ -1239,6 +1238,8 @@ class Operator:
                 raise _Unrecognised(f"unknown coefficient field {f.name}")
         if any(n not in byname for n in ('vp', 'epsilon', 'delta', 'theta')):
             raise _Unrecognised("TTI fast path needs vp/epsilon/delta/theta[/phi] (Constants or Functions)")
+        if nd == 2 and 'phi' in byname:
+            raise _Unrecognised("a 2-D TTI update has no azimuth phi")
         for n in (c for c in consts if c.name not in pnames):
             raise _Unrecognised(f"unknown Constant {n.name} in the TTI update")
         # every access of damp must be at the centre
@@ -1258,7 +1259,7 @@ class Operator:
             # also checks WHERE each factor is sampled (the reference samples the rotation factors
             # at the shifted points of the outer derivative, tti/operators.py:92-102)
             base = {n: rng.uniform(0.2, 0.8) for n in pnames}
-            gradv = {n: (rng.uniform(-0.02, 0.02, size=3) if isinstance(byname.get(n), Function) else np.zeros(3))
+            gradv = {n: (rng.uniform(-0.02, 0.02, size=nd) if isinstance(byname.get(n), Function) else np.zeros(nd))
                      for n in pnames}
             if 'phi' not in byname:
                 base['phi'] = 0.0
@@ -1279,13 +1280,13 @@ class Operator:
                         raise _Unrecognised("non-affine parameter access")
                     return P(f.name, k[1])
                 if n.is_Constant:
-                    return P(n.name, (0, 0, 0))
+                    return P(n.name, (0,) * nd)
                 if n.name == dtsym.name:
                     return dt
                 if n.name in spv:
                     return spv[n.name]
                 raise _Unrecognised(f"unknown symbol {n.name}")
-            pu, pv = predict_tti(w2, w1, R, P, dval, dt, adjoint=adjoint)
+            pu, pv = predict_tti(w2, w1, R, P, dval, dt, adjoint=adjoint, nd=nd)
             for got, pred, nm in ((ku, pu, 'u'), (kv, pv, 'v')):
                 keys = set(got) | set(pred)
                 for k in keys:
@@ -1381,15 +1382,15 @@ class Operator:
                         raise _Unrecognised("dm accessed off-centre")
         dtsym = plan['dt']
         spv = {sp.name: float(v) for sp, v in grid.spacing_map.items()}
-        zero = (0, 0, 0)
+        zero = (0,) * grid.dim
         rng = np.random.default_rng(2718)
         errors = []
         for du, dv, own_u, ext_u, own_v, ext_v in cand:
             try:
                 for probe in range(2):
                     base = {n: rng.uniform(0.2, 0.8) for n in pnames}
-                    gradv = {n: (rng.uniform(-0.02, 0.02, size=3) if isinstance(consts.get(n), Function)
-                                 else np.zeros(3)) for n in pnames}
+                    gradv = {n: (rng.uniform(-0.02, 0.02, size=grid.dim) if isinstance(consts.get(n), Function)
+                                 else np.zeros(grid.dim)) for n in pnames}
                     if 'phi' not in consts:
                         base['phi'] = 0.0
                     dt = rng.uniform(0.5, 2.0)
@@ -1686,6 +1687,8 @@ class Operator:
         if grid.distributor.is_parallel:
             if p['kind'] == 'sa':
                 raise InvalidArgument("the self-adjoint update does not run on a decomposed grid in this version")
+            if p['kind'] == 'tti' and grid.dim == 2:
+                raise InvalidArgument("2-D TTI modelling does not run on a decomposed grid in this version")
             if p['kind'] == 'tti' and p.get('adjoint'):
                 raise InvalidArgument("the TTI adjoint does not run on a decomposed grid in this version")
             if 'born_du' in args:
@@ -2164,22 +2167,26 @@ def predict_sa(c, R, nd, bval, vp, w, dt, dirn):
 # the stencil the TTI kernels implement, as linear coefficients (float64) — used only by the
 # recogniser to confirm that a user's equations are this scheme.
 # ---------------------------------------------------------------------------------------------
-def predict_tti(w2, w1, R, P, damp, dt, adjoint=False):
+def predict_tti(w2, w1, R, P, damp, dt, adjoint=False, nd=3):
     """`P(name, offset)` -> value of parameter `name` sampled `offset` grid points from the output
     point (constants ignore the offset). `adjoint`: the backward pair of `kernel_centered(..., forward=False)`,
-    H0 = Gh(e2 p + sd r), Hz = Gzz(sd p + r) with e2, sd sampled at each tap point, the previous level t+1."""
+    H0 = Gh(e2 p + sd r), Hz = Gzz(sd p + r) with e2, sd sampled at each tap point, the previous level t+1.
+    `nd` = 2: the rotation (sin theta, cos theta) on (x, z) of `Gzz_centered_2d`."""
     h = R // 2
-    z3 = (0, 0, 0)
+    z3 = (0,) * nd
 
     def C(off):
-        th, ph = P('theta', off), P('phi', off)
-        st, ct, sp, cp = np.sin(th), np.cos(th), np.sin(ph), np.cos(ph)
-        return [st * cp, st * sp, ct]
+        th = P('theta', off)
+        st, ct = np.sin(th), np.cos(th)
+        if nd == 2:
+            return [st, ct]
+        ph = P('phi', off)
+        return [st * np.cos(ph), st * np.sin(ph), ct]
     e2 = 1 + 2 * P('epsilon', z3)
     sd = np.sqrt(1 + 2 * P('delta', z3))
 
     def unit(d, o):
-        v = [0, 0, 0]
+        v = [0] * nd
         v[d] = o
         return tuple(v)
 
@@ -2188,17 +2195,17 @@ def predict_tti(w2, w1, R, P, damp, dt, adjoint=False):
 
     # Gzz = sum_d D-_d ( C_d(q) * Gz(q) ),  Gz(q) = sum_e C_e(q) D+_e f(q)
     gzz = {}
-    for d in range(3):
+    for d in range(nd):
         for j in range(R):
             q = unit(d, j - h)
             cq = C(q)
-            for e in range(3):
+            for e in range(nd):
                 for i in range(R):
                     off = tuple(a + b for a, b in zip(q, unit(e, i - h + 1)))
                     add(gzz, off, w1[d][j] * cq[d] * cq[e] * w1[e][i])
     lap = {}
     add(lap, z3, sum(w[0] for w in w2))
-    for d in range(3):
+    for d in range(nd):
         for k in range(1, R + 1):
             add(lap, unit(d, k), w2[d][k])
             add(lap, unit(d, -k), w2[d][k])

@@ -9,16 +9,25 @@ __all__ = ['kernel_centered', 'ForwardOperator', 'AdjointOperator', 'JacobianOpe
 
 
 def trig_func(model):
+    """operators.py `trig_func`: (cos theta, sin theta) on a 2-D model, which has no azimuth, and (cos theta, sin theta,
+    cos phi, sin phi) in 3-D."""
     theta = getattr(model, 'theta', 0)
+    grid = getattr(model, 'grid', None)
+    if getattr(model, 'dim', grid.dim if grid is not None else 3) == 2:
+        return cos(theta), sin(theta)
     phi = getattr(model, 'phi', 0)
     return cos(theta), sin(theta), cos(phi), sin(phi)
+
+
+def _order1(field):
+    # `field` may be an expression (the adjoint's mixes): its order is that of the fields it reads
+    return (field.space_order if hasattr(field, 'space_order') else field._default_fd_order) // 2
 
 
 def Gzz_centered(model, field):
     """Rotated second derivative along the symmetry axis (operators.py:65-104)."""
     costheta, sintheta, cosphi, sinphi = trig_func(model)
-    # `field` may be an expression (the adjoint's mixes): its order is that of the fields it reads
-    order1 = (field.space_order if hasattr(field, 'space_order') else field._default_fd_order) // 2
+    order1 = _order1(field)
     x, y, z = field.grid.dimensions if hasattr(field, 'grid') else model.grid.dimensions
     dx, dy, dz = x.spacing / 2, y.spacing / 2, z.spacing / 2
     Gz = (sintheta * cosphi * field.dx(fd_order=order1, x0=x + dx) +
@@ -32,6 +41,21 @@ def Gzz_centered(model, field):
     return Gzz
 
 
+def Gzz_centered_2d(model, field):
+    """The 2-D rotated second derivative along the symmetry axis (operators.py `Gzz_centered_2d`): the rotation
+    (sin theta, cos theta) on (x, z)."""
+    costheta, sintheta = trig_func(model)
+    order1 = _order1(field)
+    x, z = field.grid.dimensions if hasattr(field, 'grid') else model.grid.dimensions
+    dx, dz = x.spacing / 2, z.spacing / 2
+    Gz = (sintheta * field.dx(fd_order=order1, x0=x + dx) +
+          costheta * field.dy(fd_order=order1, x0=z + dz))
+    Gzz = (Gz * costheta).dy(fd_order=order1, x0=z - dz)
+    if sintheta != 0:
+        Gzz += (Gz * sintheta).dx(fd_order=order1, x0=x - dx)
+    return Gzz
+
+
 def _is_zero(q):
     return isinstance(q, (int, float)) and q == 0
 
@@ -41,17 +65,18 @@ def kernel_centered(model, u, v, qu=0, qv=0, forward=True):
     operator passes -dm * u0.dt2 / -dm * v0.dt2). `forward=False` builds the adjoint pair: H0 = Gh(e2 u + sd v),
     Hz = Gzz(sd u + v), solved for u.backward / v.backward with the transposed damping term."""
     delta, epsilon = sqrt(1 + 2 * model.delta), 1 + 2 * model.epsilon
+    Gzz_centered_ = Gzz_centered_2d if model.dim == 2 else Gzz_centered
     if not forward:
         m, damp = model.m, model.damp
         a, b = epsilon * u + delta * v, delta * u + v
-        H0 = a.laplace - Gzz_centered(model, a)
-        Hz = Gzz_centered(model, b)
+        H0 = a.laplace - Gzz_centered_(model, a)
+        Hz = Gzz_centered_(model, b)
         stencilp = solve(m * u.dt2 - H0 - qu + damp * u.dt.T, u.backward)
         stencilr = solve(m * v.dt2 - Hz - qv + damp * v.dt.T, v.backward)
         sd = model.grid.subdomains['physdomain']
         return [Eq(u.backward, stencilp, subdomain=sd), Eq(v.backward, stencilr, subdomain=sd)]
-    Gxx = u.laplace - Gzz_centered(model, u)
-    Gzz = Gzz_centered(model, v)
+    Gxx = u.laplace - Gzz_centered_(model, u)
+    Gzz = Gzz_centered_(model, v)
     H0 = epsilon * Gxx + delta * Gzz
     Hz = delta * Gxx + Gzz
     m, damp = model.m, model.damp
@@ -69,8 +94,8 @@ def kernel_centered(model, u, v, qu=0, qv=0, forward=True):
 
 def ForwardOperator(model, geometry, space_order=4, save=False, kernel='centered', **kwargs):
     """operators.py:431-480"""
-    if kernel != 'centered' or model.dim != 3:
-        raise NotImplementedError("only the 3-D centred TTI kernel is on this backend's path")
+    if kernel != 'centered':
+        raise NotImplementedError("only the centred TTI kernel is on this backend's path")
     dt = model.grid.time_dim.spacing
     m = model.m
     u = TimeFunction(name='u', grid=model.grid, save=geometry.nt if save else None, time_order=2,
@@ -87,8 +112,8 @@ def ForwardOperator(model, geometry, space_order=4, save=False, kernel='centered
 def AdjointOperator(model, geometry, space_order=4, kernel='centered', **kwargs):
     """operators.py `AdjointOperator`: the adjoint pair (p, r) driven by the receivers, injected into
     (p.backward, r.backward); the adjoint source `srca` samples p + r."""
-    if kernel != 'centered' or model.dim != 3:
-        raise NotImplementedError("only the 3-D centred TTI kernel is on this backend's path")
+    if kernel != 'centered':
+        raise NotImplementedError("only the centred TTI kernel is on this backend's path")
     dt = model.grid.time_dim.spacing
     m = model.m
     p = TimeFunction(name='p', grid=model.grid, time_order=2, space_order=space_order)
@@ -104,8 +129,6 @@ def AdjointOperator(model, geometry, space_order=4, kernel='centered', **kwargs)
 def JacobianOperator(model, geometry, space_order=4, **kwargs):
     """operators.py:532-586: the background pair (u0, v0) driven by the source, the linearised pair (du, dv) by
     -dm * u0.dt2 / -dm * v0.dt2, the receivers sampling du + dv."""
-    if model.dim != 3:
-        raise NotImplementedError("only the 3-D centred TTI kernel is on this backend's path")
     dt = model.grid.stepping_dim.spacing
     m = model.m
     mk = lambda n: TimeFunction(name=n, grid=model.grid, save=None, time_order=2, space_order=space_order)
@@ -122,8 +145,6 @@ def JacobianOperator(model, geometry, space_order=4, **kwargs):
 def JacobianAdjOperator(model, geometry, space_order=4, save=True, **kwargs):
     """operators.py `JacobianAdjOperator`: the adjoint pair (du, dv) driven by the receivers and the imaging
     condition Inc(dm, -(u0 * du.dt2 + v0 * dv.dt2)) with the saved forward wavefields u0, v0."""
-    if model.dim != 3:
-        raise NotImplementedError("only the 3-D centred TTI kernel is on this backend's path")
     dt = model.grid.stepping_dim.spacing
     m = model.m
     mk = lambda n, nt: TimeFunction(name=n, grid=model.grid, save=nt, time_order=2, space_order=space_order)

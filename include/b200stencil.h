@@ -164,9 +164,9 @@ struct b2_iso_args {
 int b2_iso_forward(const struct b2_iso_args *a);
 
 /* ---- TTI centred forward (replaces generated `ForwardTTI`,
- *      examples/seismic/tti/operators.py:186-247, 431-480), scalar Thomsen parameters ----- */
+ *      examples/seismic/tti/operators.py:186-247, 431-480), 2-D and 3-D ----------------------- */
 struct b2_tti_args {
-    int space_order;                  /* 3-D only                                           */
+    int space_order;                  /* halo width of u / v                                */
     int radius;                       /* space_order/2                                      */
     const float *w2[3];               /* 2nd-derivative weights incl 1/h^2, [0..radius]     */
     const float *w1[3];               /* half-node 1st-derivative weights incl 1/h:         *
@@ -214,6 +214,14 @@ struct b2_tti_args {
      * without usave and vsave, grad without adjoint, or a saved field whose space layout differs from u's
      * returns 210.                                                                                          */
     struct b2_dataobj *grad, *usave, *vsave;
+    /* 0 or 3: a 3-D grid. 2: a 2-D grid (x, z) (the reference's `Gzz_centered_2d`, tti/operators.py): u, v are
+     * (tsize, x+2so, z+2so), every space array is (x, z) with its halo, w2 / w1 / x_m..y_M carry x and z in slots 0
+     * and 1 (z_m / z_M ignored), and the rotation is (sin theta, cos theta) on (x, z). A 2-D call takes no azimuth:
+     * phi != 0, phi_arr != NULL or halo != NULL returns 210. kernel 0 sweeps with the single-pass k_tti2d<R> when
+     * the layout qualifies (radius 2 or 4, z extent and z start multiples of 4, 16-byte aligned arrays), else with
+     * the two-pass kernels; kernel 2 on a layout that does not qualify returns 210. b2_last_sweep_kernel reports
+     * "tti2d<R>" / "tti2d_arr<R>" (array parameters) or "tti_two_pass", with the suffixes of the 3-D calls.    */
+    int ndim;
 };
 int b2_tti_forward(const struct b2_tti_args *a);
 
