@@ -19,6 +19,64 @@ TOL = {'iso': 1e-5, 'tti': 1e-4}       # rel L-inf against float64 (BASELINE.jso
 TTI_SCALARS = dict(vp=2.0, epsilon=0.2, delta=0.1, theta=0.6, phi=0.35)
 SUBBOX = ((1, 2, 4), (SHAPE[0] - 3, SHAPE[1] - 4, SHAPE[2] - 9))   # reaches the halo in x and y, z_m % 4 == 0
 
+# Boxes on SHAPE whose z extent is not a multiple of 4, z_m % 4 == 0 (so the TMA sweeps still take them): the last
+# float4 group of every row holds 1, 2 or 3 points and goes through the sweeps' partial (scalar) loads and stores.
+# face3 reaches every face; unlike a grid of nz = 67 (an allocation the TMA sweeps refuse) its allocation is aligned.
+ZTAIL = {
+    'tail1': ((1, 2, 4), (34, 41, 60)),        # z extent 57
+    'tail2': ((1, 2, 4), (34, 41, 61)),        # 58
+    'tail3': ((1, 2, 4), (34, 41, 62)),        # 59
+    'face3': ((0, 0, 0), (36, 44, 66)),        # 67
+}
+# The size gate of iso_plan_init / tti_plan_init: boxes with n[1] < 8 or n[2] < 16 run the generic / two-pass kernels.
+GATE = {
+    'gate_in': ((1, 2, 4), (8, 9, 19)),        # n = (8, 8, 16): the TMA / fused sweep
+    'gate_y': ((1, 2, 4), (8, 8, 19)),         # n = (8, 7, 16): falls back
+    'gate_z': ((1, 2, 4), (8, 9, 15)),         # n = (8, 8, 12): falls back
+}
+# One x-plane (the 2.5-D march primes 2R planes for one output plane), z extent 59
+XPLANE = ((5, 2, 4), (5, 41, 62))
+# Boxes for the sweeps without a size gate (sa_plan_init), z_m % 4 == 0: a corner point, a corner float4 group at the
+# far faces, a small interior box with a z tail of 3
+TINY = {
+    'tiny111': ((0, 0, 0), (0, 0, 0)),
+    'tiny114': ((36, 44, 64), (36, 44, 67)),
+    'tiny257': ((3, 5, 8), (4, 9, 14)),
+}
+BOXES = dict(ZTAIL, **GATE, xplane=XPLANE, **TINY, sub=SUBBOX)
+
+# Grids cut into several yz-tiles by every iso tile configuration (TILES):
+#   MULTI: >= 2 y tiles and >= 3 z tiles, the last of each partial. 16 x 128: 3 x 3 tiles, the last 12 x 44;
+#          32 x 64: 2 x 5, the last 12 x 44; 16 x 64: 3 x 5, the last 12 x 44; 8 x 64: 6 x 5, the last 4 x 44.
+#   EXACT: every tile full. 16 x 128: 2 x 2; 32 x 64: 1 x 4; 16 x 64: 2 x 4; 8 x 64: 4 x 4.
+MULTI = (13, 44, 300)
+MULTI_TAIL = ((0, 0, 0), (12, 43, 297))        # z extent 298: 16 x 128 tiles 3 x 3, the last 12 x 42
+EXACT = (9, 32, 256)
+
+# (TY, TZ) of the yz-tile each 3-D sweep marches along x, per `b2_last_sweep_kernel` name
+TILES = {
+    # b2_iso.cu TileOf<R, ARR>: (TY, 4 TZ4)
+    'iso_tma<2,scalar>': (32, 64), 'iso_tma<2,vp>': (32, 64), 'iso_tma<2,m>': (32, 64),
+    'iso_tma<4,scalar>': (16, 128), 'iso_tma<4,vp>': (32, 64), 'iso_tma<4,m>': (32, 64),
+    'iso_tma<6,scalar>': (16, 64), 'iso_tma<6,vp>': (16, 64), 'iso_tma<6,m>': (16, 64),
+    'iso_tma<8,scalar>': (8, 64), 'iso_tma<8,vp>': (8, 64), 'iso_tma<8,m>': (8, 64),
+    # b2_tti.cu TtiTile<R>::TY, kTtiWsTY, TtiArrTile<R>::TY; TZ: TtiCfg / TtiWsCfg
+    'tti_fused<2>': (32, 64), 'tti_fused<4>': (28, 64), 'tti_ws<pf1>': (24, 64),
+    'tti_arr_ct2<2>': (30, 64), 'tti_arr_ct2<4>': (20, 64),
+    # b2_sa.cu SaTmaCfg<R>
+    'sa_tma<2>': (16, 64), 'sa_tma<4>': (16, 64),
+}
+
+
+def tiling(n, t):
+    """(number of tiles, extent of the last one) of an extent n cut into tiles of t"""
+    k = -(-n // t)
+    return k, n - (k - 1) * t
+
+
+def box_extent(box):
+    return tuple(h - l + 1 for l, h in zip(*box))
+
 
 def _alloc(shape, so):
     return tuple(n + 2 * so for n in shape)
@@ -37,7 +95,7 @@ def iso_case(so, param, shape=SHAPE, box=None, seed=0):
                 dt=float(O.critical_dt(so, 3, min(SPACING), 2.5)))
 
 
-def tti_case(so, arrays, shape=SHAPE, seed=0):
+def tti_case(so, arrays, shape=SHAPE, box=None, seed=0):
     """arrays: vp, epsilon, delta, theta, phi as white-noise fields (else the scalars TTI_SCALARS, phi != 0)."""
     rng = np.random.default_rng(seed + 100 * so + 7)
     a = _alloc(shape, so)
@@ -49,8 +107,9 @@ def tti_case(so, arrays, shape=SHAPE, seed=0):
         params = {n: rng.uniform(lo, hi, a).astype(np.float32) for n, (lo, hi) in rg.items()}
     else:
         params = {n: np.float32(x) for n, x in TTI_SCALARS.items()}
-    return dict(kind='tti', so=so, shape=shape, u=u, v=v, damp=damp, params=params, lo=(0, 0, 0),
-                hi=tuple(n - 1 for n in shape), dt=float(O.critical_dt(so, 3, min(SPACING), 2.5, eps_max=0.3)))
+    lo, hi = box if box is not None else ((0,) * len(shape), tuple(n - 1 for n in shape))
+    return dict(kind='tti', so=so, shape=shape, u=u, v=v, damp=damp, params=params, lo=tuple(lo), hi=tuple(hi),
+                dt=float(O.critical_dt(so, 3, min(SPACING), 2.5, eps_max=0.3)))
 
 
 def sparse_coordinates(shape=SHAPE, seed=3):

@@ -57,6 +57,8 @@ MUTATIONS = {
     'c_at_output': "TTI: the outer derivative takes C_d at the output point instead of the shifted point",
     'tail_y': "the last row of the box in y is not updated",
     'tail_z': "the last four points of the box in z (one float4 group) are not updated",
+    'tail_z_over': "the 1-3 points past z_M in the last float4 group of a row are updated too",
+    'tail_z_short': "the last n2 % 4 points of the box in z (a partial float4 group) are not updated",
     'swap_levels': "u and u- exchanged in the update",
     'adj_inject_level': "adjoint: the sources are injected into u[t] instead of the level just written",
     'fs_surface_tap': "free surface: the vertical tap landing on z = 0 reads u[0] instead of contributing 0",
@@ -105,6 +107,14 @@ def _bounds(shape, so, lo, hi):
     lo = list(lo) if lo is not None else [0] * len(n)
     hi = list(hi) if hi is not None else [x - 1 for x in n]
     return lo, hi
+
+
+def _update_hi(lo, hi, mut):
+    """The upper corner of the points a kernel updates: with 'tail_z_over', the z extent rounded up to whole float4
+    groups (the sparse points still see the box as given)."""
+    if mut != 'tail_z_over':
+        return hi
+    return list(hi[:-1]) + [lo[-1] + (hi[-1] - lo[-1] + 4) // 4 * 4 - 1]
 
 
 def _halo_zeroed(f, so):
@@ -263,7 +273,8 @@ def iso_forward(u, so, w, dt, time_m, time_M, damp=None, param=('vp', 1.5), lo=N
     w = _weights(w, mut)
     if free_surface:
         assert lo[-1] == 0, "a free surface needs the box to start at z = 0"
-    S_ = _Iso(so, w, dt, damp, param, lo, hi, mut)
+    uhi = _update_hi(lo, hi, mut)
+    S_ = _Iso(so, w, dt, damp, param, lo, uhi, mut)
     box = S_.box
     if mut == 'transpose_xy':
         _transpose_xy(u)
@@ -281,11 +292,11 @@ def iso_forward(u, so, w, dt, time_m, time_M, damp=None, param=('vp', 1.5), lo=N
         H = S_.H(u0, ot4)
         new = S_.new(u0, u[t2], H)
         if free_surface:
-            corr, rows = _fs_correction(u0, w, lo, hi, so, mut)
+            corr, rows = _fs_correction(u0, w, lo, uhi, so, mut)
             new[..., :rows] += corr / (S_.den[..., :rows] if np.ndim(S_.den) else S_.den)
             if mut != 'fs_keep_row0':
                 new[..., 0] = 0.0
-        _store(u[t1], new, lo, hi, so, mut)
+        _store(u[t1], new, lo, uhi, so, mut)
         if S is not None:
             S.inject([u[t0] if mut == 'adj_inject_level' else u[t1]], time, inj_scale)
         if snap is not None and time % snap_factor == 0:
@@ -349,6 +360,9 @@ def _store(f1, new, lo, hi, so, mut):
         new[:, -1, :] = f1[box][:, -1, :]
     elif mut == 'tail_z':
         new[:, :, -4:] = f1[box][:, :, -4:]
+    elif mut == 'tail_z_short' and new.shape[-1] % 4:
+        k = new.shape[-1] % 4
+        new[:, :, -k:] = f1[box][:, :, -k:]
     f1[box] = new
 
 
@@ -362,15 +376,16 @@ def tti_forward(u, v, so, w2, w1, dt, time_m, time_M, damp, params, lo=None, hi=
     R = so // 2
     h = R // 2
     lo, hi = _bounds(u.shape[1:], so, lo, hi)
+    uhi = _update_hi(lo, hi, mut)
     w2 = _weights(w2, mut)
     w1 = _weights(w1, mut)
     P = {k: _shifted(np.asarray(x, dtype=np.float64), mut) for k, x in params.items()}
-    box = _box(lo, hi, so)
+    box = _box(lo, uhi, so)
     # Gz is needed on the box grown by [-h, h-1]: the points q of the outer derivative
     elo = [x - h for x in lo]
-    ehi = [x + h - 1 for x in hi]
+    ehi = [x + h - 1 for x in uhi]
     ebox = _box(elo, ehi, so)
-    nb = [b - a + 1 for a, b in zip(lo, hi)]
+    nb = [b - a + 1 for a, b in zip(lo, uhi)]
     st, ct = np.sin(P['theta']), np.cos(P['theta'])
     sp, cp = np.sin(P['phi']), np.cos(P['phi'])
     Call = [st * cp, st * sp, ct * np.ones_like(sp)]
@@ -411,13 +426,13 @@ def tti_forward(u, v, so, w2, w1, dt, time_m, time_M, damp, params, lo=None, hi=
             t0, t2 = t2, t0
         u0 = _halo_zeroed(u[t0], so) if mut == 'halo_zero' else u[t0]
         v0 = _halo_zeroed(v[t0], so) if mut == 'halo_zero' else v[t0]
-        lap = _lap(u0, w2, lo, hi, so)
+        lap = _lap(u0, w2, lo, uhi, so)
         gu, gv = gzz(u0), gzz(v0)
         den = m / dt ** 2 + d / dt
         un = (e2 * (lap - gu) + sd * gv + m / dt ** 2 * (2 * u0[box] - u[t2][box]) + d / dt * u0[box]) / den
         vn = (sd * (lap - gu) + gv + m / dt ** 2 * (2 * v0[box] - v[t2][box]) + d / dt * v0[box]) / den
-        _store(u[t1], un, lo, hi, so, mut)
-        _store(v[t1], vn, lo, hi, so, mut)
+        _store(u[t1], un, lo, uhi, so, mut)
+        _store(v[t1], vn, lo, uhi, so, mut)
         if S is not None:
             S.inject([u[t1], v[t1]], time, inj_scale)
         if R_ is not None:

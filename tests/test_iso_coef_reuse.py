@@ -35,14 +35,20 @@ def _profile(n, so):
     return (0.08 * d * d).astype(np.float32)
 
 
+# x-planes perturbed inside the box, and the one perturbed outside the box's rows, per grid
+PERTURBED = {KC.SHAPE: ((9, 12, 24), 17),                      # 12, 24: first planes of B2_ISO_LX=12 chunks
+             KC.MULTI: ((2, 5, 10), 7)}
+
+
 def layered_damp(shape, so, lo):
     """sum of per-axis profiles (float32, x + y + z), then perturbed planes; lo: the box's lower corner"""
     p = [_profile(n, so) for n in shape]
     damp = (p[0][:, None, None] + p[1][None, :, None]) + p[2][None, None, :]
     y, z = so + lo[1] + 3, so + lo[2] + 5                        # inside every box used below
-    for x in (9, 12, 24):                                        # 12, 24: first planes of B2_ISO_LX=12 chunks
+    inside, outside = PERTURBED[shape]
+    for x in inside:
         damp[so + x, y, z] += np.float32(1e-3)
-    damp[so + 17, so + lo[1] - 1, z] += np.float32(1e-3)         # outside the box's rows: still repeated
+    damp[so + outside, so + lo[1] - 1, z] += np.float32(1e-3)   # outside the box's rows: still repeated
     return damp
 
 
@@ -56,10 +62,10 @@ def expected_reuse(damp, so, lo, hi):
 
 
 @functools.lru_cache(maxsize=None)
-def _setup(so, adjoint):
+def _setup(so, adjoint, shape=KC.SHAPE):
     from devito_b200 import Constant, Eq, Function, Grid, Operator, TimeFunction, solve
-    c = KC.iso_case(so, 'scalar')
-    grid = Grid(shape=KC.SHAPE, extent=tuple((n - 1) * h for n, h in zip(KC.SHAPE, KC.SPACING)))
+    c = KC.iso_case(so, 'scalar', shape=shape)
+    grid = Grid(shape=shape, extent=tuple((n - 1) * h for n, h in zip(shape, KC.SPACING)))
     u = TimeFunction(name='v' if adjoint else 'u', grid=grid, time_order=2, space_order=so)
     damp = Function(name='damp', grid=grid, space_order=so)
     m = 1 / Constant(name='vp', value=float(c['param'][1])) ** 2
@@ -70,11 +76,11 @@ def _setup(so, adjoint):
     return op, u, damp, c
 
 
-def _apply(so, adjoint, box, white=False, **kw):
+def _apply(so, adjoint, box, white=False, shape=KC.SHAPE, **kw):
     """(u after time 1..K, damp, lo, hi, case)"""
-    op, u, damp, c = _setup(so, adjoint)
-    lo, hi = box if box is not None else ((0, 0, 0), tuple(n - 1 for n in KC.SHAPE))
-    d = c['damp'] if white else layered_damp(KC.SHAPE, so, lo)
+    op, u, damp, c = _setup(so, adjoint, shape)
+    lo, hi = box if box is not None else ((0, 0, 0), tuple(n - 1 for n in shape))
+    d = c['damp'] if white else layered_damp(shape, so, lo)
     damp.data_with_halo[:] = d
     u.data_with_halo[:] = c['u']
     bounds = dict(x_m=lo[0], x_M=hi[0], y_m=lo[1], y_M=hi[1], z_m=lo[2], z_M=hi[2])
@@ -106,6 +112,21 @@ def test_reuse_matches_float64(so, adjoint, box, lx, monkeypatch):
     assert rel_linf(got, want) < KC.TOL['iso']
     n = expected_reuse(d, so, lo, hi)
     assert 0 < n < hi[0] - lo[0] + 1 - 3                        # the three perturbed planes are streamed
+    assert _lib().b2_last_iso_coef_reuse() == n
+
+
+@pytest.mark.parametrize('adjoint', [False, True], ids=['forward', 'adjoint'])
+def test_reuse_on_several_tiles(adjoint):
+    """kernel_cases.MULTI (13, 44, 300) at so = 8: 3 x 3 yz-tiles of 16 x 128, the last of each partial. The layered
+    damp differs from tile to tile (its y and z ramps), so a CTA that took its pinned A from another tile than its
+    own would change the answer."""
+    got, d, lo, hi, c = _apply(8, adjoint, None, shape=KC.MULTI)
+    want, _ = ref64.iso_forward(c['u'], 8, [ref64.fd2_weights(8, h) for h in KC.SPACING], c['dt'], 1, KC.K,
+                                damp=d, param=c['param'], lo=lo, hi=hi, adjoint=adjoint)
+    assert np.abs(got).max() > 0.5
+    assert rel_linf(got, want) < KC.TOL['iso']
+    n = expected_reuse(d, 8, lo, hi)
+    assert 0 < n < hi[0] - lo[0] + 1 - 3
     assert _lib().b2_last_iso_coef_reuse() == n
 
 

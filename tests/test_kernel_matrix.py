@@ -76,10 +76,10 @@ def _iso_setup(so, param, shape=KC.SHAPE, box=None, interpolation=None):
 
 
 @functools.lru_cache(maxsize=None)
-def _tti_setup(so, arrays):
+def _tti_setup(so, arrays, box=None):
     from devito_b200 import Constant, Eq, Operator, TimeFunction, solve, sqrt
     from devito_b200.seismic.tti import Gzz_centered
-    c = KC.tti_case(so, arrays)
+    c = KC.tti_case(so, arrays, box=box)
     grid = _grid(KC.SHAPE)
     u = TimeFunction(name='u', grid=grid, time_order=2, space_order=so)
     v = TimeFunction(name='v', grid=grid, time_order=2, space_order=so)
@@ -148,14 +148,35 @@ def test_iso_generic(so, param):
     _check_iso(('iso', so, param), 'iso_generic', kernel=1)
 
 
-@pytest.mark.parametrize('lx', [None, '12'])
-@pytest.mark.parametrize('param', PARAMS)
-@pytest.mark.parametrize('so', [4, 8, 12, 16])
-def test_iso_tma(so, param, lx, monkeypatch):
-    """Default selection; B2_ISO_LX=12 cuts the 37 x-planes into four chunks, the last of one plane."""
+ISO_TMA = [pytest.param(so, param, lx, None, id=f'{so}-{param}-{lx}')
+           for so in (4, 8, 12, 16) for param in PARAMS for lx in (None, '12')] + \
+          [pytest.param(so, param, None, box, id=f'{so}-{param}-{box}')
+           for so in (4, 8, 12, 16) for param in PARAMS for box in KC.ZTAIL]
+
+
+@pytest.mark.parametrize('so,param,lx,box', ISO_TMA)
+def test_iso_tma(so, param, lx, box, monkeypatch):
+    """Default selection; B2_ISO_LX=12 cuts the 37 x-planes into four chunks, the last of one plane. The z-tail boxes
+    (kernel_cases.ZTAIL) end every row in a partial float4 group, which the sweep stores point by point."""
     if lx:
         monkeypatch.setenv('B2_ISO_LX', lx)
-    _check_iso(('iso', so, param), f'iso_tma<{so // 2},{PK[param]}>')
+    key = ('iso', so, param) if box is None else ('iso', so, param, KC.SHAPE, KC.ZTAIL[box])
+    _check_iso(key, f'iso_tma<{so // 2},{PK[param]}>')
+
+
+MULTI_TILE = [(8, 'scalar'), (8, 'vp'), (8, 'm'), (4, 'scalar'), (12, 'scalar'), (16, 'scalar')]
+MULTI_GRIDS = {'multi': (KC.MULTI, None), 'multi_tail': (KC.MULTI, KC.MULTI_TAIL), 'exact': (KC.EXACT, None)}
+
+
+@pytest.mark.parametrize('grid', list(MULTI_GRIDS))
+@pytest.mark.parametrize('so,param', MULTI_TILE)
+def test_iso_tma_several_tiles(so, param, grid, monkeypatch):
+    """Grids that every tile configuration cuts into several yz-tiles (kernel_cases.MULTI: >= 2 in y and >= 3 in z,
+    the last of each partial; with a z extent of 298 as well) or into full tiles only (EXACT), with B2_ISO_LX=5
+    (x-chunks of five planes, the last partial on MULTI)."""
+    monkeypatch.setenv('B2_ISO_LX', '5')
+    shape, box = MULTI_GRIDS[grid]
+    _check_iso(('iso', so, param, shape, box), f'iso_tma<{so // 2},{PK[param]}>')
 
 
 @pytest.mark.parametrize('shape,box', [((37, 45, 67), None), (KC.SHAPE, ((0, 0, 3), (36, 44, 67)))],
@@ -169,6 +190,45 @@ def test_iso_sub_box():
     """An interior update box (x_m = 1, y_m = 2, z_m = 4, upper ends inside too): cells outside it keep their
     white noise, and the stencil still reads the halo in x and y."""
     _check_iso(('iso', 8, 'vp', KC.SHAPE, KC.SUBBOX), 'iso_tma<4,vp>')
+
+
+@pytest.mark.parametrize('gate', list(KC.GATE))
+@pytest.mark.parametrize('param', ['scalar', 'vp'])
+@pytest.mark.parametrize('so', [4, 8])
+def test_iso_size_gate(so, param, gate):
+    """Boxes on either side of iso_plan_init's size gate (n[1] >= 8 and n[2] >= 16): n = (8, 8, 16) runs the TMA
+    sweep, (8, 7, 16) and (8, 8, 12) the generic kernel."""
+    expect = f'iso_tma<{so // 2},{PK[param]}>' if gate == 'gate_in' else 'iso_generic'
+    _check_iso(('iso', so, param, KC.SHAPE, KC.GATE[gate]), expect)
+
+
+@pytest.mark.parametrize('param', ['scalar', 'vp'])
+@pytest.mark.parametrize('so', [4, 8, 12, 16])
+def test_iso_one_x_plane(so, param):
+    """x_m == x_M: the march primes 2R planes for a single output plane (z extent 59, a tail of 3)."""
+    _check_iso(('iso', so, param, KC.SHAPE, KC.XPLANE), f'iso_tma<{so // 2},{PK[param]}>')
+
+
+def _tti_fused_name(so, arrays):
+    """the sweep the default selection runs on a layout the fused kernels take"""
+    if arrays:
+        return f'tti_arr_ct2<{so // 2}>'
+    return 'tti_fused<2>' if so == 4 else 'tti_ws<pf1>'
+
+
+@pytest.mark.parametrize('gate', list(KC.GATE))
+@pytest.mark.parametrize('arrays', [False, True], ids=['scalar', 'arrays'])
+@pytest.mark.parametrize('so', [4, 8])
+def test_tti_size_gate(so, arrays, gate):
+    """tti_plan_init's size gate: n = (8, 8, 16) runs the fused sweep, (8, 7, 16) and (8, 8, 12) the two-pass one."""
+    expect = _tti_fused_name(so, arrays) if gate == 'gate_in' else 'tti_two_pass'
+    _check_tti(('tti', so, arrays, KC.GATE[gate]), expect)
+
+
+@pytest.mark.parametrize('arrays', [False, True], ids=['scalar', 'arrays'])
+@pytest.mark.parametrize('so', [4, 8])
+def test_tti_one_x_plane(so, arrays):
+    _check_tti(('tti', so, arrays, KC.XPLANE), _tti_fused_name(so, arrays))
 
 
 @pytest.mark.parametrize('arrays', [False, True], ids=['scalar', 'arrays'])

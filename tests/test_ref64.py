@@ -46,6 +46,10 @@ def _case_mutations(c):
     arrays = (c['kind'] == 'iso' and np.ndim(c['param'][1]) > 0) or \
              (c['kind'] == 'tti' and any(np.ndim(x) for x in c['params'].values()))
     out = ['w_xy', 'w_yz', 'transpose_xy', 'halo_zero', 'tail_y', 'tail_z', 'swap_levels']
+    # a partial last float4 group exists where the TMA sweeps take the layout (z extent of the allocation and z_m
+    # multiples of 4) and the box's z extent is not a multiple of 4
+    if c['shape'][2] % 4 == 0 and c['lo'][2] % 4 == 0 and (c['hi'][2] - c['lo'][2] + 1) % 4:
+        out += ['tail_z_over', 'tail_z_short']
     if arrays:
         out += ['shift_x', 'shift_y', 'shift_z']
         if c['kind'] == 'tti':
@@ -57,13 +61,13 @@ def _distance(a, b):
     return max(rel_linf(x, y) for x, y in zip(a, b))
 
 
-def _check(c, oracle_fields):
+def _check(c, oracle_fields, unclaimed=()):
     tol = KC.TOL[c['kind']]
     ref, _ = KC.reference(c)
     assert np.abs(ref[0]).max() > 0.5
     err = _distance(oracle_fields, ref)
     assert err < tol, f"oracle vs float64: {err:.2e}"
-    for mut in _case_mutations(c):
+    for mut in [m for m in _case_mutations(c) if m not in unclaimed]:
         moved = _distance(KC.reference(c, mut=mut)[0], ref)
         assert moved >= 100 * tol, f"mutation {mut!r} moves the result by only {moved:.2e}"
 
@@ -74,28 +78,113 @@ def test_iso_reference_matches_oracle_and_mutations_show(so, param):
     _check(c, _iso_oracle(c))
 
 
-@pytest.mark.parametrize('name', ['subbox', 'nz67', 'zm3'])
-def test_iso_reference_boxes_and_fallback_shapes(name):
-    """The boxes of the sub-box and fallback GPU cases: an interior box (z_m % 4 == 0), nz % 4 != 0, z_m = 3."""
-    if name == 'subbox':
-        c = KC.iso_case(8, 'vp', box=KC.SUBBOX)
-    elif name == 'nz67':
-        c = KC.iso_case(8, 'vp', shape=(37, 45, 67))
-    else:
-        c = KC.iso_case(8, 'vp', box=((0, 0, 3), (36, 44, 67)))
-    _check(c, _iso_oracle(c))
-    # outside the box nothing moves
+def _outside_the_box_nothing_moves(c):
     lo, hi, so = c['lo'], c['hi'], c['so']
     ref, _ = KC.reference(c)
     keep = np.ones(ref[0].shape[1:], dtype=bool)
     keep[tuple(slice(l + so, h + so + 1) for l, h in zip(lo, hi))] = False
-    assert np.array_equal(ref[0][:, keep], c['u'][:, keep].astype(np.float64))
+    for got, name in zip(ref, ('u', 'v')):
+        assert np.array_equal(got[:, keep], c[name][:, keep].astype(np.float64))
+
+
+@pytest.mark.parametrize('name', ['subbox', 'nz67', 'zm3'] + list(KC.ZTAIL))
+def test_iso_reference_boxes_and_fallback_shapes(name):
+    """The boxes of the sub-box and fallback GPU cases: an interior box (z_m % 4 == 0), nz % 4 != 0, z_m = 3; and the
+    z-tail boxes (z extent 1, 2 or 3 past a multiple of 4), whose mutations include the partial float4 group."""
+    if name == 'subbox':
+        c = KC.iso_case(8, 'vp', box=KC.SUBBOX)
+    elif name == 'nz67':
+        c = KC.iso_case(8, 'vp', shape=(37, 45, 67))
+    elif name == 'zm3':
+        c = KC.iso_case(8, 'vp', box=((0, 0, 3), (36, 44, 67)))
+    else:
+        c = KC.iso_case(8, 'vp', box=KC.ZTAIL[name])
+        assert {'tail_z_over', 'tail_z_short'} <= set(_case_mutations(c))
+    _check(c, _iso_oracle(c))
+    _outside_the_box_nothing_moves(c)
 
 
 @pytest.mark.parametrize('so,arrays', TTI)
 def test_tti_reference_matches_oracle_and_mutations_show(so, arrays):
     c = KC.tti_case(so, arrays)
     _check(c, _tti_oracle(c))
+
+
+@pytest.mark.parametrize('arrays', [False, True], ids=['scalar', 'arrays'])
+@pytest.mark.parametrize('name', list(KC.ZTAIL))
+def test_tti_reference_z_tail_boxes(name, arrays):
+    """TTI on the z-tail boxes: pinned against the oracle, every mutation (the partial float4 group's included) far
+    above the tolerance, and nothing outside the box moves."""
+    c = KC.tti_case(8, arrays, box=KC.ZTAIL[name])
+    assert {'tail_z_over', 'tail_z_short'} <= set(_case_mutations(c))
+    # an interior box reads the halo only with the outer taps in x and y: a halo read as zero moves TTI by ~5e-3
+    # there, below 100x the tolerance; face3 (and the whole-grid cases) claim it
+    _check(c, _tti_oracle(c), unclaimed=('halo_zero',) if name != 'face3' else ())
+    _outside_the_box_nothing_moves(c)
+
+
+@pytest.mark.parametrize('kind', ['iso', 'tti'])
+def test_tail_mutations_change_only_the_tail(kind):
+    """One step on the z-tail boxes: tail_z_over moves exactly the 4 - n2 % 4 points past z_M of every row of the box,
+    tail_z_short exactly its last n2 % 4 points."""
+    for lo, hi in KC.ZTAIL.values():
+        c = KC.iso_case(4, 'vp', box=(lo, hi)) if kind == 'iso' else KC.tti_case(4, False, box=(lo, hi))
+        so, r = c['so'], (hi[2] - lo[2] + 1) % 4
+        fields = ('u',) if kind == 'iso' else ('u', 'v')
+        out = {}
+        for mut in (None, 'tail_z_over', 'tail_z_short'):
+            if kind == 'iso':
+                f = ref64.iso_forward(c['u'], so, KC.weights('iso', so)[0], c['dt'], 1, 1, damp=c['damp'],
+                                      param=c['param'], lo=lo, hi=hi, mut=mut)[:1]
+            else:
+                (w2, w1), _ = KC.weights('tti', so)
+                f = ref64.tti_forward(c['u'], c['v'], so, w2, w1, c['dt'], 1, 1, c['damp'], c['params'], lo=lo,
+                                      hi=hi, mut=mut)[:2]
+            out[mut] = [x[2] for x in f]                                     # the slot written by time 1
+        xy = tuple(slice(l + so, h + so + 1) for l, h in zip(lo[:2], hi[:2]))
+        zover = slice(hi[2] + 1 + so, hi[2] + 1 + so + 4 - r)
+        zshort = slice(hi[2] + 1 + so - r, hi[2] + 1 + so)
+        for i, _ in enumerate(fields):
+            base = out[None][i]
+            for mut, zs in (('tail_z_over', zover), ('tail_z_short', zshort)):
+                moved = out[mut][i] != base
+                assert moved[xy + (zs,)].all(), mut
+                moved[xy + (zs,)] = False
+                assert not moved.any(), mut
+
+
+def test_kernel_case_tilings():
+    """The tilings the kernel_cases comments claim: (y tiles, z tiles), (last y tile, last z tile) per (TY, TZ)."""
+    assert set(KC.TILES.values()) == {(32, 64), (16, 128), (16, 64), (8, 64), (28, 64), (24, 64), (30, 64), (20, 64)}
+    claims = {
+        ('MULTI', (16, 128)): ((3, 3), (12, 44)), ('MULTI', (32, 64)): ((2, 5), (12, 44)),
+        ('MULTI', (16, 64)): ((3, 5), (12, 44)), ('MULTI', (8, 64)): ((6, 5), (4, 44)),
+        ('MULTI_TAIL', (16, 128)): ((3, 3), (12, 42)),
+        ('EXACT', (16, 128)): ((2, 2), (16, 128)), ('EXACT', (32, 64)): ((1, 4), (32, 64)),
+        ('EXACT', (16, 64)): ((2, 4), (16, 64)), ('EXACT', (8, 64)): ((4, 4), (8, 64)),
+    }
+    n = {'MULTI': KC.MULTI, 'MULTI_TAIL': KC.box_extent(KC.MULTI_TAIL), 'EXACT': KC.EXACT}
+    for (name, (ty, tz)), want in claims.items():
+        (ky, ly), (kz, lz) = KC.tiling(n[name][1], ty), KC.tiling(n[name][2], tz)
+        assert ((ky, kz), (ly, lz)) == want, (name, ty, tz)
+    # every iso tile: MULTI cuts >= 2 y tiles and >= 3 z tiles, the last of each partial; EXACT only full tiles
+    for name, (ty, tz) in KC.TILES.items():
+        if name.startswith('iso_tma'):
+            (ky, ly), (kz, lz) = KC.tiling(KC.MULTI[1], ty), KC.tiling(KC.MULTI[2], tz)
+            assert ky >= 2 and kz >= 3 and ly < ty and lz < tz, name
+            assert KC.EXACT[1] % ty == 0 and KC.EXACT[2] % tz == 0, name
+    # the z-tail boxes: a partial last float4 group of 1, 2, 3 and 3 points, z_m % 4 == 0
+    for name, want in (('tail1', 1), ('tail2', 2), ('tail3', 3), ('face3', 3)):
+        lo, hi = KC.ZTAIL[name]
+        assert lo[2] % 4 == 0 and KC.box_extent((lo, hi))[2] % 4 == want, name
+    assert KC.box_extent(KC.ZTAIL['face3']) == (37, 45, 67) and KC.ZTAIL['face3'][0] == (0, 0, 0)
+    lo, hi = KC.XPLANE
+    assert lo[0] == hi[0] and lo[2] % 4 == 0 and KC.box_extent(KC.XPLANE)[2] % 4 == 3
+    # the size gate (n[1] >= 8 and n[2] >= 16): in, out in y, out in z
+    assert [KC.box_extent(KC.GATE[g]) for g in ('gate_in', 'gate_y', 'gate_z')] == [(8, 8, 16), (8, 7, 16), (8, 8, 12)]
+    assert [KC.box_extent(b) for b in KC.TINY.values()] == [(1, 1, 1), (1, 1, 4), (2, 5, 7)]
+    for lo, hi in KC.BOXES.values():
+        assert lo[2] % 4 == 0 and all(0 <= l <= h < n for l, h, n in zip(lo, hi, KC.SHAPE))
 
 
 @pytest.mark.parametrize('param', ['vp', 'm'])

@@ -97,7 +97,7 @@ def _check(key, sweep, box, **kw):
     if box == 'full':
         lo, hi = [0] * nd, [n - 1 for n in c['shape']]
     elif nd == 3:
-        lo, hi = list(KC.SUBBOX[0]), list(KC.SUBBOX[1])
+        lo, hi = list(KC.BOXES[box][0]), list(KC.BOXES[box][1])
     else:
         lo, hi = [1, 4], [c['shape'][0] - 3, c['shape'][1] - 9]
     bounds = {}
@@ -126,12 +126,28 @@ def _variant(so, nd, kernel, adjoint):
     return name + ('+adj' if adjoint else '')
 
 
-@pytest.mark.parametrize('box', ['full', 'sub'])
-@pytest.mark.parametrize('so,arrays,adjoint,nd,kernel', CASES,
-                         ids=[f"so{c[0]}-{'arr' if c[1] else 'scalar'}-{'adj' if c[2] else 'fwd'}-{c[3]}d-k{c[4]}"
-                              for c in CASES])
-def test_sa_kernel(so, arrays, adjoint, nd, kernel, box):
+def _case_id(c):
+    return f"so{c[0]}-{'arr' if c[1] else 'scalar'}-{'adj' if c[2] else 'fwd'}-{c[3]}d-k{c[4]}"
+
+
+# 3-D cases also run the z-tail boxes of kernel_cases.ZTAIL: every row ends in a partial float4 group
+SA_BOXES = [pytest.param(c, box, id=f'{_case_id(c)}-{box}') for c in CASES
+            for box in ['full', 'sub'] + (list(KC.ZTAIL) if c[3] == 3 else [])]
+
+
+@pytest.mark.parametrize('case,box', SA_BOXES)
+def test_sa_kernel(case, box):
+    so, arrays, adjoint, nd, kernel = case
     _check((so, arrays, adjoint, nd), _variant(so, nd, kernel, adjoint), box, kernel=kernel)
+
+
+@pytest.mark.parametrize('box', list(KC.TINY) + ['xplane'])
+@pytest.mark.parametrize('adjoint', [False, True], ids=['fwd', 'adj'])
+@pytest.mark.parametrize('so', [4, 8])
+def test_tma_tiny_boxes(so, adjoint, box):
+    """sa_plan_init has no size gate: boxes of (1, 1, 1), (1, 1, 4) and (2, 5, 7) points at the corners and inside,
+    and one x-plane, run the TMA sweep."""
+    _check((so, True, adjoint, 3), _variant(so, 3, 0, adjoint), box)
 
 
 def test_tma_and_generic_agree():

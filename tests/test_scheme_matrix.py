@@ -194,6 +194,8 @@ def _check(key, expect, **kw):
 
 PARAMS = ['scalar', 'vp', 'm']
 PK = {'scalar': 'scalar', 'vp': 'vp', 'm': 'm'}
+# tail3: a z extent of 59, every row ending in a partial float4 group
+BOXES = dict(full=None, sub=KC.SUBBOX, tail3=KC.ZTAIL['tail3'])
 
 
 def _tma(so, param):
@@ -217,24 +219,24 @@ def test_adjoint_free_surface_and_ot4(scheme, expect):
     _check((scheme, 8, 'vp', None, 0, 'sinc'), expect)
 
 
-@pytest.mark.parametrize('box', ['full', 'sub'])
+@pytest.mark.parametrize('box', list(BOXES))
 @pytest.mark.parametrize('kernel', ['generic', 'tma'])
 def test_gradient(kernel, box):
     """Imaging condition into a grad with halo 1, after each adjoint step and its injection."""
-    key = ('grad', 8, 'vp', KC.SUBBOX if box == 'sub' else None, 0, 'sinc')
+    key = ('grad', 8, 'vp', BOXES[box], 0, 'sinc')
     if kernel == 'generic':
         _check(key, 'iso_generic', kernel=1)
     else:
         _check(key, 'iso_tma<4,vp>')
 
 
-@pytest.mark.parametrize('box', ['full', 'sub'])
+@pytest.mark.parametrize('box', list(BOXES))
 @pytest.mark.parametrize('dmh', [0, 3])
 @pytest.mark.parametrize('kernel', ['generic', 'tma'])
 @pytest.mark.parametrize('param', ['vp', 'm'])
 @pytest.mark.parametrize('so', [4, 8])
 def test_born(so, param, kernel, dmh, box):
-    key = ('born', so, param, KC.SUBBOX if box == 'sub' else None, dmh, 'sinc' if so >= 8 else 'linear')
+    key = ('born', so, param, BOXES[box], dmh, 'sinc' if so >= 8 else 'linear')
     if kernel == 'generic':
         _check(key, 'iso_generic', kernel=1)
     else:
@@ -304,16 +306,17 @@ def _disjoint_source_traces(c, tables):
 
 @pytest.mark.parametrize('rec_fwd', [False, True], ids=['rec_u', 'rec_u_forward'])
 @pytest.mark.parametrize('interpolation', ['linear', 'sinc'])
-@pytest.mark.parametrize('box', ['full', 'sub'])
+@pytest.mark.parametrize('box', list(BOXES))
 @pytest.mark.parametrize('so', [4, 8])
 @pytest.mark.parametrize('dim', [0, 1])
 def test_streamed_loop(dim, so, box, interpolation, rec_fwd, monkeypatch):
     """Chunks of 12 planes (16 at so = 8) cut along x (dim 0) or y (dim 1); the KC points sit on the cuts' faces.
-    With SUBBOX the box starts at x = 1, y = 2: every range, upload and download is offset by that origin.
+    With SUBBOX the box starts at x = 1, y = 2: every range, upload and download is offset by that origin; tail3
+    starts there too and ends every row in a partial float4 group, which every range must keep.
     Against float64 with every KC point; against the resident apply bit for bit with the points whose supports
     overlap switched off (deposits of two points into one cell are atomics in either order, which moves the last
     bit); the traces up to the order of the partial sums."""
-    key = ('plain', so, 'vp', KC.SUBBOX if box == 'sub' else None, 0, interpolation, KC.SHAPE, rec_fwd)
+    key = ('plain', so, 'vp', BOXES[box], 0, interpolation, KC.SHAPE, rec_fwd)
     _, _, c, tables = _setup(*key)
     resident = _apply(key, _tma(so, 'vp'))
     assert not _last_call_streamed()

@@ -4,9 +4,11 @@ non-cubic grid of tests/kernel_cases.py, for the adjoint variant of every TTI sw
 The operators are built with the DSL in the formulation of devito_b200/seismic/tti.py (`AdjointOperator`: the pair
 (p, r) solved for .backward, the receivers injected into both at the level written, srca sampling p + r;
 `JacobianAdjOperator`: the same pair plus Inc(grad, -(usave * p.dt2 + vsave * r.dt2))). Every time slot starts as
-white noise, halo included; usave, vsave and grad (halo KC.GRAD_HALO) are white noise too. Each case asserts from
-`b2_last_sweep_kernel` which sweep variant ran: the scalar so=8 sweep k_tti_ws has no adjoint variant (it would spill
-registers), so its adjoint runs k_tti_fused<4>. Tolerance: rel L-inf 1e-4 for p, r, the traces and grad.
+white noise, halo included; usave, vsave and grad (halo KC.GRAD_HALO) are white noise too. The update box is the
+whole grid, an interior box, or one whose z extent ends in a partial float4 group (kernel_cases.ZTAIL tail1 / tail3:
+the adjoint sweeps' partial loads of p and r). Each case asserts from `b2_last_sweep_kernel` which sweep variant ran:
+the scalar so=8 sweep k_tti_ws has no adjoint variant (it would spill registers), so its adjoint runs
+k_tti_fused<4>. Tolerance: rel L-inf 1e-4 for p, r, the traces and grad.
 """
 import functools
 from types import SimpleNamespace
@@ -29,13 +31,11 @@ def _last_kernel():
 
 
 def adj_case(so, arrays, box=None, seed=0):
-    c = KC.tti_case(so, arrays, seed=seed)
+    c = KC.tti_case(so, arrays, box=box, seed=seed)
     rng = np.random.default_rng(seed + 100 * so + 71)
     c['usave'] = rng.standard_normal((KC.K + 2,) + c['u'].shape[1:]).astype(np.float32)
     c['vsave'] = rng.standard_normal((KC.K + 2,) + c['u'].shape[1:]).astype(np.float32)
     c['grad'] = rng.standard_normal(tuple(n + 2 * KC.GRAD_HALO for n in KC.SHAPE)).astype(np.float32)
-    if box is not None:
-        c['lo'], c['hi'] = tuple(box[0]), tuple(box[1])
     return c
 
 
@@ -145,7 +145,10 @@ VARIANTS = [
 ]
 
 
-@pytest.mark.parametrize('box', ['full', 'sub'])
+BOXES = dict(full=None, sub=KC.SUBBOX, tail1=KC.ZTAIL['tail1'], tail3=KC.ZTAIL['tail3'])
+
+
+@pytest.mark.parametrize('box', list(BOXES))
 @pytest.mark.parametrize('gradient', [False, True], ids=['adjoint', 'gradient'])
 @pytest.mark.parametrize('so,arrays,env,kernel,sweep', VARIANTS,
                          ids=[f"so{v[0]}-{'arr' if v[1] else 'scalar'}-{v[4]}-{'-'.join(v[2].values()) or 'default'}"
@@ -154,4 +157,4 @@ def test_tti_adjoint(so, arrays, env, kernel, sweep, gradient, box, monkeypatch)
     monkeypatch.setenv('B2_TTI_LX', '12')
     for k, val in env.items():
         monkeypatch.setenv(k, val)
-    _check((so, arrays, gradient, KC.SUBBOX if box == 'sub' else None), sweep, kernel=kernel)
+    _check((so, arrays, gradient, BOXES[box]), sweep, kernel=kernel)

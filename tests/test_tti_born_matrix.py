@@ -4,9 +4,11 @@ on the anisotropic, non-cubic grid of tests/kernel_cases.py, for every TTI sweep
 The operator is built with the DSL in the formulation of devito_b200/seismic/tti.py::JacobianOperator (the
 background pair (u0, v0) driven by the sources, the linearised pair (du, dv) by -dm * u0.dt2 / -dm * v0.dt2, the
 receivers sampling du + dv). Every time slot of the four wavefields starts as white noise, halo included; dm is
-white noise with halo 0 or 3. Each case asserts from `b2_last_sweep_kernel` which sweep variant ran for both pairs
-and which path of the Born source term ran ("+born_v4": float4 along z, taken when dm's halo keeps the z rows
-16-byte aligned; "+born_s" otherwise). Tolerance: rel L-inf 1e-4 for u0, v0, du, dv and the traces.
+white noise with halo 0 or 3. The update box is the whole grid, an interior box, or one whose z extent ends in a
+partial float4 group (kernel_cases.ZTAIL tail1 / tail3). Each case asserts from `b2_last_sweep_kernel` which sweep
+variant ran for both pairs and which path of the Born source term ran ("+born_v4": float4 along z, taken when dm's
+halo keeps the z rows 16-byte aligned and the z extent is a multiple of 4; "+born_s" otherwise). Tolerance: rel L-inf
+1e-4 for u0, v0, du, dv and the traces.
 """
 import functools
 from types import SimpleNamespace
@@ -30,14 +32,12 @@ def _last_kernel():
 
 def born_case(so, arrays, box=None, dmh=0, seed=0):
     """A KC TTI case plus the linearised pair (white noise in every slot) and dm with halo `dmh`."""
-    c = KC.tti_case(so, arrays, seed=seed)
+    c = KC.tti_case(so, arrays, box=box, seed=seed)
     rng = np.random.default_rng(seed + 100 * so + 53)
     c['du'] = rng.standard_normal(c['u'].shape).astype(np.float32)
     c['dv'] = rng.standard_normal(c['u'].shape).astype(np.float32)
     c['dm'] = (0.05 * rng.standard_normal(tuple(n + 2 * dmh for n in KC.SHAPE))).astype(np.float32)
     c['dmh'] = dmh
-    if box is not None:
-        c['lo'], c['hi'] = tuple(box[0]), tuple(box[1])
     return c
 
 
@@ -109,7 +109,9 @@ def _apply(key, **kw):
 
 def _check(key, sweep, **kw):
     got = _apply(key, **kw)
-    born = 'v4' if key[3] == 0 else 's'
+    _, _, c, _ = _setup(*key)
+    # float4 along z needs dm's z rows 16-byte aligned (halo 0) and a z extent of whole float4 groups
+    born = 'v4' if key[3] == 0 and (c['hi'][2] - c['lo'][2] + 1) % 4 == 0 else 's'
     assert _last_kernel() == f'{sweep}+born_{born}'
     want = _reference(key)
     assert np.abs(got['du']).max() > 0.1
@@ -140,7 +142,10 @@ VARIANTS = [
 ]
 
 
-@pytest.mark.parametrize('box', ['full', 'sub'])
+BOXES = dict(full=None, sub=KC.SUBBOX, tail1=KC.ZTAIL['tail1'], tail3=KC.ZTAIL['tail3'])
+
+
+@pytest.mark.parametrize('box', list(BOXES))
 @pytest.mark.parametrize('dmh', [0, 3])
 @pytest.mark.parametrize('so,arrays,env,kernel,sweep', VARIANTS,
                          ids=[f"so{v[0]}-{'arr' if v[1] else 'scalar'}-{v[4]}-{'-'.join(v[2].values()) or 'default'}"
@@ -149,4 +154,4 @@ def test_tti_born(so, arrays, env, kernel, sweep, dmh, box, monkeypatch):
     monkeypatch.setenv('B2_TTI_LX', '12')
     for k, val in env.items():
         monkeypatch.setenv(k, val)
-    _check((so, arrays, KC.SUBBOX if box == 'sub' else None, dmh), sweep, kernel=kernel)
+    _check((so, arrays, BOXES[box], dmh), sweep, kernel=kernel)

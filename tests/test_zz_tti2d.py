@@ -626,8 +626,16 @@ def test_adjoint_and_imaging_lookalikes_are_refused(kind):
 # GPU: every 2-D sweep variant against the float64 restatement
 # ---------------------------------------------------------------------------------------------------------------
 MATRIX = ([(so, preset, box, 0) for so in (4, 8) for preset in ('constant-tti', 'layers-tti')
-           for box in ('whole', 'interior')] +
+           for box in ('whole', 'interior', 'tiny1x5', 'tiny3x1')] +
           [(so, preset, 'whole', 1) for so in (4, 8, 12) for preset in ('constant-tti', 'layers-tti')])
+# update boxes (lo, hi) in (x, z) by grid shape; the tiny ones start at z = 4 (z_m % 4 == 0: the single-pass sweep,
+# which has no size gate, takes them)
+BOXES_2D = {
+    'whole': lambda nx, nz: ([0, 0], [nx - 1, nz - 1]),
+    'interior': lambda nx, nz: ([3, 4], [nx - 5, nz - 7]),
+    'tiny1x5': lambda nx, nz: ([3, 4], [3, 8]),
+    'tiny3x1': lambda nx, nz: ([3, 4], [5, 4]),
+}
 
 
 @pytest.mark.gpu
@@ -635,8 +643,9 @@ MATRIX = ([(so, preset, box, 0) for so in (4, 8) for preset in ('constant-tti', 
 def test_kernel_matrix_against_float64(so, preset, box, kernel):
     """Forward, adjoint, Born and gradient through the solver from white-noise fields (every slot, halo included)
     against tests/tti2d_ref.py, below 1e-4. kernel 0 takes the single-pass sweep on a z extent of three segments, the
-    last one partial (1148 + 2 nbl points), and several x chunks, on the whole box and an interior box; kernel 1 (and
-    so=12, which only the two-pass path runs) the two-pass sweep. Each case asserts the variant that ran."""
+    last one partial (1148 + 2 nbl points), and several x chunks, on the whole box, an interior box and boxes of
+    1 x 5 and 3 x 1 points; kernel 1 (and so=12, which only the two-pass path runs) the two-pass sweep. Each case
+    asserts the variant that ran."""
     from devito_b200 import Function, TimeFunction
     from devito_b200.operator import half_node_first_derivative_weights, second_derivative_weights
     from devito_b200.seismic import demo_model, setup_geometry
@@ -647,8 +656,8 @@ def test_kernel_matrix_against_float64(so, preset, box, kernel):
     solver = AnisotropicWaveSolver(model, geometry, space_order=so)
     arrays = preset == 'layers-tti'
     nx, nz = model.grid.shape
-    lim = {} if box == 'whole' else dict(x_m=3, x_M=nx - 5, y_m=4, y_M=nz - 7)
-    lo, hi = ([0, 0], [nx - 1, nz - 1]) if box == 'whole' else ([3, 4], [nx - 5, nz - 7])
+    lo, hi = BOXES_2D[box](nx, nz)
+    lim = {} if box == 'whole' else dict(x_m=lo[0], x_M=hi[0], y_m=lo[1], y_M=hi[1])
     K, dt = 3, float(solver.dt)
     rng = np.random.default_rng(so + 7 * kernel + (box == 'whole'))
     hs = [float(h) for h in model.spacing]
