@@ -378,6 +378,111 @@ static int iso_forward_streamed(const b2_iso_args *a, IsoPlan &p, FieldGeom g, D
 
 }  // namespace b2
 
+namespace b2 {
+
+// ---------------------------------------------------------------------------------------------------------
+// Two-level time loop (k_iso_tma2, DESIGN.md §3.7): each pass advances two time levels for one read of u[t] and
+// u[t-1]. u[t+1] goes to its slot, u[t+2] to one of two scratch slots used in turn (so the pass never writes
+// cells another CTA may still read as u[t-1]); a later pass reads its u[t] from there, and the levels left in
+// scratch are copied into their slots at the end. Only taken when every slot is zero outside the update box and
+// no source reaches outside it, so a level held in scratch sees the halo its slot would.
+// ---------------------------------------------------------------------------------------------------------
+static IsoInj *g_inj = nullptr;
+static int *g_iso2_flag = nullptr;
+
+static int two_level_wanted(const b2_iso_args *a, const IsoPlan &p, const DevArray &u, const SparseDev &src,
+                            const FieldGeom &g, bool streamed, bool host_io, bool &want) {
+    want = false;
+    const char *e = getenv("B2_ISO2");
+    if (e && atoi(e) == 0) return B2_OK;
+    const bool forced = e && atoi(e) == 2;                 // tests: also on small grids
+    if (streamed || host_io || u.owned || a->ndim != 3 || a->halo || !iso2_supported(p)) return B2_OK;
+    if (a->adjoint || a->free_surface || a->ot4 || a->born_U || a->born_dm || a->snap || a->grad || a->errctl)
+        return B2_OK;
+    if (a->time_M - a->time_m + 1 < 2) return B2_OK;
+    if (!forced && u.nbytes < ((size_t)1 << 30)) return B2_OK;
+    if (inject_entry_count(src) > B2_ISO2_MAX_INJ) return B2_OK;
+    if (!g_inj || !g_iso2_flag) {
+        if (g_inj) cudaFree(g_inj);
+        if (g_iso2_flag) cudaFree(g_iso2_flag);
+        g_inj = nullptr;
+        g_iso2_flag = nullptr;
+        if (cudaMalloc(&g_inj, B2_ISO2_MAX_INJ * sizeof(IsoInj)) != cudaSuccess ||
+            cudaMalloc(&g_iso2_flag, sizeof(int)) != cudaSuccess) {
+            cudaGetLastError();                           // no room: one step per sweep
+            if (g_inj) cudaFree(g_inj);
+            g_inj = nullptr;
+            g_iso2_flag = nullptr;
+            return B2_OK;
+        }
+    }
+    B2_CUDA(cudaMemsetAsync(g_iso2_flag, 0, sizeof(int), stream()), B2_ERR_MEMORY);
+    int rc;
+    if ((rc = iso2_halo_nonzero(p, g_iso2_flag))) return rc;
+    if ((rc = launch_inject_entries(src, g, a->time_m, p.param_kind, p.param, 0.f, 0.f, nullptr, g_iso2_flag)))
+        return rc;
+    int flag = 1;
+    B2_CUDA(cudaMemcpyAsync(&flag, g_iso2_flag, sizeof(int), cudaMemcpyDeviceToHost, stream()), B2_ERR_MEMORY);
+    B2_CUDA(cudaStreamSynchronize(stream()), B2_ERR_DEVICE);
+    if (flag != 0) return B2_OK;
+    // two more slot-sized buffers: where they do not fit, the call runs one step per sweep as before
+    return iso2_reserve(p, want);
+}
+
+// `se` (null: no timers): every `stride`-th pass is bracketed like a sampled step of the one-step loop (sweep |
+// injection | interpolation) and counts as two sampled steps in `nsampled`.
+static int iso_forward_two_level(const b2_iso_args *a, const IsoPlan &p, const FieldGeom &g, const SparseDev &src,
+                                 const SparseDev &rec, float scalar_scale, float dt2, StepEvents *se, int stride,
+                                 int &nsampled) {
+    int rc;
+    float *scr[2];
+    if ((rc = iso2_prepare(p, scr))) return rc;
+    const int ninj = inject_entry_count(src);
+    const size_t bytes = p.slot_elems * sizeof(float);
+    auto level = [&](int s) { return p.u + (size_t)s * p.slot_elems; };
+    int time = a->time_m;
+    if ((a->time_M - a->time_m + 1) % 2) {
+        // an odd step count: one ordinary step first
+        const int t0 = slot(time, 3), t1 = slot(time + 1, 3), t2 = slot(time - 1, 3);
+        if ((rc = iso_step(p, t0, t2, t1, 0, p.n[0]))) return rc;
+        if ((rc = launch_inject(src, g, level(t1), nullptr, time, p.param_kind, p.param, scalar_scale, dt2))) return rc;
+        if ((rc = launch_interp(rec, g, level(a->rec_toff ? t1 : t0), nullptr, time))) return rc;
+        ++time;
+    }
+    int cur = -1;                  // scratch slot that holds u[time] (-1: its own slot)
+    // the injection entries of a pass's first step are written after the previous pass (before the first one here)
+    if (ninj && (rc = launch_inject_entries(src, g, time, p.param_kind, p.param, scalar_scale, dt2, g_inj, nullptr)))
+        return rc;
+    for (int pass = 0; time + 1 <= a->time_M; time += 2, ++pass) {
+        const int t0 = slot(time, 3), t1 = slot(time + 1, 3), tm = slot(time - 1, 3);
+        const int w = cur == 0 ? 1 : 0;
+        const bool events = se && pass % stride == 0 && se->used + 4 <= 16384;
+        if (events) { se->next(); nsampled += 2; }
+        if ((rc = iso_step2(p, t0, cur, tm, t1, w, g_inj, ninj))) return rc;
+        if (events) se->next();
+        // step time+1's injection into u[time+2], the next pass's entries, then the two receiver rows
+        if ((rc = launch_inject(src, g, scr[w], nullptr, time + 1, p.param_kind, p.param, scalar_scale, dt2))) return rc;
+        if (ninj && time + 3 <= a->time_M &&
+            (rc = launch_inject_entries(src, g, time + 2, p.param_kind, p.param, scalar_scale, dt2, g_inj, nullptr)))
+            return rc;
+        if (events) se->next();
+        const float *u0 = cur < 0 ? level(t0) : scr[cur];
+        if ((rc = launch_interp(rec, g, a->rec_toff ? level(t1) : u0, nullptr, time))) return rc;
+        if ((rc = launch_interp(rec, g, a->rec_toff ? scr[w] : level(t1), nullptr, time + 1))) return rc;
+        if (events) se->next();
+        // u[time] is dead unless it is the last pass's u[t]: copied back below
+        if (time + 3 > a->time_M && cur >= 0)
+            B2_CUDA(cudaMemcpyAsync(level(t0), scr[cur], bytes, cudaMemcpyDeviceToDevice, stream()), B2_ERR_MEMORY);
+        cur = w;
+    }
+    // u[time_M + 1] sits in scratch
+    B2_CUDA(cudaMemcpyAsync(level(slot(a->time_M + 1, 3)), scr[cur], bytes, cudaMemcpyDeviceToDevice, stream()),
+            B2_ERR_MEMORY);
+    return B2_OK;
+}
+
+}  // namespace b2
+
 extern "C" void b2_last_call_profile(double out[5]) {
     for (int i = 0; i < 5; ++i) out[i] = b2::g_last_profile[i];
 }
@@ -618,7 +723,12 @@ static int iso_forward_body(const b2_iso_args *a, Staging &st, SnapStreamer &str
         u->written = false;                       // the loop has brought u home
         g_last_profile[4] = 1.0;
     }
-    if (!streamed)
+    bool two_level = false;
+    if (!streamed && (rc = two_level_wanted(a, p, *u, src, g, streamed, host_io, two_level))) return rc;
+    if (two_level && (rc = iso_forward_two_level(a, p, g, src, rec, scalar_scale, dt2, timing ? &se : nullptr,
+                                                 std::max(sample_stride / 2, 1), nsampled)))
+        return rc;
+    if (!streamed && !two_level)
     for (int time = a->adjoint ? a->time_M : a->time_m; a->adjoint ? time >= a->time_m : time <= a->time_M;
          time += dir) {
         const int t0 = slot(time, T);

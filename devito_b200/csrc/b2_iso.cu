@@ -8,7 +8,7 @@
 //
 // with w_d[k] = finite_diff_weights(2, ...)/h_d^2 (devito/finite_differences/tools.py:231-236).
 //
-// Two kernels:
+// Kernels:
 //   k_iso_generic : one thread per point, any radius <= 8, 2-D or 3-D, any alignment.
 //   k_iso_tma     : 2.5-D sweep. A CTA owns a (TY x TZ) yz-tile and marches along x.
 //                   A producer warp streams haloed yz-planes of u[t] (and the matching tiles
@@ -19,6 +19,7 @@
 //                   u[t+1] with 16-byte coalesced stores. No tensor cores: the update is
 //                   HBM-bandwidth bound (16 B/point; 12 B with a scalar vp on the x-planes whose
 //                   coefficient A repeats the pinned plane's, see IsoTK::reuse).
+//   k_iso_tma2    : the same sweep advancing two time levels per pass (so=8, scalar vp; DESIGN.md §3.7).
 #include "b2_iso.cuh"
 #include "b2_iso_point.cuh"
 #include "b2_ptx.cuh"
@@ -414,6 +415,294 @@ k_iso_tma(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUt
     }
 }
 
+
+// ------------------------------------------------------------------------------------------
+// Two-level TMA sweep (so = 8, scalar parameter): one pass over HBM advances u[t] to u[t+1] AND u[t+2]
+// ------------------------------------------------------------------------------------------
+// A CTA owns a TY x TZ output tile and marches along x. Level 1 computes u[t+1] on the tile grown by R in y
+// and z (24 x 72, the cells level 2's y/z taps reach), level 2 computes u[t+2] on the tile, R planes behind.
+//   u[t]    : haloed 32 x 80 planes, TMA ring of Q = 2R+1 stages; every level-1 thread keeps its own
+//             column's x-history in registers (q1), as k_iso_tma does
+//   u[t-1]  : 24 x 72 tiles with the level-1 plane (ring of R+1 stages, like k_iso_tma's tile ring)
+//   A       : 24 x 72 tiles likewise, or the pinned tile on the planes whose A repeats (IsoTK::reuse)
+//   u[t+1]  : each level-1 plane is also written to a ring of R+2 shared planes (level 2's y/z taps); the
+//             256 tile threads keep their own column's level-1 x-history in registers (q2), and level 2's
+//             u[t-1] (= u[t]) is already in q1
+// Level-1 values outside the update box are the halo's, which the caller guarantees to be zero (iso2_halo_zero).
+// u[t+1] goes to its own slot, u[t+2] to a scratch slot: the pass never writes a cell another CTA may still read.
+// Source injection of step t into u[t+1] is applied to the level-1 values (IsoInj entries of this CTA's region),
+// so that level 2 reads u[t+1] exactly as the one-step loop leaves it; only the owning CTA stores a cell.
+constexpr int I2R = 4, I2TY = 16, I2TZ4 = 16;
+struct Iso2Cfg {
+    static constexpr int R = I2R, RZ = 4, TY = I2TY, TZ4 = I2TZ4, TZ = 4 * TZ4;
+    static constexpr int BY = TY + 4 * R, BZ = TZ + 4 * RZ;        // u[t] box: 32 x 80
+    static constexpr int EY = TY + 2 * R, EZ = TZ + 2 * RZ;        // level-1 region: 24 x 72
+    static constexpr int EZ4 = EZ / 4;
+    static constexpr int Q = 2 * R + 1, NS = R + 1, NL = R + 2;
+    static constexpr int PLANE = align32f(BY * BZ);
+    static constexpr int EPL = EY * EZ;
+    static constexpr int NTH1 = EY * EZ4;                          // level-1 threads (432)
+    static constexpr int NCW = (NTH1 + 31) / 32;                   // consumer warps (14)
+    static constexpr int NT = 32 * NCW + 32;
+    static constexpr size_t SMEM = (size_t)(Q * PLANE + NL * EPL + 2 * NS * EPL + EPL) * 4 + 2 * Q * 8 + 8 +
+                                   NS * 4 + B2_ISO2_MAX_INJ * sizeof(IsoInj) + 16 + 128;
+    static_assert(SMEM <= 227 * 1024, "k_iso_tma2: shared memory over the 227 KB of one SM");
+};
+
+struct Iso2K {
+    float *__restrict__ u1;       // base of u[t+1]'s slot
+    float *__restrict__ u2;       // base of u[t+2]'s scratch slot
+    const float *__restrict__ A;  // coefficient table (level 2 reads the planes whose A is not pinned)
+    long long sx, sy;
+    int nx, ny, nz;
+    int ox, oy, oz;
+    int lx, ntz, nty;
+    int slot0, slotm;             // tensor-map time coordinates of u[t] and u[t-1]
+    float m_dt2;
+    float wx[I2R + 1], wy[I2R + 1], wz[I2R + 1];
+    const unsigned char *reuse;
+    int pin_x;
+    const IsoInj *inj;
+    int ninj;
+};
+
+// acc = centre + z, y, x taps in the order k_iso_tma sums them (bit-identical results)
+__device__ __forceinline__ float4 iso2_lap(const float *cp, int bz, float4 c, const float4 *q, int pc, float wc,
+                                          const float *wx, const float *wy, const float *wz) {
+    constexpr int R = I2R, RZ = 4, Q = 2 * R + 1;
+    float zr[4 + 2 * RZ];
+    const float4 l = b2ptx::lds128(cp - RZ);
+    const float4 r = b2ptx::lds128(cp + 4);
+    zr[0] = l.x; zr[1] = l.y; zr[2] = l.z; zr[3] = l.w;
+    zr[RZ + 0] = c.x; zr[RZ + 1] = c.y; zr[RZ + 2] = c.z; zr[RZ + 3] = c.w;
+    zr[RZ + 4] = r.x; zr[RZ + 5] = r.y; zr[RZ + 6] = r.z; zr[RZ + 7] = r.w;
+    float4 acc = make_float4(wc * c.x, wc * c.y, wc * c.z, wc * c.w);
+#pragma unroll
+    for (int i = 1; i <= R; ++i) {
+        acc.x = fmaf(wz[i], zr[RZ + 0 - i] + zr[RZ + 0 + i], acc.x);
+        acc.y = fmaf(wz[i], zr[RZ + 1 - i] + zr[RZ + 1 + i], acc.y);
+        acc.z = fmaf(wz[i], zr[RZ + 2 - i] + zr[RZ + 2 + i], acc.z);
+        acc.w = fmaf(wz[i], zr[RZ + 3 - i] + zr[RZ + 3 + i], acc.w);
+    }
+#pragma unroll
+    for (int i = 1; i <= R; ++i) f4fma(acc, wy[i], f4add(b2ptx::lds128(cp - i * bz), b2ptx::lds128(cp + i * bz)));
+#pragma unroll
+    for (int i = 1; i <= R; ++i) f4fma(acc, wx[i], f4add(q[(pc - i + Q) % Q], q[(pc + i) % Q]));
+    return acc;
+}
+
+__device__ __forceinline__ float4 iso2_update(float4 c, float4 pv, float4 ca, float4 acc, float m_dt2) {
+    const float4 d = f4sub(c, pv);
+    return make_float4(fmaf(ca.x, fmaf(m_dt2, d.x, acc.x), c.x), fmaf(ca.y, fmaf(m_dt2, d.y, acc.y), c.y),
+                       fmaf(ca.z, fmaf(m_dt2, d.z, acc.z), c.z), fmaf(ca.w, fmaf(m_dt2, d.w, acc.w), c.w));
+}
+
+__device__ __forceinline__ void iso2_store(float *dst, float4 o, int zcnt) {
+    if (zcnt == 4) {
+        *reinterpret_cast<float4 *>(dst) = o;
+    } else if (zcnt > 0) {
+        dst[0] = o.x;
+        if (zcnt > 1) dst[1] = o.y;
+        if (zcnt > 2) dst[2] = o.z;
+    }
+}
+
+__global__ void __launch_bounds__(Iso2Cfg::NT, 1)
+k_iso_tma2(const __grid_constant__ CUtensorMap tm_uh, const __grid_constant__ CUtensorMap tm_uc,
+           const __grid_constant__ CUtensorMap tm_a, const Iso2K k) {
+    using C = Iso2Cfg;
+    constexpr int R = C::R, RZ = C::RZ, TY = C::TY, TZ = C::TZ, BZ = C::BZ, EZ = C::EZ, EZ4 = C::EZ4;
+    constexpr int Q = C::Q, NS = C::NS, NL = C::NL, PLANE = C::PLANE, EPL = C::EPL, NCW = C::NCW;
+
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    float *s_u = reinterpret_cast<float *>(smem_raw);
+    float *s_l1 = s_u + Q * PLANE;
+    float *s_prev = s_l1 + NL * EPL;
+    float *s_a = s_prev + NS * EPL;
+    float *s_pin = s_a + NS * EPL;
+    uint64_t *full = reinterpret_cast<uint64_t *>(s_pin + EPL);
+    uint64_t *empty = full + Q;
+    uint64_t *pinbar = empty + Q;
+    int *s_reused = reinterpret_cast<int *>(pinbar + 1);
+    IsoInj *s_inj = reinterpret_cast<IsoInj *>(s_reused + NS + (NS & 1));
+    int *s_ninj = reinterpret_cast<int *>(s_inj + B2_ISO2_MAX_INJ);
+    const bool pin = k.reuse != nullptr;
+
+    int b = blockIdx.x;
+    const int iz = b % k.ntz;
+    b /= k.ntz;
+    const int iy = b % k.nty;
+    const int ix = b / k.nty;
+    const int z0 = iz * TZ, y0 = iy * TY;
+    const int xs = ix * k.lx;
+    const int xe = min(xs + k.lx, k.nx);
+    // plane j of the march is x = xs - 2R + j; iteration j computes level 1 on x - R = xs - 3R + j and
+    // level 2 on xs - 4R + j
+    const int NP = (xe - xs) + 4 * R;
+
+    const int tid = threadIdx.x;
+    const int warp = tid >> 5, lane = tid & 31;
+
+    if (tid == 0) {
+        for (int i = 0; i < Q; ++i) {
+            b2ptx::mbar_init(&full[i], 1);
+            b2ptx::mbar_init(&empty[i], NCW);
+        }
+        b2ptx::mbar_init(pinbar, 1);
+        b2ptx::fence_mbar_init();
+        // the injection entries that land in this CTA's level-1 region
+        int n = 0;
+        for (int i = 0; i < k.ninj; ++i) {
+            const IsoInj e = k.inj[i];
+            if (e.x >= xs - R && e.x < xe + R && e.y >= y0 - R && e.y < y0 + TY + R && e.z >= z0 - RZ &&
+                e.z < z0 + TZ + RZ)
+                s_inj[n++] = e;
+        }
+        *s_ninj = n;
+    }
+    __syncthreads();
+
+    if (warp == NCW) {
+        if (lane == 0) {
+            b2ptx::tma_prefetch_desc(&tm_uh);
+            b2ptx::tma_prefetch_desc(&tm_uc);
+            b2ptx::tma_prefetch_desc(&tm_a);
+            if (pin) {
+                b2ptx::mbar_arrive_expect_tx(pinbar, EPL * 4);
+                b2ptx::tma_load_3d(s_pin, &tm_a, pinbar, k.oz + z0 - RZ, k.oy + y0 - R, k.pin_x);
+            }
+            int slot = 0, round = 0, ss = 0;
+            for (int j = 0; j < NP; ++j) {
+                if (round > 0) b2ptx::mbar_wait(&empty[slot], (round - 1) & 1);
+                const int x1 = xs - 3 * R + j;                     // level-1 plane of iteration j
+                bool reused = false;
+                uint32_t bytes = C::BY * BZ * 4;
+                if (j >= 2 * R) {
+                    reused = pin && __ldg(k.reuse + k.ox + x1) != 0;
+                    s_reused[ss] = reused;
+                    bytes += EPL * 4 * (reused ? 1 : 2);
+                }
+                b2ptx::mbar_arrive_expect_tx(&full[slot], bytes);
+                b2ptx::tma_load_4d(s_u + slot * PLANE, &tm_uh, &full[slot], k.oz + z0 - 2 * RZ, k.oy + y0 - 2 * R,
+                                   k.ox + xs - 2 * R + j, k.slot0);
+                if (j >= 2 * R) {
+                    b2ptx::tma_load_4d(s_prev + ss * EPL, &tm_uc, &full[slot], k.oz + z0 - RZ, k.oy + y0 - R,
+                                       k.ox + x1, k.slotm);
+                    if (!reused)
+                        b2ptx::tma_load_3d(s_a + ss * EPL, &tm_a, &full[slot], k.oz + z0 - RZ, k.oy + y0 - R,
+                                           k.ox + x1);
+                    if (++ss == NS) ss = 0;
+                }
+                if (++slot == Q) { slot = 0; ++round; }
+            }
+        }
+        return;
+    }
+
+    // ---------------- consumers: thread -> (ey, ec) of the level-1 region ----------------
+    // threads [0, 256): the output tile (level 1 and level 2, whole warps); then the y-halo rows, then the two
+    // z-halo columns; threads >= NTH1 only take part in the barriers
+    int ey, ec;
+    if (tid < TY * C::TZ4) {
+        ey = R + tid / C::TZ4; ec = 1 + tid % C::TZ4;
+    } else if (tid < TY * C::TZ4 + 2 * R * EZ4) {
+        const int h = tid - TY * C::TZ4, r = h / EZ4;
+        ey = r < R ? r : r + TY; ec = h % EZ4;
+    } else {
+        const int h = tid - TY * C::TZ4 - 2 * R * EZ4;
+        ey = R + h / 2; ec = (h & 1) ? EZ4 - 1 : 0;
+    }
+    const bool active = tid < C::NTH1;
+    const bool inner = tid < TY * C::TZ4;
+    if (!active) { ey = 0; ec = 0; }
+    const int gy = y0 - R + ey, gz = z0 - RZ + 4 * ec;             // relative to the iteration origin
+    const bool yin = gy >= 0 && gy < k.ny;
+    // components of my float4 inside the update box along z (level-1 values outside the box are the halo's: 0)
+    const bool zin0 = yin && gz + 0 >= 0 && gz + 0 < k.nz, zin1 = yin && gz + 1 >= 0 && gz + 1 < k.nz;
+    const bool zin2 = yin && gz + 2 >= 0 && gz + 2 < k.nz, zin3 = yin && gz + 3 >= 0 && gz + 3 < k.nz;
+    const int zcnt = inner && yin ? min(max(k.nz - gz, 0), 4) : 0;
+    const float *my_col = s_u + (ey + R) * BZ + RZ + 4 * ec;
+    const int eoff = ey * EZ + 4 * ec;
+    const long long rowoff = (long long)(k.oy + gy) * k.sy + (k.oz + gz);
+    const int ninj = *s_ninj;
+
+    float4 q1[Q], q2[Q];
+#pragma unroll
+    for (int i = 0; i < Q; ++i) { q1[i] = make_float4(0.f, 0.f, 0.f, 0.f); q2[i] = q1[i]; }
+
+    const float wc = k.wx[0] + k.wy[0] + k.wz[0];
+    if (pin) b2ptx::mbar_wait(pinbar, 0);
+    uint32_t par = 0;
+    int ss = 0;                     // tile-ring stage of the level-1 plane
+    int l1w = 0, l1r = R % NL;      // s_l1 stage of level-1 plane j - 2R (written) / j - 3R (read by level 2)
+    unsigned pinned = 0;            // bit i: the level-1 plane of iteration j - i took A from the pinned tile
+
+    for (int jb = 0; jb < NP; jb += Q) {
+#pragma unroll
+        for (int p = 0; p < Q; ++p) {
+            const int j = jb + p;
+            if (j >= NP) break;
+            b2ptx::mbar_wait(&full[p], par);
+            q1[p] = b2ptx::lds128(my_col + p * PLANE);
+
+            if (j >= 2 * R) {
+                const int x1 = xs - 3 * R + j;
+                const int pc = (p - R + Q) % Q;
+                const float4 c = q1[pc];
+                const float4 acc = iso2_lap(my_col + pc * PLANE, BZ, c, q1, pc, wc, k.wx, k.wy, k.wz);
+                const float4 pv = b2ptx::lds128(s_prev + ss * EPL + eoff);
+                const int reused = s_reused[ss];
+                pinned = (pinned << 1) | (unsigned)reused;
+                const float4 ca = b2ptx::lds128((reused ? s_pin : s_a + ss * EPL) + eoff);
+                float4 o = iso2_update(c, pv, ca, acc, k.m_dt2);
+                const bool xin = x1 >= 0 && x1 < k.nx;
+                o.x = xin && zin0 ? o.x : 0.f;
+                o.y = xin && zin1 ? o.y : 0.f;
+                o.z = xin && zin2 ? o.z : 0.f;
+                o.w = xin && zin3 ? o.w : 0.f;
+                for (int i = 0; i < ninj; ++i) {
+                    const IsoInj e = s_inj[i];
+                    if (e.x == x1 && e.y == gy && e.z >= gz && e.z < gz + 4) {
+                        const int cz = e.z - gz;
+                        if (cz == 0) o.x += e.v;
+                        else if (cz == 1) o.y += e.v;
+                        else if (cz == 2) o.z += e.v;
+                        else o.w += e.v;
+                    }
+                }
+                if (active) *reinterpret_cast<float4 *>(s_l1 + l1w * EPL + eoff) = o;
+                q2[p] = o;
+                if (x1 >= xs && x1 < xe) iso2_store(k.u1 + (long long)(k.ox + x1) * k.sx + rowoff, o, zcnt);
+                if (++ss == NS) ss = 0;
+                if (++l1w == NL) l1w = 0;
+            }
+            if (j >= R) {
+                __syncwarp();
+                if (lane == 0) b2ptx::mbar_arrive(&empty[(p - R + Q) % Q]);
+            }
+            if (j >= 4 * R) {
+                // level-1 plane x2 (written R iterations ago) is complete in s_l1; the barrier also orders this
+                // iteration's level-1 store after every read of its stage (two iterations ago)
+                asm volatile("bar.sync 1, %0;" ::"n"(NCW * 32) : "memory");
+                if (zcnt > 0) {
+                    const int x2 = xs - 4 * R + j;
+                    const int pc2 = (p - R + Q) % Q;
+                    const float4 c = q2[pc2];
+                    const float4 acc = iso2_lap(s_l1 + l1r * EPL + eoff, EZ, c, q2, pc2, wc, k.wx, k.wy, k.wz);
+                    float4 ca;
+                    if ((pinned >> R) & 1u)
+                        ca = b2ptx::lds128(s_pin + eoff);
+                    else
+                        ca = __ldg(reinterpret_cast<const float4 *>(k.A + (long long)(k.ox + x2) * k.sx + rowoff));
+                    const float4 o = iso2_update(c, q1[(p + 1) % Q], ca, acc, k.m_dt2);
+                    iso2_store(k.u2 + (long long)(k.ox + x2) * k.sx + rowoff, o, zcnt);
+                }
+                if (++l1r == NL) l1r = 0;
+            }
+        }
+        par ^= 1;
+    }
+}
 
 // A = 1/(m/dt^2 + damp/dt), B = m/dt^2 * A on the full allocated array (halo included; halo
 // values are never used by the stencil)
@@ -859,6 +1148,137 @@ int iso_step_fused(const IsoPlan &p, int slot0, int slotm, int slot1, const IsoF
         case 8: return launch_tma_pk<8>(p, slot0, slotm, slot1, 0, p.n[0], &f);
     }
     return B2_ERR_INVALID;
+}
+
+bool iso2_supported(const IsoPlan &p) {
+    return p.use_tma && !p.ot4 && p.tsize == 3 && p.param_kind == B2_PARAM_SCALAR && p.radius[0] == I2R &&
+           p.radius[1] == I2R && p.radius[2] == I2R && p.n[0] >= 1;
+}
+
+// scratch slots of the two-level pass, cached like g_coef; g_s2_box: the array extents and update box they are zero
+// outside of
+static float *g_s2 = nullptr;
+static size_t g_s2_elems = 0;
+static int g_s2_box[9] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};
+static CUtensorMap g_s2_tm_uh, g_s2_tm_uh_s, g_s2_tm_uc, g_s2_tm_a;
+
+int iso2_reserve(const IsoPlan &p, bool &ok) {
+    ok = true;
+    if (g_s2_elems == p.slot_elems) return B2_OK;
+    if (g_s2) cudaFree(g_s2);
+    g_s2 = nullptr;
+    g_s2_elems = 0;
+    if (cudaMalloc(&g_s2, 2 * p.slot_elems * sizeof(float)) != cudaSuccess) {
+        cudaGetLastError();                  // an allocation failure is not sticky: clear it, run one step per sweep
+        g_s2 = nullptr;
+        ok = false;
+        return B2_OK;
+    }
+    g_s2_elems = p.slot_elems;
+    g_s2_box[0] = -1;
+    return B2_OK;
+}
+
+int iso2_prepare(const IsoPlan &p, float *scratch[2]) {
+    using C = Iso2Cfg;
+    if (g_s2_elems != p.slot_elems) { set_error("iso2_prepare: scratch not reserved"); return B2_ERR_INVALID; }
+    const int box[9] = {p.a[0], p.a[1], p.a[2], p.o[0], p.o[1], p.o[2], p.n[0], p.n[1], p.n[2]};
+    if (memcmp(box, g_s2_box, sizeof(box)) != 0) {
+        // the pass writes only the update box: everything else stays the zero halo the slots hold
+        B2_CUDA(cudaMemsetAsync(g_s2, 0, 2 * p.slot_elems * sizeof(float), stream()), B2_ERR_MEMORY);
+        memcpy(g_s2_box, box, sizeof(box));
+    }
+    const int dims4[4] = {p.a[2], p.a[1], p.a[0], p.tsize};
+    const int dims4s[4] = {p.a[2], p.a[1], p.a[0], 2};
+    const int dims3[3] = {p.a[2], p.a[1], p.a[0]};
+    int rc;
+    if ((rc = make_tmap(&g_s2_tm_uh, p.u, 4, dims4, C::BZ, C::BY))) return rc;
+    if ((rc = make_tmap(&g_s2_tm_uh_s, g_s2, 4, dims4s, C::BZ, C::BY))) return rc;
+    if ((rc = make_tmap(&g_s2_tm_uc, p.u, 4, dims4, C::EZ, C::EY))) return rc;
+    if ((rc = make_tmap(&g_s2_tm_a, p.coefA, 3, dims3, C::EZ, C::EY))) return rc;
+    scratch[0] = g_s2;
+    scratch[1] = g_s2 + p.slot_elems;
+    return B2_OK;
+}
+
+// one warp per (slot, x, y) row: rows outside the box in x or y are checked whole, the others outside [o2, o2 + n2)
+__global__ void __launch_bounds__(256)
+k_iso2_halo_nonzero(const float *__restrict__ u, size_t slot_elems, long long sx, int a0, int a1, int a2, int o0,
+                    int o1, int o2, int n0, int n1, int n2, int *flag) {
+    const long long rows = 3LL * a0 * a1;
+    const int lane = threadIdx.x & 31;
+    bool nz = false;
+    for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < rows;
+         r += (gridDim.x * (long long)blockDim.x) >> 5) {
+        const int s = (int)(r / ((long long)a0 * a1));
+        const int xy = (int)(r % ((long long)a0 * a1));
+        const int x = xy / a1, y = xy % a1;
+        const float *row = u + s * slot_elems + (size_t)x * sx + (size_t)y * a2;
+        const bool inside = x >= o0 && x < o0 + n0 && y >= o1 && y < o1 + n1;
+        for (int z = lane; z < a2; z += 32) {
+            if (inside && z >= o2 && z < o2 + n2) continue;
+            nz |= row[z] != 0.f;
+        }
+    }
+    if (__any_sync(0xffffffffu, nz) && lane == 0) atomicOr(flag, 1);
+}
+
+int iso2_halo_nonzero(const IsoPlan &p, int *flag) {
+    B2_SM_COUNT(sms);
+    k_iso2_halo_nonzero<<<sms * 8, 256, 0, stream()>>>(p.u, p.slot_elems, p.sx, p.a[0], p.a[1], p.a[2], p.o[0],
+                                                        p.o[1], p.o[2], p.n[0], p.n[1], p.n[2], flag);
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
+}
+
+int iso_step2(const IsoPlan &p, int slot0, int src_scratch, int slotm, int slot1, int dst_scratch, const IsoInj *inj,
+              int ninj) {
+    using C = Iso2Cfg;
+    static bool attr_set = false;
+    if (!attr_set) {
+        B2_CUDA(cudaFuncSetAttribute(k_iso_tma2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM),
+                B2_ERR_LAUNCH);
+        attr_set = true;
+    }
+    Iso2K k;
+    k.u1 = p.u + (size_t)slot1 * p.slot_elems;
+    k.u2 = g_s2 + (size_t)dst_scratch * p.slot_elems;
+    k.A = p.coefA;
+    k.sx = p.sx;
+    k.sy = p.sy;
+    k.nx = p.n[0]; k.ny = p.n[1]; k.nz = p.n[2];
+    k.ox = p.o[0]; k.oy = p.o[1]; k.oz = p.o[2];
+    k.ntz = (p.n[2] + C::TZ - 1) / C::TZ;
+    k.nty = (p.n[1] + C::TY - 1) / C::TY;
+    int lx = env_int("B2_ISO_LX", 0);
+    if (lx <= 0) {
+        B2_SM_COUNT(sms);
+        lx = choose_chunk_len(sms, k.ntz * k.nty, p.n[0], 4 * C::R, 32);
+    }
+    k.lx = std::min(lx, p.n[0]);
+    const int ntx = (p.n[0] + k.lx - 1) / k.lx;
+    k.slot0 = src_scratch < 0 ? slot0 : src_scratch;
+    k.slotm = slotm;
+    k.m_dt2 = (1.0f / (p.vp * p.vp)) * (1.0f / (p.dt * p.dt));
+    for (int i = 0; i <= C::R; ++i) {
+        k.wx[i] = p.w[0][i];
+        k.wy[i] = p.w[1][i];
+        k.wz[i] = p.w[2][i];
+    }
+    k.reuse = p.coef_reuse;
+    k.pin_x = p.o[0] + p.n[0] / 2;
+    k.inj = inj;
+    k.ninj = ninj;
+    const unsigned grid = (unsigned)(k.ntz * k.nty * ntx);
+    timing_begin();
+    k_iso_tma2<<<grid, C::NT, C::SMEM, stream()>>>(src_scratch < 0 ? g_s2_tm_uh : g_s2_tm_uh_s, g_s2_tm_uc,
+                                                   g_s2_tm_a, k);
+    note_sweep_kernel("iso_tma2<%d,scalar>", C::R);
+    timing_end();
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
 }
 
 int iso_step(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount) {

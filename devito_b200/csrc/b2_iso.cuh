@@ -70,6 +70,29 @@ int iso_step_fused(const IsoPlan &p, int slot0, int slotm, int slot1, const IsoF
 // with mirrored vertical taps and clear the surface row (b2_iso_args.free_surface).
 int iso_fs_fix(const IsoPlan &p, int slot0, int slotm, int slot1, int xlo, int xcount);
 
+// ---- two-level pass (so = 8, scalar parameter): u[t] -> u[t+1] (its slot) and u[t+2] (a scratch slot) ----
+// One source-injection entry of a step: cell (x, y, z) relative to the iteration origin, value added.
+struct IsoInj {
+    int x, y, z;
+    float v;
+};
+constexpr int B2_ISO2_MAX_INJ = 64;                 // entries the pass takes; more: the one-step loop
+// The plan qualifies for the pass (radius 4 on every axis, scalar parameter, TMA layout, 3 slots).
+bool iso2_supported(const IsoPlan &p);
+// Allocates the two scratch slots (u's slot layout, 2 x slot_elems floats, cached across calls); ok = false, with no
+// error, when the device has no room for them.
+int iso2_reserve(const IsoPlan &p, bool &ok);
+// After iso2_reserve: zeroes the scratch slots outside the update box when the layout changed, encodes their
+// tensor maps; `scratch[k]` is slot k's base.
+int iso2_prepare(const IsoPlan &p, float *scratch[2]);
+// flag |= 1 when any of u's 3 slots holds a non-zero outside the update box (device; the caller reads it back)
+int iso2_halo_nonzero(const IsoPlan &p, int *flag);
+// One pass: level 1 reads u[t] from slot `slot0` (src_scratch < 0) or scratch `src_scratch`, u[t-1] from slot
+// `slotm`, writes u[t+1] to slot `slot1` with the entries `inj` (device, `ninj` of them) added, and u[t+2] to
+// scratch `dst_scratch`.
+int iso_step2(const IsoPlan &p, int slot0, int src_scratch, int slotm, int slot1, int dst_scratch, const IsoInj *inj,
+              int ninj);
+
 // Snapshot: copy the iteration box of time slot `slot` into one snapshot (own strides; (d0,d1,d2) = index
 // of the first iterated point in the snapshot array)
 int iso_snapshot(const IsoPlan &p, int slot, float *snap, long long dsx, long long dsy, int d0, int d1, int d2);

@@ -10,6 +10,7 @@
 // devito/passes/iet/languages/openacc.py:79-80). One warp handles one point; lanes stride over
 // the (2r)^ndim support cells; interpolation reduces with warp shuffles.
 #include "b2_sparse.cuh"
+#include <climits>
 
 namespace b2 {
 
@@ -209,6 +210,61 @@ int launch_inject(const SparseDev &s, const FieldGeom &g, float *f0, float *f1, 
     const int warps = k.p_cnt;
     const int blocks = (warps * 32 + 127) / 128;
     k_inject<<<blocks, 128, 0, stream()>>>(k, f0, f1, time, param_kind, param, scalar_scale, dt2);
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
+}
+
+// The cells and values k_inject would add at `time`, as entries relative to the iteration origin (cells that
+// k_inject skips, or a time outside the traces: x = INT_MIN, never matched); flag |= 1 when a cell lies outside
+// the iteration box.
+__global__ void __launch_bounds__(128)
+k_inject_entries(SparseK k, int time, int valid_time, int param_kind, const float *__restrict__ param,
+                 float scalar_scale, float dt2, IsoInj *__restrict__ out, int *__restrict__ flag) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (warp >= k.p_cnt) return;
+    const int p = k.p_m + warp;
+    const int n = 2 * k.r;
+    const int ncell = n * n * n;
+    for (int c = lane; c < ncell; c += 32) {
+        IsoInj e = {INT_MIN, 0, 0, 0.f};
+        long long idx;
+        float w;
+        int c0, c1, c2;
+        if (sparse_cell(k, p, c, idx, w, c0, c1, c2)) {
+            if (flag && (c0 < k.lo0 || c0 > k.hi0 || c1 < k.lo1 || c1 > k.hi1 || c2 < k.lo2 || c2 > k.hi2))
+                atomicOr(flag, 1);
+            if (valid_time) {
+                const float sv = k.data[(long long)time * k.npoint_total + p];
+                float scale = scalar_scale;
+                if (param_kind == B2_PARAM_VP) {
+                    const float v = param[idx];
+                    scale = dt2 * v * v;
+                } else if (param_kind == B2_PARAM_M) {
+                    scale = dt2 / param[idx];
+                }
+                e = {c0 - k.lo0, c1 - k.lo1, c2 - k.lo2, w * sv * scale};
+            }
+        }
+        if (out) out[(long long)warp * ncell + c] = e;
+    }
+}
+
+int inject_entry_count(const SparseDev &s) {
+    if (!s.present) return 0;
+    const int n = 2 * s.r;
+    return (s.p_M - s.p_m + 1) * n * n * n;
+}
+
+int launch_inject_entries(const SparseDev &s, const FieldGeom &g, int time, int param_kind, const float *param,
+                          float scalar_scale, float dt2, IsoInj *out, int *outside_flag) {
+    if (!s.present) return B2_OK;
+    if (s.ndim != 3) { set_error("inject entries: 3-D only"); return B2_ERR_INVALID; }
+    SparseK k = make_k(s, g, true);
+    const int blocks = (k.p_cnt * 32 + 127) / 128;
+    k_inject_entries<<<blocks, 128, 0, stream()>>>(k, time, time >= 0 && time < s.nt, param_kind, param,
+                                                   scalar_scale, dt2, out, outside_flag);
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
     return B2_OK;

@@ -1,6 +1,7 @@
 // Sparse source injection / receiver interpolation kernels (internal interface).
 #pragma once
 #include "b2_common.cuh"
+#include "b2_iso.cuh"
 
 namespace b2 {
 
@@ -50,6 +51,13 @@ constexpr int B2_SCALE_TABLE = 3;
 // scale(cell) = dt^2 * vp^2 | dt^2 * vp[cell]^2 | dt^2 / m[cell] | param[cell] (B2_SCALE_TABLE)
 int launch_inject(const SparseDev &s, const FieldGeom &g, float *f0, float *f1, int time,
                   int param_kind, const float *param, float scalar_scale, float dt2);
+
+// The (cell, value) entries launch_inject would add at `time` (3-D; inject_entry_count of them, skipped cells never
+// match), written to `out` (device) when not null; `outside_flag` (device, may be null) |= 1 when a support cell lies
+// outside the iteration box.
+int inject_entry_count(const SparseDev &s);
+int launch_inject_entries(const SparseDev &s, const FieldGeom &g, int time, int param_kind, const float *param,
+                          float scalar_scale, float dt2, IsoInj *out, int *outside_flag);
 
 // rec[time][p] = sum w*w*w * (f0[cell] (+ f1[cell]))
 int launch_interp(const SparseDev &s, const FieldGeom &g, const float *f0, const float *f1, int time);

@@ -112,6 +112,81 @@ k_copy(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtenso
     }
 }
 
+// The two-level pass's (k_iso_tma2) stream mix: per CTA LX2 output planes of a 16 x 64 tile (the pass's own x-chunks:
+// 4R priming planes per chunk weigh 4x as much as the one-step sweep's R); per plane one 32 x 80 box of
+// u[t] (LX + 4R planes), a 24 x 72 tile of u[t-1] on the level-1 planes (LX + 2R) and, with NT == 2, one of A; the
+// consumers store a 16 x 64 tile of u[t+1] on the owned level-1 planes and one of u[t+2], R planes behind.
+template <int NT>
+struct Copy2Cfg {
+    static constexpr int TY = 16, TZ = 64, BY = TY + 4 * R, BZ = TZ + 16, EY = TY + 2 * R, EZ = TZ + 8;
+    static constexpr int UBOX = (BY * BZ + 31) / 32 * 32, ETILE = EY * EZ;
+    static constexpr int NST = R + 1;                                 // the pass's lead of R planes
+    static constexpr int NCT = 448;
+    static constexpr int LX2 = 205;                                   // choose_chunk_len at 1024^3: 5 chunks
+    static constexpr size_t SMEM = (size_t)NST * (UBOX + NT * ETILE) * 4 + 2 * NST * 8 + 128;
+};
+
+template <int NT>
+__global__ void __launch_bounds__(Copy2Cfg<NT>::NCT + 32, 1)
+k_copy2(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_um,
+        const __grid_constant__ CUtensorMap tm_a, float *__restrict__ out1, float *__restrict__ out2, Grid g) {
+    using C = Copy2Cfg<NT>;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    float *s_u = reinterpret_cast<float *>(smem_raw);
+    float *s_t = s_u + C::NST * C::UBOX;
+    uint64_t *full = reinterpret_cast<uint64_t *>(s_t + C::NST * NT * C::ETILE);
+    uint64_t *empty = full + C::NST;
+    constexpr int NCW = C::NCT / 32;
+
+    int b = blockIdx.x;
+    const int iz = b % g.ntz;
+    b /= g.ntz;
+    const int iy = b % g.nty;
+    const int ix = b / g.nty;
+    const int z0 = H + iz * C::TZ, y0 = H + iy * C::TY, xs = H + ix * C::LX2, xe = min(xs + C::LX2, H + N);
+    const int NP = (xe - xs) + 4 * R;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (tid == 0) {
+        for (int i = 0; i < C::NST; ++i) {
+            b2ptx::mbar_init(&full[i], 1);
+            b2ptx::mbar_init(&empty[i], NCW);
+        }
+        b2ptx::fence_mbar_init();
+    }
+    __syncthreads();
+    if (warp == NCW) {
+        if (lane == 0) {
+            for (int j = 0; j < NP; ++j) {
+                const int st = j % C::NST;
+                if (j >= C::NST) b2ptx::mbar_wait(&empty[st], ((j / C::NST) - 1) & 1);
+                const bool tiles = j >= 2 * R && j < NP - R;               // level-1 planes xs - R .. xs + LX + R
+                b2ptx::mbar_arrive_expect_tx(&full[st], (C::BY * C::BZ + (tiles ? NT * C::ETILE : 0)) * 4);
+                b2ptx::tma_load_3d(s_u + st * C::UBOX, &tm_u, &full[st], z0 - 8, y0 - 2 * R, xs - 2 * R + j);
+                if (tiles) {
+                    float *t = s_t + st * NT * C::ETILE;
+                    const int x1 = xs - 3 * R + j;
+                    b2ptx::tma_load_3d(t, &tm_um, &full[st], z0 - 4, y0 - R, x1);
+                    if (NT == 2) b2ptx::tma_load_3d(t + C::ETILE, &tm_a, &full[st], z0 - 4, y0 - R, x1);
+                }
+            }
+        }
+        return;
+    }
+    const int yy = tid / 16, zz = 4 * (tid % 16);                     // threads 0..255: one float4 of the tile
+    for (int j = 0; j < NP; ++j) {
+        const int st = j % C::NST;
+        b2ptx::mbar_wait(&full[st], (j / C::NST) & 1);
+        const float4 v = b2ptx::lds128(s_u + st * C::UBOX + (yy + 2 * R) * C::BZ + 8 + zz);
+        const int x1 = xs - 3 * R + j, x2 = x1 - R;
+        if (tid < 256 && x1 >= xs && x1 < xe)
+            *reinterpret_cast<float4 *>(out1 + (size_t)x1 * A * A + (size_t)(y0 + yy) * A + z0 + zz) = v;
+        if (tid < 256 && x2 >= xs && x2 < xe)
+            *reinterpret_cast<float4 *>(out2 + (size_t)x2 * A * A + (size_t)(y0 + yy) * A + z0 + zz) = v;
+        __syncwarp();
+        if (lane == 0) b2ptx::mbar_arrive(&empty[st]);
+    }
+}
+
 __global__ void k_stream(const float4 *__restrict__ src, float4 *__restrict__ dst, size_t n4) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x)
         dst[i] = src[i];
@@ -175,12 +250,45 @@ static void run_copy(const char *name, bool first) {
     CK(cudaEventDestroy(e1));
 }
 
+static float *g_out2;
+
+template <int NT>
+static void run_copy2(const char *name) {
+    using C = Copy2Cfg<NT>;
+    auto kern = k_copy2<NT>;
+    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
+    CUtensorMap tu = tmap(g_u, C::BZ, C::BY), tum = tmap(g_um, C::EZ, C::EY), ta = tmap(g_a, C::EZ, C::EY);
+    Grid g{N / C::TZ, N / C::TY, (N + C::LX2 - 1) / C::LX2};
+    const unsigned grid = g.ntz * g.nty * g.ntx;
+    kern<<<grid, C::NCT + 32, C::SMEM>>>(tu, tum, ta, g_out, g_out2, g);
+    CK(cudaGetLastError());
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0));
+    CK(cudaEventCreate(&e1));
+    CK(cudaEventRecord(e0));
+    for (int r = 0; r < kReps; ++r) kern<<<grid, C::NCT + 32, C::SMEM>>>(tu, tum, ta, g_out, g_out2, g);
+    CK(cudaEventRecord(e1));
+    CK(cudaEventSynchronize(e1));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, e0, e1));
+    ms /= kReps;
+    const double tiles = (double)g.ntz * g.nty;
+    const double moved = tiles * ((double)(N + 4 * R * g.ntx) * C::BY * C::BZ * 4 +
+                                  (double)(N + 2 * R * g.ntx) * C::ETILE * 4 * NT + 2.0 * N * C::TY * C::TZ * 4);
+    printf(", {\"name\": \"%s\", \"u_box\": [%d, %d], \"tile\": [%d, %d], \"tiles_in\": %d, \"lead\": %d, "
+           "\"smem\": %zu, \"chunk\": %d, \"ms\": %.4f, \"ms_per_step\": %.4f, \"moved_gbs\": %.1f}",
+           name, C::BY, C::BZ, C::EY, C::EZ, NT, C::NST - 1, C::SMEM, C::LX2, ms, ms / 2, moved / ms * 1e-6);
+    CK(cudaEventDestroy(e0));
+    CK(cudaEventDestroy(e1));
+}
+
 int main() {
     const size_t elems = (size_t)A * A * A;
     CK(cudaMalloc(&g_u, elems * 4));
     CK(cudaMalloc(&g_um, elems * 4));
     CK(cudaMalloc(&g_a, elems * 4));
     CK(cudaMalloc(&g_out, elems * 4));
+    CK(cudaMalloc(&g_out2, elems * 4));
     CK(cudaMemset(g_u, 0, elems * 4));
     CK(cudaMemset(g_um, 0, elems * 4));
     CK(cudaMemset(g_a, 0, elems * 4));
@@ -206,6 +314,9 @@ int main() {
     // the sweep's 16 x 128 boxes with the A tile (16 B/point) and without it (the planes whose A is pinned, 12 B/point)
     run_copy<16, 128, 4, 4, 4>("sweep_16x128", false);
     run_copy<16, 128, 4, 4, 4, 1>("sweep_16x128_noA", false);
+    // the two-level pass's boxes (k_iso_tma2): A pinned (tiles_in 1, most planes of the headline) and streamed (2)
+    run_copy2<1>("two_level_16x64_noA");
+    run_copy2<2>("two_level_16x64");
     printf("]");
 
     // plain read/write stream over 2 x 4.4 GB
@@ -229,5 +340,6 @@ int main() {
     cudaFree(g_um);
     cudaFree(g_a);
     cudaFree(g_out);
+    cudaFree(g_out2);
     return 0;
 }

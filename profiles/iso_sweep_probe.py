@@ -4,7 +4,8 @@
 Compiles iso_sweep_probe.cu with nvcc for sm_90a in a private temporary directory, runs it on GPU 0 and prints
 one JSON line: the TMA copy (the sweep's producer/mbarrier structure, no arithmetic) for the sweep's boxes at
 producer leads 1..8, the same copy without the u[t] halo and with 512-byte rows, the 16 x 128 sweep's boxes with and
-without the A tile (`tiles_in` 2 / 1: the mix of the planes whose A the sweep pins), and a plain read/write stream;
+without the A tile (`tiles_in` 2 / 1: the mix of the planes whose A the sweep pins), the two-level pass's boxes
+(`two_level_16x64*`: k_iso_tma2's mix of one u[t] read, the level-1 tiles and two stores), and a plain read/write stream;
 with the card's name, power limit and the SM clock sampled while it ran. The stream's rate is also written to
 MEASURED_PEAKS.json (`hbm_gbs`) at the repository root, the peak `bench.py` states its roofline against.
 
