@@ -161,6 +161,10 @@ def test_window_locality_full_size(kind, n):
     names = ['u'] if kind == 'iso' else ['u', 'v']
     fields = {nm: TimeFunction(name=nm, grid=model.grid, time_order=2, space_order=SO) for nm in names}
     solver.forward(src=src, time_m=1, time_M=K, **fields)
+    if kind == 'iso':
+        # the headline's kernel: an even step count, 5 linear sources (40 injection entries), a zero halo, 13.5 GB of u
+        from devito_b200 import _lib
+        assert _lib.lib().b2_last_sweep_kernel().decode() == 'iso_tma2<4,scalar>'
     devs = [fields[nm].storage.dev for nm in names]
     for dev in devs:
         assert isinstance(dev, torch.Tensor) and dev.is_cuda
