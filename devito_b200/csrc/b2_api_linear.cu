@@ -16,9 +16,10 @@ namespace b2 {
 
 __global__ void __launch_bounds__(256) k_linear(LinK k) {
     const int z = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (z >= k.n2 || y >= k.n1) return;
-    for (int x = blockIdx.z; x < k.n0; x += gridDim.z) linear_point(k, x, y, z);
+    if (z >= k.n2) return;
+    // y and x are grid-strided: gridDim.y and gridDim.z are clamped to the hardware's 65 535
+    for (int y = blockIdx.y * blockDim.y + threadIdx.y; y < k.n1; y += gridDim.y * blockDim.y)
+        for (int x = blockIdx.z; x < k.n0; x += gridDim.z) linear_point(k, x, y, z);
 }
 
 }  // namespace b2
@@ -41,7 +42,13 @@ static int linear_forward_body(const b2_linear_args *a, Staging &st) {
     int shifts[4], nshift = 0;
     for (int i = 0; i < a->ntaps; ++i) {
         const b2_tap &t = a->taps[i];
-        if (t.tshift == a->wshift) { set_error("b2_linear_forward: a tap reads the level being written"); return B2_ERR_INVALID; }
+        // the slot rule: no level read may share the written slot modulo T, or a point would read a cell that
+        // another point of the same launch is writing
+        if (slot(t.tshift - a->wshift, T) == 0) {
+            set_error("b2_linear_forward: tap %d reads level t%+d, the slot being written (t%+d modulo %d slots)", i,
+                      t.tshift, a->wshift, T);
+            return B2_ERR_INVALID;
+        }
         int s = -1;
         for (int j = 0; j < nshift; ++j) if (shifts[j] == t.tshift) s = j;
         if (s < 0) {
@@ -63,10 +70,6 @@ static int linear_forward_body(const b2_linear_args *a, Staging &st) {
         k.delta[i] = delta;
         k.coef[i] = t.coef;
     }
-    if (T <= nshift) {   // every level read and the one written must be distinct slots
-        set_error("b2_linear_forward: %d time slots cannot hold %d levels", T, nshift + 1);
-        return B2_ERR_INVALID;
-    }
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (a->timers) {
         cudaEventCreate(&e0);
@@ -74,7 +77,7 @@ static int linear_forward_body(const b2_linear_args *a, Staging &st) {
         cudaEventRecord(e0, stream());
     }
     dim3 block(64, 4, 1);
-    dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
+    dim3 grid((k.n2 + 63) / 64, (unsigned)std::min((k.n1 + 3) / 4, 65535), (unsigned)std::min(k.n0, 65535));
     float *base = (float *)f->d;
     // an update of `f.backward` (wshift = -1) runs from time_M down to time_m, like the reference's
     // backward-in-time loop (devito/ir/support/space.py: Backward direction)

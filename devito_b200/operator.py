@@ -319,8 +319,6 @@ class Operator:
             k = _space_offsets(acc, None)
             if k is None:
                 raise _Unrecognised("non-affine access")
-            if k[0] == kl[0]:
-                raise _Unrecognised("implicit scheme: the written time level is read")
             if any(abs(o) > f.space_order for o in k[1]):
                 raise _Unrecognised("stencil reaches beyond the halo")
             for n in coef.preorder():
@@ -329,8 +327,10 @@ class Operator:
             taps.append((k[0], k[1], coef))
         if not taps or len(taps) > L_.MAX_TAPS or len({t for t, _, _ in taps}) > 4:
             raise _Unrecognised("unsupported number of taps / time levels")
-        if f.time_size < len({t for t, _, _ in taps}) + 1:
-            raise _Unrecognised("not enough time slots")
+        # the slot rule (as in b2_linear_forward): no level read may share the written slot modulo time_size,
+        # or a point would read a cell another point of the same step is writing
+        if any((t - kl[0]) % f.time_size == 0 for t, _, _ in taps):
+            raise _Unrecognised("a level read shares the written time slot (implicit, or aliased modulo time_size)")
         taps.sort(key=lambda t: (t[0], t[1]))
         # iteration box: the equation's SubDomain (rectangular) or the whole grid
         box = []
@@ -2068,12 +2068,13 @@ class Operator:
             env[p['dt'].name] = float(np.float32(kwargs.pop('dt')))
         elif need_dt:
             raise InvalidArgument("No value found for parameter dt")
+        # a Constant may appear in many taps: resolve each one (and its override) once
+        nodes = {id(n): n for _, _, c in p['taps'] for n in c.preorder() if n.is_Constant}
+        over = {n.name: kwargs.pop(n.name) for n in nodes.values() if n.name in kwargs}
         consts = {}
-        for _, _, c in p['taps']:
-            for n in c.preorder():
-                if n.is_Constant:
-                    v = kwargs.pop(n.name, n)
-                    consts[id(n)] = float(v.data if isinstance(v, Constant) else v)
+        for k, n in nodes.items():
+            v = over.get(n.name, n)
+            consts[k] = float(v.data if isinstance(v, Constant) else v)
 
         def leaf(n):
             if n.is_Constant:

@@ -117,7 +117,7 @@ extern "C" int emu_snapshot(const float *slot, const int *alloc, int so, float *
     return 0;
 }
 
-// Generic constant-coefficient update, same marshalling as b2_linear_forward (b2_api_linear.cu)
+// Generic constant-coefficient update, same marshalling and loop direction as b2_linear_forward (b2_api_linear.cu)
 extern "C" int emu_linear_steps(float *f, int tsize, int ndim, const int *size /* ndim */, int halo, int ntaps,
                                 const int *tshift, const int *off /* ntaps x 3 */, const float *coef,
                                 int wshift, const int *lo_in, const int *hi_in, int time_m, int time_M) {
@@ -147,7 +147,9 @@ extern "C" int emu_linear_steps(float *f, int tsize, int ndim, const int *size /
         k.delta[i] = delta;
         k.coef[i] = coef[i];
     }
-    for (int time = time_m; time <= time_M; ++time) {
+    // like b2_linear_forward: an update of `f.backward` (wshift = -1) runs from time_M down to time_m
+    const int dirn = wshift;
+    for (int time = dirn > 0 ? time_m : time_M; dirn > 0 ? time <= time_M : time >= time_m; time += dirn) {
         k.out = f + (size_t)((((time + wshift) % tsize) + tsize) % tsize) * slot;
         for (int j = 0; j < 4; ++j)
             k.lvl[j] = f + (size_t)((((time + shifts[j < nshift ? j : 0]) % tsize) + tsize) % tsize) * slot;

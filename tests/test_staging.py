@@ -245,6 +245,31 @@ def test_tti_born_du_without_born_dm():
     _refused('b2_tti_forward', a, host, 'born_du, born_dv and born_dm together')
 
 
+@pytest.mark.parametrize('T,taps,wshift,what', [
+    (3, [(0, (0, 0, 0)), (-2, (1, 0, 0))], 1, 'the slot being written'),      # t - 2 is t + 1 modulo 3
+    (2, [(0, (0, 0, 0)), (1, (0, 0, -1))], -1, 'the slot being written'),     # t + 1 is t - 1 modulo 2
+    (2, [(1, (0, 0, 0))], 1, 'the slot being written'),                        # implicit
+    (2, [(0, (0, 0, 0)), (0, (0, 2, 0))], 1, 'leaves the allocated array'),    # halo 1
+    (2, [], 1, '0 taps'),
+    (2, [(0, (0, 0, 0))] * 65, 1, '65 taps'),
+    (6, [(-k, (0, 0, 0)) for k in range(5)], 1, 'more than 4 time levels'),
+    (2, [(-1, (0, 0, 0))], 0, 'wshift must be'),
+], ids=['alias-fwd', 'alias-bwd', 'implicit', 'beyond-alloc', '0-taps', '65-taps', '5-levels', 'wshift-0'])
+def test_linear_refusals(T, taps, wshift, what):
+    L = _L()
+    c = Call(1)
+    f = c.field((T,))
+    arr = (L.Tap * max(len(taps), 1))()
+    for i, (s, off) in enumerate(taps):
+        arr[i].tshift, arr[i].coef = s, 0.5
+        for d in range(3):
+            arr[i].off[d] = off[d]
+    a = L.LinearArgs()
+    a.ndim, a.f, a.halo, a.ntaps, a.taps, a.wshift = 3, c.obj(f), 1, len(taps), arr, wshift
+    c.box(a)
+    _refused('b2_linear_forward', a, {'f': f}, what)
+
+
 # ---- a NaN stops the call (100), and the written arrays still come back ----------------------------------------
 
 def test_iso_gradient_nan_writes_back():

@@ -15,6 +15,7 @@ import pytest
 
 from oracle import oracle as O
 from helpers import rel_linf
+import linear_cases as LC
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = pytest.mark.skipif(shutil.which('nvcc') is None, reason="nvcc not available")
@@ -220,6 +221,30 @@ def test_linear_point_kernel_runs_the_diffusion_example(emu):
             (ref[1:-1, 2:] - 2 * ref[1:-1, 1:-1] + ref[1:-1, :-2]) / hy ** 2)
         ref = new
     assert rel_linf(f[nt % 2, so:-so, so:-so], ref) < 1e-5
+
+
+@pytest.mark.parametrize('m', [m for m in LC.MATRIX if m[2] in ('fwd4', 'bwd3')], ids=LC.case_id)
+def test_linear_point_kernel_vs_float64(emu, m):
+    """Cases of the generic-update matrix (tests/test_linear_matrix.py) through `linear_point` on the CPU, with the
+    taps and box the operator computes at apply, against tests/linear_ref.py: the 1-D and 3-D index arithmetic, the
+    backward loop and the recogniser's taps, without a GPU."""
+    c = LC.case(*m)
+    op, _, _, _ = LC.build(c)
+    _, _, over = LC.bounds(c)
+    args = op.arguments(time_m=c['time_m'], time_M=c['time_M'], dt=LC.DEFAULTS['dt'], **over)
+    taps = args['taps']
+    tshift = np.array([t for t, _, _ in taps], dtype=np.int32)
+    off = np.zeros((len(taps), 3), dtype=np.int32)
+    for i, (_, o, _) in enumerate(taps):
+        off[i, :c['nd']] = o
+    coef = np.array([x for _, _, x in taps], dtype=np.float32)
+    f = c['f'].copy()
+    rc = emu.emu_linear_steps(_fp(f), f.shape[0], c['nd'], _ip(np.array(f.shape[1:], dtype=np.int32)), c['so'],
+                              len(taps), _ip(tshift), _ip(off), _fp(coef), op._plan['wshift'],
+                              _ip(np.array(args['lo'], dtype=np.int32)), _ip(np.array(args['hi'], dtype=np.int32)),
+                              args['time_m'], args['time_M'])
+    assert rc == 0
+    LC.check(c, f, LC.reference(c))
 
 
 def _emu_scheme(emu, c):
