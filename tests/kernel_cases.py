@@ -66,12 +66,54 @@ TILES = {
     # b2_sa.cu SaTmaCfg<R>
     'sa_tma<2>': (16, 64), 'sa_tma<4>': (16, 64),
 }
+TTI_SA_TILES = {name: t for name, t in TILES.items() if name.startswith(('tti_', 'sa_'))}
+
+# Grids cut into several yz-tiles by every TTI and SA tile (tests/test_tti_sa_tiling.py checks these claims):
+#   TTI_MULTI: y tiles of 32, 28, 24, 30, 20, 16 rows: 3, 3, 3, 3, 4, 5 tiles, the last 7, 15, 23, 11, 11, 7 rows;
+#              z: 6 tiles, the last 44 points. nty != ntz everywhere, so a block index decoded with the two counts
+#              exchanged (or the tile origins of y and z exchanged) covers other tiles. The z allocation 364 + 2 so
+#              keeps the rows 16-byte aligned.
+#   TTI_MULTI_TAIL: z extent 362: the last z tile 42 points, every row ends in a partial float4 group of 2.
+#   TTI_MULTI_SUB: y extent 65 (a last y tile of one row for TY 32 and 16), z extent 352 (the last z tile 32);
+#                  x extent 11: x-chunks of 5, 5, 1 with B2_TTI_LX=5.
+#   TTI_EXACT: (9, 3 TY, 256) per sweep: 3 x 4 full tiles.
+#   LONGX: nothing forced, choose_chunk_len on 132 SMs cuts the 150 x-planes of every TTI sweep into chunks of
+#          LONGX_LX = 38 planes (38, 38, 38, 36).
+TTI_MULTI = (13, 71, 364)
+TTI_MULTI_TAIL = ((0, 0, 0), (12, 70, 361))
+TTI_MULTI_SUB = ((1, 3, 4), (11, 67, 355))
+TTI_EXACT = {name: (9, 3 * ty, 256) for name, (ty, _) in TTI_SA_TILES.items()}
+LONGX = (150, 30, 64)
+LONGX_LX = 38
+H100_SMS = 132
 
 
 def tiling(n, t):
     """(number of tiles, extent of the last one) of an extent n cut into tiles of t"""
     k = -(-n // t)
     return k, n - (k - 1) * t
+
+
+def chunk_len(sms, tiles, xcount, prime, min_len=32):
+    """b2_common.cuh choose_chunk_len: the x-chunk length that minimises wave quantisation x priming overhead"""
+    best, best_n = 1e30, 1
+    for n in range(1, 65):
+        lx = -(-xcount // n)
+        if n > 1 and lx < min_len:
+            break
+        if lx > 256 and (xcount + n) // (n + 1) >= min_len:
+            continue
+        ctas = tiles * n
+        rounds = -(-ctas // sms)
+        cost = rounds * sms / ctas * (1.0 + prime / lx)
+        if cost < best - 1e-9:
+            best, best_n = cost, n
+    return -(-xcount // best_n)
+
+
+def x_chunks(xcount, lx):
+    """extents of the x-chunks of length lx (the last may be shorter)"""
+    return [min(lx, xcount - s) for s in range(0, xcount, lx)]
 
 
 def box_extent(box):
@@ -112,10 +154,14 @@ def tti_case(so, arrays, shape=SHAPE, box=None, seed=0):
                 dt=float(O.critical_dt(so, 3, min(SPACING), 2.5, eps_max=0.3)))
 
 
-def sparse_coordinates(shape=SHAPE, seed=3):
+def sparse_coordinates(shape=SHAPE, seed=3, seams=None):
     """Physical coordinates (origin 0) of points within one cell of every face, points outside the domain on both
     sides of every axis (their supports reach into the halo, or miss the grid entirely), and two points in one
-    cell (their deposits meet in the same cells)."""
+    cell (their deposits meet in the same cells).
+
+    seams = (origin, xcuts) appends, after those, points half a cell either side of every seam inside the grid: of the
+    TTI and SA yz-tiles counted from the box corner `origin` (y = origin + TY k for every tile height TY, z = origin +
+    64 and + 128) and of the x-chunks that begin at the x indices `xcuts`. Their supports straddle the seam."""
     rng = np.random.default_rng(seed)
     n = np.array(shape)
     h = np.array(SPACING)
@@ -135,6 +181,20 @@ def sparse_coordinates(shape=SHAPE, seed=3):
     c = np.floor(interior())
     pts.append(c + 0.27)
     pts.append(c + np.array([0.81, 0.62, 0.55]))                    # same base cell as the point above
+    if seams is not None:
+        origin, xcuts = seams
+        tys = sorted({ty for ty, _ in TTI_SA_TILES.values()})
+        (tz,) = {tz for _, tz in TTI_SA_TILES.values()}
+        cuts = [sorted(xcuts),
+                sorted({origin[1] + ty * k for ty in tys for k in range(1, n[1] // ty + 1)}),
+                [origin[2] + tz, origin[2] + 2 * tz]]
+        for d, cs in enumerate(cuts):
+            for cut in cs:
+                for where in (cut - 0.5, cut + 0.5):
+                    if 0 < where < n[d] - 1:
+                        p = interior()
+                        p[d] = where
+                        pts.append(p)
     return (np.array(pts) * h).astype(np.float32)
 
 

@@ -76,11 +76,14 @@ def _iso_setup(so, param, shape=KC.SHAPE, box=None, interpolation=None):
 
 
 @functools.lru_cache(maxsize=None)
-def _tti_setup(so, arrays, box=None):
-    from devito_b200 import Constant, Eq, Operator, TimeFunction, solve, sqrt
+def _tti_setup(so, arrays, box=None, shape=KC.SHAPE, seams=None):
+    """(operator, (u, v), rec, case, source tables). With `seams` (see KC.sparse_coordinates) the sources are injected
+    into u and v and the receivers sample u + v, as in devito_b200/seismic/tti.py (sinc from so = 8 on, else linear);
+    without, the operator has no sparse terms and rec and the tables are None."""
+    from devito_b200 import Constant, Eq, Operator, SparseTimeFunction, TimeFunction, solve, sqrt
     from devito_b200.seismic.tti import Gzz_centered
-    c = KC.tti_case(so, arrays, box=box)
-    grid = _grid(KC.SHAPE)
+    c = KC.tti_case(so, arrays, shape=shape, box=box)
+    grid = _grid(shape)
     u = TimeFunction(name='u', grid=grid, time_order=2, space_order=so)
     v = TimeFunction(name='v', grid=grid, time_order=2, space_order=so)
     damp = _function('damp', grid, so, c['damp'])
@@ -93,20 +96,28 @@ def _tti_setup(so, arrays, box=None):
     sd, e2 = sqrt(1 + 2 * P['delta']), 1 + 2 * P['epsilon']
     eqs = [Eq(u.forward, solve(m * u.dt2 - (e2 * gxx + sd * gzz) + damp * u.dt, u.forward)),
            Eq(v.forward, solve(m * v.dt2 - (sd * gxx + gzz) + damp * v.dt, v.forward))]
+    rec, tables = None, None
+    if seams is not None:
+        interpolation = 'sinc' if so >= 8 else 'linear'
+        coords = KC.sparse_coordinates(shape, seams=seams)
+        tables = KC.sparse_tables(coords, interpolation, KC.K + 2)
+        sp = lambda n: SparseTimeFunction(name=n, grid=grid, npoint=len(coords), nt=KC.K + 2,
+                                          interpolation=interpolation, r=tables['r'], coordinates=coords)
+        src, rec = sp('src'), sp('rec')
+        src.data[:] = tables['data']
+        dt = grid.stepping_dim.spacing
+        eqs += src.inject(field=(u.forward, v.forward), expr=src * dt ** 2 / m) + rec.interpolate(expr=u + v)
     op = Operator(eqs)
     assert op.backend == 'cuda-sm90a'
-    return op, (u, v), c
+    return op, (u, v), rec, c, tables
 
 
 @functools.lru_cache(maxsize=None)
 def _reference(key):
     """float64 result of a configuration (shared by all its kernel variants)."""
-    if key[0] == 'iso':
-        _, _, _, c, tables = _iso_setup(*key[1:])
-        rec = dict(tables, data=np.zeros_like(tables['data'])) if tables is not None else None
-        return KC.reference(c, src=tables, rec=rec)
-    _, _, c = _tti_setup(*key[1:])
-    return KC.reference(c)
+    *_, c, tables = (_iso_setup if key[0] == 'iso' else _tti_setup)(*key[1:])
+    rec = dict(tables, data=np.zeros_like(tables['data'])) if tables is not None else None
+    return KC.reference(c, src=tables, rec=rec)
 
 
 def _run(fields, c, op, expect, rec=None, **kw):
@@ -132,11 +143,14 @@ def _check_iso(key, expect, **kw):
 
 
 def _check_tti(key, expect, **kw):
-    op, (u, v), c = _tti_setup(*key[1:])
-    got = _run([u, v], c, op, expect, **kw)
-    want, _ = _reference(key)
+    op, (u, v), rec, c, _ = _tti_setup(*key[1:])
+    got = _run([u, v], c, op, expect, rec=rec, **kw)
+    want, traces = _reference(key)
     for g, w in zip(got, want):
         assert rel_linf(g, w) < KC.TOL['tti']
+    if rec is not None:
+        assert np.abs(traces).max() > 0
+        assert rel_linf(np.array(rec.data), traces) < KC.TOL['tti']
 
 
 PARAMS = ['scalar', 'vp', 'm']

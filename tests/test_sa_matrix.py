@@ -41,7 +41,9 @@ def sa_case(so, arrays, nd=3, seed=0, shape=None):
 
 
 @functools.lru_cache(maxsize=None)
-def _setup(so, arrays, adjoint, nd=3, shape=None):
+def _setup(so, arrays, adjoint, nd=3, shape=None, seams=None):
+    """(operator, u, rec, case, source tables); `seams` (3-D): KC.sparse_coordinates' points beside the tile and
+    x-chunk seams, added to its usual points"""
     from devito_b200 import Constant, Function, Grid, Operator, SparseTimeFunction, TimeFunction
     from devito_b200.seismic.self_adjoint import iso_stencil
     c = sa_case(so, arrays, nd, shape=shape)
@@ -57,7 +59,7 @@ def _setup(so, arrays, adjoint, nd=3, shape=None):
     u = TimeFunction(name='u', grid=grid, time_order=2, space_order=so)
     eqs = iso_stencil(u, model, forward=not adjoint)
     interpolation = 'sinc' if so >= 8 else 'linear'
-    coords = KC.sparse_coordinates(shape=c['shape']) if nd == 3 else KC.sparse_coordinates()
+    coords = KC.sparse_coordinates(shape=c['shape'], seams=seams) if nd == 3 else KC.sparse_coordinates()
     if nd == 2:
         coords = np.ascontiguousarray(coords[:, [0, 2]])
     tables = sparse_tables(coords, interpolation, KC.K + 2, c['spacing'])
@@ -90,6 +92,7 @@ def _reference(key, lo, hi):
 
 
 def _check(key, sweep, box, **kw):
+    """box: 'full', a name of KC.BOXES (3-D; 2-D: an interior box) or a 3-D (lo, hi)"""
     op, u, rec, c, _ = _setup(*key)
     u.data_with_halo[:] = c['u']
     rec.data[:] = 0.0
@@ -97,7 +100,7 @@ def _check(key, sweep, box, **kw):
     if box == 'full':
         lo, hi = [0] * nd, [n - 1 for n in c['shape']]
     elif nd == 3:
-        lo, hi = list(KC.BOXES[box][0]), list(KC.BOXES[box][1])
+        lo, hi = map(list, KC.BOXES[box] if isinstance(box, str) else box)
     else:
         lo, hi = [1, 4], [c['shape'][0] - 3, c['shape'][1] - 9]
     bounds = {}

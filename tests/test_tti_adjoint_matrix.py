@@ -30,22 +30,24 @@ def _last_kernel():
     return _lib.lib().b2_last_sweep_kernel().decode()
 
 
-def adj_case(so, arrays, box=None, seed=0):
-    c = KC.tti_case(so, arrays, box=box, seed=seed)
+def adj_case(so, arrays, box=None, seed=0, shape=KC.SHAPE):
+    c = KC.tti_case(so, arrays, shape=shape, box=box, seed=seed)
     rng = np.random.default_rng(seed + 100 * so + 71)
     c['usave'] = rng.standard_normal((KC.K + 2,) + c['u'].shape[1:]).astype(np.float32)
     c['vsave'] = rng.standard_normal((KC.K + 2,) + c['u'].shape[1:]).astype(np.float32)
-    c['grad'] = rng.standard_normal(tuple(n + 2 * KC.GRAD_HALO for n in KC.SHAPE)).astype(np.float32)
+    c['grad'] = rng.standard_normal(tuple(n + 2 * KC.GRAD_HALO for n in shape)).astype(np.float32)
     return c
 
 
 @functools.lru_cache(maxsize=None)
-def _setup(so, arrays, gradient, box=None):
+def _setup(so, arrays, gradient, box=None, shape=KC.SHAPE, seams=None):
+    """(operator, functions, case, receiver tables) on `shape`; `seams`: KC.sparse_coordinates' points beside the
+    tile and x-chunk seams, added to its usual points"""
     from devito_b200 import (Constant, Eq, Function, Grid, Inc, Operator, SparseTimeFunction, TimeFunction, solve,
                              sqrt)
     from devito_b200.seismic.tti import Gzz_centered
-    c = adj_case(so, arrays, box)
-    grid = Grid(shape=KC.SHAPE, extent=tuple((n - 1) * h for n, h in zip(KC.SHAPE, KC.SPACING)))
+    c = adj_case(so, arrays, box, shape=shape)
+    grid = Grid(shape=shape, extent=tuple((n - 1) * h for n, h in zip(shape, KC.SPACING)))
 
     def fn(name, values, space_order=so):
         f = Function(name=name, grid=grid, space_order=space_order)
@@ -63,7 +65,7 @@ def _setup(so, arrays, gradient, box=None):
     eqs = [Eq(p.backward, solve(m * p.dt2 - H0 + damp * p.dt.T, p.backward)),
            Eq(r.backward, solve(m * r.dt2 - Hz + damp * r.dt.T, r.backward))]
     interpolation = 'sinc' if so >= 8 else 'linear'
-    coords = KC.sparse_coordinates()
+    coords = KC.sparse_coordinates(shape, seams=seams)
     tables = KC.sparse_tables(coords, interpolation, KC.K + 2)
     sp = lambda n: SparseTimeFunction(name=n, grid=grid, npoint=len(coords), nt=KC.K + 2, interpolation=interpolation,
                                       r=tables['r'], coordinates=coords)

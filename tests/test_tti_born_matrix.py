@@ -30,24 +30,26 @@ def _last_kernel():
     return _lib.lib().b2_last_sweep_kernel().decode()
 
 
-def born_case(so, arrays, box=None, dmh=0, seed=0):
+def born_case(so, arrays, box=None, dmh=0, seed=0, shape=KC.SHAPE):
     """A KC TTI case plus the linearised pair (white noise in every slot) and dm with halo `dmh`."""
-    c = KC.tti_case(so, arrays, box=box, seed=seed)
+    c = KC.tti_case(so, arrays, shape=shape, box=box, seed=seed)
     rng = np.random.default_rng(seed + 100 * so + 53)
     c['du'] = rng.standard_normal(c['u'].shape).astype(np.float32)
     c['dv'] = rng.standard_normal(c['u'].shape).astype(np.float32)
-    c['dm'] = (0.05 * rng.standard_normal(tuple(n + 2 * dmh for n in KC.SHAPE))).astype(np.float32)
+    c['dm'] = (0.05 * rng.standard_normal(tuple(n + 2 * dmh for n in shape))).astype(np.float32)
     c['dmh'] = dmh
     return c
 
 
 @functools.lru_cache(maxsize=None)
-def _setup(so, arrays, box=None, dmh=0):
+def _setup(so, arrays, box=None, dmh=0, shape=KC.SHAPE, seams=None):
+    """(operator, functions, case, source tables) on `shape`; `seams`: KC.sparse_coordinates' points beside the
+    tile and x-chunk seams, added to its usual points"""
     from devito_b200 import (Constant, Eq, Function, Grid, Operator, SparseTimeFunction, TimeFunction, solve,
                              sqrt)
     from devito_b200.seismic.tti import Gzz_centered
-    c = born_case(so, arrays, box, dmh)
-    grid = Grid(shape=KC.SHAPE, extent=tuple((n - 1) * h for n, h in zip(KC.SHAPE, KC.SPACING)))
+    c = born_case(so, arrays, box, dmh, shape=shape)
+    grid = Grid(shape=shape, extent=tuple((n - 1) * h for n, h in zip(shape, KC.SPACING)))
 
     def fn(name, values, space_order=so):
         f = Function(name=name, grid=grid, space_order=space_order)
@@ -68,7 +70,7 @@ def _setup(so, arrays, box=None, dmh=0):
         return [Eq(u.forward, solve(m * u.dt2 - (e2 * gxx + sd * gzz) - qu + damp * u.dt, u.forward)),
                 Eq(v.forward, solve(m * v.dt2 - (sd * gxx + gzz) - qv + damp * v.dt, v.forward))]
     interpolation = 'sinc' if so >= 8 else 'linear'
-    coords = KC.sparse_coordinates()
+    coords = KC.sparse_coordinates(shape, seams=seams)
     tables = KC.sparse_tables(coords, interpolation, KC.K + 2)
     sp = lambda n: SparseTimeFunction(name=n, grid=grid, npoint=len(coords), nt=KC.K + 2, interpolation=interpolation,
                                       r=tables['r'], coordinates=coords)
