@@ -498,7 +498,6 @@ static int iso_forward_body(const b2_iso_args *a, Staging &st, SnapStreamer &str
     DevArray snap_host;                           // host snapshots streamed out: described, not staged
     SparseDev src, rec;
     IsoPlan p;
-    FieldGeom g;
 
     // A large host-staged wavefield is a candidate for the streamed time loop (copies overlapped with a
     // skewed sweep, iso_forward_streamed): its uploads are then issued chunk by chunk, not here. Whether the
@@ -524,15 +523,7 @@ static int iso_forward_body(const b2_iso_args *a, Staging &st, SnapStreamer &str
         if (!a->param) { set_error("b2_iso_forward: param array missing"); return B2_ERR_INVALID; }
         if ((rc = st.array(a->param, nd, false, param, !maybe_stream))) return rc;
     }
-    if ((rc = sparse_stage_in(st, a->src, nd, false, src))) return rc;
-    if ((rc = sparse_stage_in(st, a->rec, nd, true, rec))) return rc;
-    // the support of a sparse point reaches r cells beyond the iterated box: it must fit in the halo
-    // (devito/operations/interpolators.py:28-37 `check_radius`)
-    if ((src.present && src.r > so) || (rec.present && rec.r > so)) {
-        set_error("b2_iso_forward: sparse radius %d exceeds the halo (space_order %d)",
-                  src.present && src.r > so ? src.r : rec.r, so);
-        return B2_ERR_INVALID;
-    }
+    if ((rc = sparse_stage_pair("b2_iso_forward", st, a->src, a->rec, nd, so, src, rec))) return rc;
     int gh = 0;
     if (a->grad || a->usave) {
         if (!a->grad || !a->usave || nd != 3) {
@@ -595,40 +586,14 @@ static int iso_forward_body(const b2_iso_args *a, Staging &st, SnapStreamer &str
         }
     }
 
-    // ---- geometry in the internal 3-dim convention ----
-    const int lo_in[3] = {a->x_m, a->y_m, a->z_m};
-    const int hi_in[3] = {a->x_M, a->y_M, a->z_M};
-    p.tsize = u->size[0];
-    p.so = so;
-    if (nd == 3) {
-        for (int d = 0; d < 3; ++d) {
-            p.a[d] = u->size[d + 1];
-            p.n[d] = hi_in[d] - lo_in[d] + 1;
-            p.o[d] = lo_in[d] + so;
-            p.radius[d] = a->radius;
-        }
-    } else {
-        p.a[0] = 1; p.n[0] = 1; p.o[0] = 0; p.radius[0] = 0;
-        for (int d = 0; d < 2; ++d) {
-            p.a[d + 1] = u->size[d + 1];
-            p.n[d + 1] = hi_in[d] - lo_in[d] + 1;
-            p.o[d + 1] = lo_in[d] + so;
-            p.radius[d + 1] = a->radius;
-        }
+    static_cast<Box &>(p) = make_box(a, nd, u->size, so);
+    bool empty;
+    if ((rc = check_reach("b2_iso_forward", p, nd, a->radius, empty))) return rc;
+    if (empty) {
+        u->written = false;       // nothing ran, and u's host -> device copy may still be deferred (maybe_stream)
+        return B2_OK;
     }
-    for (int d = 0; d < 3; ++d) {
-        if (p.n[d] <= 0) return B2_OK;
-        const int rd = p.radius[d];
-        if (p.o[d] - rd < 0 || p.o[d] + p.n[d] - 1 + rd >= p.a[d]) {
-            set_error("b2_iso_forward: iteration range [%d,%d] + radius %d leaves the allocated "
-                      "array (extent %d) on dim %d", lo_in[nd == 3 ? d : d - 1], hi_in[nd == 3 ? d : d - 1],
-                      rd, p.a[d], d);
-            return B2_ERR_INVALID;
-        }
-    }
-    p.sy = p.a[2];
-    p.sx = (long long)p.a[1] * p.a[2];
-    p.slot_elems = (size_t)p.a[0] * p.a[1] * p.a[2];
+    for (int d = 3 - nd; d < 3; ++d) p.radius[d] = a->radius;
     p.u = (float *)u->d;
     p.damp = damp ? (const float *)damp->d : nullptr;
     p.param = param ? (const float *)param->d : nullptr;
@@ -673,14 +638,7 @@ static int iso_forward_body(const b2_iso_args *a, Staging &st, SnapStreamer &str
         return B2_ERR_INVALID;
     }
 
-    g.sx = p.sx;
-    g.sy = p.sy;
-    g.slot_elems = p.slot_elems;
-    g.so = so;
-    g.ndim = nd;
-    for (int d = 0; d < nd; ++d) { g.lo[d] = lo_in[d]; g.hi[d] = hi_in[d]; }
-    if (a->halo) { g.nb_lo = a->halo->rank > 0; g.nb_hi = a->halo->rank < a->halo->nranks - 1; }
-
+    FieldGeom g = field_geom(p, nd, a->halo);
     const float dt2 = a->dt * a->dt;
     const float scalar_scale = dt2 * a->vp * a->vp;
     const int T = p.tsize;
@@ -821,27 +779,17 @@ static int iso_forward_body(const b2_iso_args *a, Staging &st, SnapStreamer &str
                 return rc;
         }
         if (per_step_events) se.next();
-        if (a->errctl && ((time - a->time_m) % 100 == 99 || time == (a->adjoint ? a->time_m : a->time_M))) {
-            bool bad = false;
-            if ((rc = check_finite(f1, p.slot_elems, bad))) return rc;
-            if (bad) { set_error("NaN/Inf detected in u at time=%d", time); return B2_ERR_NAN; }
-        }
+        if (a->errctl && errctl_due(time, a->time_m, a->adjoint ? a->time_m : a->time_M) &&
+            (rc = check_finite(f1, p.slot_elems, "u", time)))
+            return rc;
     }
     if (a->halo && (rc = halo_p2p_drain(a->halo))) return rc;
     if (timing) cudaEventRecord(ev_tot[1], stream());
     cudaEventRecord(ev_prof[1], stream());
-    if (streamed && a->errctl) {
-        bool bad = false;
-        const int tl = slot(a->time_M + 1, T);
-        if ((rc = check_finite(p.u + (size_t)tl * p.slot_elems, p.slot_elems, bad))) return rc;
-        if (bad) { set_error("NaN/Inf detected in u at time=%d", a->time_M); return B2_ERR_NAN; }
-    }
-
-    cudaError_t e = cudaStreamSynchronize(stream());
-    if (e != cudaSuccess) {
-        set_error("b2_iso_forward: device error: %s", cudaGetErrorString(e));
-        return B2_ERR_LAUNCH;
-    }
+    if (streamed && a->errctl &&
+        (rc = check_finite(p.u + (size_t)slot(a->time_M + 1, T) * p.slot_elems, p.slot_elems, "u", a->time_M)))
+        return rc;
+    if ((rc = sync_call("b2_iso_forward"))) return rc;
     {
         float ms = 0.f;
         if (cudaEventElapsedTime(&ms, ev_prof[0], ev_prof[1]) == cudaSuccess) g_last_profile[1] = ms;

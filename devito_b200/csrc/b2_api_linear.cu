@@ -29,14 +29,13 @@ static int linear_forward_body(const b2_linear_args *a, Staging &st) {
     DevArray *f;
     int rc = st.array(a->f, nd + 1, true, f);
     if (rc) return rc;
-    const Box3 b = box3(a, nd, &f->size[1], a->halo);
-    const int T = f->size[0];
+    const Box b = make_box(a, nd, f->size, a->halo);
+    const int T = b.tsize;
     LinK k;
-    k.sy = b.alloc[2];
-    k.sx = (long long)b.alloc[1] * b.alloc[2];
-    const size_t slot_len = (size_t)b.alloc[0] * b.alloc[1] * b.alloc[2];
-    k.n0 = b.hi[0] - b.lo[0] + 1; k.n1 = b.hi[1] - b.lo[1] + 1; k.n2 = b.hi[2] - b.lo[2] + 1;
-    k.o0 = b.lo[0] + b.hal[0]; k.o1 = b.lo[1] + b.hal[1]; k.o2 = b.lo[2] + b.hal[2];
+    k.sy = b.sy;
+    k.sx = b.sx;
+    k.n0 = b.n[0]; k.n1 = b.n[1]; k.n2 = b.n[2];
+    k.o0 = b.o[0]; k.o1 = b.o[1]; k.o2 = b.o[2];
     if (k.n0 <= 0 || k.n1 <= 0 || k.n2 <= 0) return B2_OK;
     k.ntaps = a->ntaps;
     int shifts[4], nshift = 0;
@@ -61,7 +60,7 @@ static int linear_forward_body(const b2_linear_args *a, Staging &st) {
         for (int d = 0; d < nd; ++d) {
             const int di = 3 - nd + d, o = t.off[d];
             // the read must stay inside the allocated array
-            if (b.lo[di] + b.hal[di] + o < 0 || b.hi[di] + b.hal[di] + o >= b.alloc[di]) {
+            if (b.o[di] + o < 0 || b.o[di] + b.n[di] - 1 + o >= b.a[di]) {
                 set_error("b2_linear_forward: tap offset %d on dim %d leaves the allocated array", o, d);
                 return B2_ERR_INVALID;
             }
@@ -70,12 +69,7 @@ static int linear_forward_body(const b2_linear_args *a, Staging &st) {
         k.delta[i] = delta;
         k.coef[i] = t.coef;
     }
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (a->timers) {
-        cudaEventCreate(&e0);
-        cudaEventCreate(&e1);
-        cudaEventRecord(e0, stream());
-    }
+    if ((rc = loop_timer_start(a->timers))) return rc;
     dim3 block(64, 4, 1);
     dim3 grid((k.n2 + 63) / 64, (unsigned)std::min((k.n1 + 3) / 4, 65535), (unsigned)std::min(k.n0, 65535));
     float *base = (float *)f->d;
@@ -83,23 +77,13 @@ static int linear_forward_body(const b2_linear_args *a, Staging &st) {
     // backward-in-time loop (devito/ir/support/space.py: Backward direction)
     const int dirn = a->wshift;
     for (int time = dirn > 0 ? a->time_m : a->time_M; dirn > 0 ? time <= a->time_M : time >= a->time_m; time += dirn) {
-        k.out = base + (size_t)slot(time + a->wshift, T) * slot_len;
-        for (int j = 0; j < nshift; ++j) k.lvl[j] = base + (size_t)slot(time + shifts[j], T) * slot_len;
+        k.out = base + (size_t)slot(time + a->wshift, T) * b.slot_elems;
+        for (int j = 0; j < nshift; ++j) k.lvl[j] = base + (size_t)slot(time + shifts[j], T) * b.slot_elems;
         for (int j = nshift; j < 4; ++j) k.lvl[j] = k.lvl[0];
         k_linear<<<grid, block, 0, stream()>>>(k);
         count_launch();
     }
-    cudaError_t e = cudaGetLastError();
-    if (a->timers) cudaEventRecord(e1, stream());
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream());
-    if (a->timers) {
-        float ms = 0.f;
-        if (e == cudaSuccess && cudaEventElapsedTime(&ms, e0, e1) == cudaSuccess) a->timers->section0 += ms * 1e-3;
-        cudaEventDestroy(e0);
-        cudaEventDestroy(e1);
-    }
-    if (e != cudaSuccess) { set_error("b2_linear_forward: %s", cudaGetErrorString(e)); return B2_ERR_LAUNCH; }
-    return B2_OK;
+    return loop_finish("b2_linear_forward", a->timers);
 }
 
 extern "C" int b2_linear_forward(const struct b2_linear_args *a) {

@@ -38,47 +38,19 @@ static int sa_forward_body(const b2_sa_args *a, Staging &st) {
                     set_error("b2_sa_forward: b, vp and damp must have the allocated space layout of u");
                     return B2_ERR_INVALID;
                 }
-    if ((rc = sparse_stage_in(st, a->src, nd, false, src))) return rc;
-    if ((rc = sparse_stage_in(st, a->rec, nd, true, rec))) return rc;
-    // devito/operations/interpolators.py:28-37 `check_radius`
-    if ((src.present && src.r > so) || (rec.present && rec.r > so)) {
-        set_error("b2_sa_forward: sparse radius %d exceeds the halo (space_order %d)",
-                  src.present && src.r > so ? src.r : rec.r, so);
-        return B2_ERR_INVALID;
-    }
+    if ((rc = sparse_stage_pair("b2_sa_forward", st, a->src, a->rec, nd, so, src, rec))) return rc;
 
-    // ---- geometry in the internal 3-dim convention ----
     SaPlan p;
-    const int lo_in[3] = {a->x_m, a->y_m, a->z_m};
-    const int hi_in[3] = {a->x_M, a->y_M, a->z_M};
-    p.tsize = u->size[0];
-    p.so = so;
-    for (int d = 0; d < 3; ++d) {
-        const int di = d - (3 - nd);          // the grid's dim, or < 0 for the dummy leading dim of a 2-D grid
-        if (di < 0) {
-            p.a[d] = 1; p.n[d] = 1; p.o[d] = 0; p.radius[d] = 0;
-            continue;
-        }
-        p.a[d] = u->size[di + 1];
-        p.n[d] = hi_in[di] - lo_in[di] + 1;
-        p.o[d] = lo_in[di] + so;
+    static_cast<Box &>(p) = make_box(a, nd, u->size, so);
+    for (int di = 0; di < nd; ++di) {
+        const int d = 3 - nd + di;
         p.radius[d] = a->radius;
         if (!a->c[di]) { set_error("b2_sa_forward: weights for dim %d missing", di); return B2_ERR_INVALID; }
         for (int i = 0; i < a->radius; ++i) p.c[d][i] = a->c[di][i];
     }
-    for (int d = 0; d < 3; ++d) {
-        if (p.n[d] <= 0) return B2_OK;
-        // the nested stencil reaches 2R-1 points; b is read over [p-R, p+R-1]
-        const int rd = p.radius[d] ? 2 * p.radius[d] - 1 : 0;
-        if (p.o[d] - rd < 0 || p.o[d] + p.n[d] - 1 + rd >= p.a[d]) {
-            set_error("b2_sa_forward: iteration range + radius %d leaves the allocated array (extent %d) on dim %d",
-                      rd, p.a[d], d - (3 - nd));
-            return B2_ERR_INVALID;
-        }
-    }
-    p.sy = p.a[2];
-    p.sx = (long long)p.a[1] * p.a[2];
-    p.slot_elems = (size_t)p.a[0] * p.a[1] * p.a[2];
+    // the nested stencil reaches 2R-1 points; b is read over [p-R, p+R-1]
+    bool empty;
+    if ((rc = check_reach("b2_sa_forward", p, nd, 2 * a->radius - 1, empty)) || empty) return rc;
     p.u = (float *)u->d;
     p.b_arr = b ? (const float *)b->d : nullptr;
     p.vp_arr = vp ? (const float *)vp->d : nullptr;
@@ -93,24 +65,9 @@ static int sa_forward_body(const b2_sa_args *a, Staging &st) {
     }
     if ((rc = sa_plan_init(p, a->kernel))) return rc;
 
-    FieldGeom g;
-    g.sx = p.sx;
-    g.sy = p.sy;
-    g.slot_elems = p.slot_elems;
-    g.so = so;
-    g.ndim = nd;
-    for (int d = 0; d < nd; ++d) { g.lo[d] = lo_in[d]; g.hi[d] = hi_in[d]; }
-
+    const FieldGeom g = field_geom(p, nd);
     const int T = p.tsize;
-    static cudaEvent_t e0 = nullptr, e1 = nullptr;      // created once (the process is bound to one device)
-    if (a->timers) {
-        if (!e0 && (cudaEventCreate(&e0) != cudaSuccess || cudaEventCreate(&e1) != cudaSuccess)) {
-            e0 = e1 = nullptr;
-            set_error("b2_sa_forward: cannot create timing events");
-            return B2_ERR_DEVICE;
-        }
-        cudaEventRecord(e0, stream());
-    }
+    if ((rc = loop_timer_start(a->timers))) return rc;
     const bool adj = p.adjoint;
     const int dir = adj ? -1 : 1;
     for (int time = adj ? a->time_M : a->time_m; adj ? time >= a->time_m : time <= a->time_M; time += dir) {
@@ -122,24 +79,11 @@ static int sa_forward_body(const b2_sa_args *a, Staging &st) {
         if ((rc = launch_inject(src, g, f1, nullptr, time, B2_SCALE_TABLE, p.C, 0.f, 0.f))) return rc;
         if ((rc = launch_interp(rec, g, p.u + (size_t)(a->rec_toff ? t1 : t0) * p.slot_elems, nullptr, time)))
             return rc;
-        if (a->errctl && ((time - a->time_m) % 100 == 99 || time == (adj ? a->time_m : a->time_M))) {
-            bool bad = false;
-            if ((rc = check_finite(f1, p.slot_elems, bad))) return rc;
-            if (bad) { set_error("NaN/Inf detected in u at time=%d", time); return B2_ERR_NAN; }
-        }
+        if (a->errctl && errctl_due(time, a->time_m, adj ? a->time_m : a->time_M) &&
+            (rc = check_finite(f1, p.slot_elems, "u", time)))
+            return rc;
     }
-    if (a->timers) cudaEventRecord(e1, stream());
-    cudaError_t e = cudaStreamSynchronize(stream());
-    if (e != cudaSuccess) {
-        set_error("b2_sa_forward: device error: %s", cudaGetErrorString(e));
-        return B2_ERR_LAUNCH;
-    }
-    if (a->timers) {
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, e0, e1);
-        a->timers->section0 += ms * 1e-3;
-    }
-    return B2_OK;
+    return loop_finish("b2_sa_forward", a->timers);
 }
 
 extern "C" int b2_sa_forward(const struct b2_sa_args *a) {

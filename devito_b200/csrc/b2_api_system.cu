@@ -60,15 +60,14 @@ static int system_forward_body(const b2_system_args *a, Staging &staging) {
         for (int d = 1; d <= nd; ++d)
             if (F[i]->size[d] != F[0]->size[d]) { set_error("b2_system_forward: field %d has another shape", i); return B2_ERR_INVALID; }
     }
-    const Box3 b = box3(a, nd, &F[0]->size[1], h);
-    const int *alloc = b.alloc, *lo = b.lo, *hi = b.hi, *hal = b.hal;
+    const Box b = make_box(a, nd, F[0]->size, h);
     int calloc_[3] = {1, 1, 1};
     for (int i = 0; i < a->ncoefs; ++i) {
         if ((rc = staging.array(a->coefs[i], nd, false, C[i]))) return rc;
         for (int d = 0; d < nd; ++d) {
             const int di = 3 - nd + d;
             if (i == 0) calloc_[di] = C[i]->size[d];
-            if (C[i]->size[d] != calloc_[di] || C[i]->size[d] != alloc[di] - 2 * hal[di]) {
+            if (C[i]->size[d] != calloc_[di] || C[i]->size[d] != b.a[di] - 2 * h) {
                 set_error("b2_system_forward: coefficient array %d does not have the grid's shape", i);
                 return B2_ERR_INVALID;
             }
@@ -90,12 +89,12 @@ static int system_forward_body(const b2_system_args *a, Staging &staging) {
         if ((rc = sparse_stage_in(staging, a->interp[i].s, nd, true, itp[i]))) return rc;
 
     SysK k;
-    k.sy = alloc[2];
-    k.sx = (long long)alloc[1] * alloc[2];
+    k.sy = b.sy;
+    k.sx = b.sx;
     k.csy = calloc_[2];
     k.csx = (long long)calloc_[1] * calloc_[2];
-    const size_t slot_len = (size_t)alloc[0] * alloc[1] * alloc[2];
-    if (hi[0] < lo[0] || hi[1] < lo[1] || hi[2] < lo[2]) return B2_OK;
+    const size_t slot_len = b.slot_elems;
+    if (b.n[0] <= 0 || b.n[1] <= 0 || b.n[2] <= 0) return B2_OK;
     for (int i = 0; i < a->ncoefs; ++i) k.cf[i] = (const float *)C[i]->d;
     for (int i = a->ncoefs; i < B2_SYS_MAX_COEFS; ++i) k.cf[i] = nullptr;
     auto slot_of = [&](int f, int time, int shift) { return slot(time + shift, F[f]->size[0]); };
@@ -124,16 +123,14 @@ static int system_forward_body(const b2_system_args *a, Staging &staging) {
             }
             for (int d = 0; d < nd; ++d) {
                 const int di = 3 - nd + d;
-                if (lo[di] - st.ext + hal[di] + t.off[d] < 0 || hi[di] + st.ext + hal[di] + t.off[d] >= alloc[di]) {
+                if (b.o[di] - st.ext + t.off[d] < 0 || b.o[di] + b.n[di] - 1 + st.ext + t.off[d] >= b.a[di]) {
                     set_error("b2_system_forward: stage %d tap offset %d on dim %d leaves the allocated array", s, t.off[d], d);
                     return B2_ERR_INVALID;
                 }
             }
         }
     }
-    FieldGeom g;
-    g.sx = k.sx; g.sy = k.sy; g.slot_elems = slot_len; g.so = h; g.ndim = nd;
-    for (int d = 0; d < nd; ++d) { g.lo[d] = lo[3 - nd + d]; g.hi[d] = hi[3 - nd + d]; }
+    const FieldGeom g = field_geom(b, nd);
 
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     double sec[3] = {0, 0, 0};
@@ -151,9 +148,10 @@ static int system_forward_body(const b2_system_args *a, Staging &staging) {
             const b2_sys_stage &st = a->stages[s];
             // the box, widened by ext on the space axes (internal axis 0 of a 2-D grid is the dummy extent 1)
             const int e0 = nd == 3 ? st.ext : 0, e = st.ext;
-            k.n0 = hi[0] - lo[0] + 1 + 2 * e0; k.n1 = hi[1] - lo[1] + 1 + 2 * e; k.n2 = hi[2] - lo[2] + 1 + 2 * e;
-            k.o0 = lo[0] - e0 + hal[0]; k.o1 = lo[1] - e + hal[1]; k.o2 = lo[2] - e + hal[2];
-            k.c0 = lo[0] - e0; k.c1 = lo[1] - e; k.c2 = lo[2] - e;       // unused when e > 0 (no cfield)
+            k.n0 = b.n[0] + 2 * e0; k.n1 = b.n[1] + 2 * e; k.n2 = b.n[2] + 2 * e;
+            k.o0 = b.o[0] - e0; k.o1 = b.o[1] - e; k.o2 = b.o[2] - e;
+            // the coefficient arrays have no halo (unused when e > 0: no cfield)
+            k.c0 = nd == 3 ? k.o0 - h : 0; k.c1 = k.o1 - h; k.c2 = k.o2 - h;
             const dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
             k.out = (float *)F[st.out_field]->d + (size_t)slot_of(st.out_field, time, st.out_tshift) * slot_len;
             for (int f = 0; f < a->nfields; ++f)
@@ -195,8 +193,7 @@ static int system_forward_body(const b2_system_args *a, Staging &staging) {
         if (per_step) rec_ev();
     }
     if (timing && !per_step) cudaEventRecord(ev[1], stream());
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream());
+    rc = sync_call("b2_system_forward");
     if (timing) {
         float ms = 0.f;
         if (per_step) {
@@ -205,7 +202,7 @@ static int system_forward_body(const b2_system_args *a, Staging &staging) {
                 if (cudaEventElapsedTime(&ms, pool[i + 1], pool[i + 2]) == cudaSuccess) sec[1] += ms;
                 if (cudaEventElapsedTime(&ms, pool[i + 2], pool[i + 3]) == cudaSuccess) sec[2] += ms;
             }
-        } else if (e == cudaSuccess && cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) {
+        } else if (rc == B2_OK && cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) {
             sec[0] = ms;
         }
         a->timers->section0 += sec[0] * 1e-3;
@@ -214,8 +211,7 @@ static int system_forward_body(const b2_system_args *a, Staging &staging) {
         for (auto &x : ev) cudaEventDestroy(x);
         for (auto &x : pool) cudaEventDestroy(x);
     }
-    if (e != cudaSuccess) { set_error("b2_system_forward: %s", cudaGetErrorString(e)); return B2_ERR_LAUNCH; }
-    return B2_OK;
+    return rc;
 }
 
 extern "C" int b2_system_forward(const struct b2_system_args *a) {

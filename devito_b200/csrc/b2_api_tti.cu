@@ -26,7 +26,6 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
              *usave = nullptr, *vsave = nullptr;
     SparseDev src, rec;
     TtiPlan p, pd, pa;
-    FieldGeom g;
 
     if ((rc = st.array(a->u, nd + 1, true, u))) return rc;
     if ((rc = st.array(a->v, nd + 1, true, v))) return rc;
@@ -84,40 +83,15 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
             (gh = grid_halo("b2_tti_forward", "grad", a->grad, *grad, 0, *u, nd, so)) < 0)
             return B2_ERR_INVALID;
     }
-    if ((rc = sparse_stage_in(st, a->src, nd, false, src))) return rc;
-    if ((rc = sparse_stage_in(st, a->rec, nd, true, rec))) return rc;
-    // devito/operations/interpolators.py:28-37 `check_radius`
-    if ((src.present && src.r > so) || (rec.present && rec.r > so)) {
-        set_error("b2_tti_forward: sparse radius %d exceeds the halo (space_order %d)",
-                  src.present && src.r > so ? src.r : rec.r, so);
-        return B2_ERR_INVALID;
-    }
+    if ((rc = sparse_stage_pair("b2_tti_forward", st, a->src, a->rec, nd, so, src, rec))) return rc;
 
-    const int lo_in[3] = {a->x_m, a->y_m, a->z_m};
-    const int hi_in[3] = {a->x_M, a->y_M, a->z_M};
+    static_cast<Box &>(p) = make_box(a, nd, u->size, so);
+    bool empty;
+    if ((rc = check_reach("b2_tti_forward", p, nd, a->radius, empty)) || empty) return rc;
+    for (int d = 1; d <= nd; ++d)
+        if (v->size[d] != u->size[d]) { set_error("b2_tti_forward: u and v shapes differ"); return B2_ERR_INVALID; }
     p.ndim = nd;
     p.R = a->radius;
-    p.so = so;
-    p.tsize = u->size[0];
-    for (int d = 0; d < 3; ++d) {
-        const int di = d - (3 - nd);          // the grid's dim, or < 0 for the dummy leading dim of a 2-D grid
-        if (di < 0) {
-            p.a[d] = 1; p.n[d] = 1; p.o[d] = 0;
-            continue;
-        }
-        p.a[d] = u->size[di + 1];
-        p.n[d] = hi_in[di] - lo_in[di] + 1;
-        p.o[d] = lo_in[di] + so;
-        if (p.n[d] <= 0) return B2_OK;
-        if (v->size[di + 1] != p.a[d]) { set_error("b2_tti_forward: u and v shapes differ"); return B2_ERR_INVALID; }
-        if (p.o[d] - p.R < 0 || p.o[d] + p.n[d] - 1 + p.R >= p.a[d]) {
-            set_error("b2_tti_forward: iteration range + radius leaves the allocated array on dim %d", d);
-            return B2_ERR_INVALID;
-        }
-    }
-    p.sy = p.a[2];
-    p.sx = (long long)p.a[1] * p.a[2];
-    p.slot_elems = (size_t)p.a[0] * p.a[1] * p.a[2];
     p.u = (float *)u->d;
     p.v = (float *)v->d;
     p.damp = damp ? (const float *)damp->d : nullptr;
@@ -146,31 +120,17 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
         if (adj && (rc = tti_plan_adjoint(p, pa))) return rc;
     }
 
-    g.sx = p.sx;
-    g.sy = p.sy;
-    g.slot_elems = p.slot_elems;
-    g.so = so;
-    g.ndim = nd;
-    for (int d = 0; d < nd; ++d) { g.lo[d] = lo_in[d]; g.hi[d] = hi_in[d]; }
+    const FieldGeom g = field_geom(p, nd, a->halo);
     DevArray grad3;                             // grad with the plan's (dummy, x, z) extents on a 2-D grid
     if (grad) {
         grad3 = *grad;
         if (nd == 2) { grad3.size[0] = 1; grad3.size[1] = grad->size[0]; grad3.size[2] = grad->size[1]; }
     }
-    if (a->halo) { g.nb_lo = a->halo->rank > 0; g.nb_hi = a->halo->rank < a->halo->nranks - 1; }
 
     const float dt2 = a->dt * a->dt;
     const float scalar_scale = dt2 * a->vp * a->vp;
     const int T = p.tsize;
-    static cudaEvent_t e0 = nullptr, e1 = nullptr;      // created once (the process is bound to one device)
-    if (a->timers) {
-        if (!e0 && (cudaEventCreate(&e0) != cudaSuccess || cudaEventCreate(&e1) != cudaSuccess)) {
-            e0 = e1 = nullptr;
-            set_error("b2_tti_forward: cannot create timing events");
-            return B2_ERR_DEVICE;
-        }
-        cudaEventRecord(e0, stream());
-    }
+    if ((rc = loop_timer_start(a->timers))) return rc;
     const bool p2p = a->halo && halo_p2p_active(a->halo, p.u) && halo_p2p_active(a->halo, p.v);
     if (a->halo) a->halo->reset_primed();
     const int dir = adj ? -1 : 1;
@@ -219,29 +179,13 @@ static int tti_forward_body(const b2_tti_args *a, Staging &st) {
                                      (const float *)vsave->d + (size_t)time * p.slot_elems, p.v, t0, t1, t2)))
                 return rc;
         }
-        if (a->errctl && ((time - a->time_m) % 100 == 99 || time == (adj ? a->time_m : a->time_M))) {
-            bool bad = false;
-            if ((rc = check_finite(fu, p.slot_elems, bad))) return rc;
-            if (bad) { set_error("NaN/Inf detected in u at time=%d", time); return B2_ERR_NAN; }
-            if (born) {
-                if ((rc = check_finite(pd.u + (size_t)t1 * p.slot_elems, p.slot_elems, bad))) return rc;
-                if (bad) { set_error("NaN/Inf detected in du at time=%d", time); return B2_ERR_NAN; }
-            }
+        if (a->errctl && errctl_due(time, a->time_m, adj ? a->time_m : a->time_M)) {
+            if ((rc = check_finite(fu, p.slot_elems, "u", time))) return rc;
+            if (born && (rc = check_finite(pd.u + (size_t)t1 * p.slot_elems, p.slot_elems, "du", time))) return rc;
         }
     }
     if (a->halo && (rc = halo_p2p_drain(a->halo))) return rc;
-    if (a->timers) cudaEventRecord(e1, stream());
-    cudaError_t e = cudaStreamSynchronize(stream());
-    if (e != cudaSuccess) {
-        set_error("b2_tti_forward: device error: %s", cudaGetErrorString(e));
-        return B2_ERR_LAUNCH;
-    }
-    if (a->timers) {
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, e0, e1);
-        a->timers->section0 += ms * 1e-3;
-    }
-    return B2_OK;
+    return loop_finish("b2_tti_forward", a->timers);
 }
 
 extern "C" int b2_tti_forward(const struct b2_tti_args *a) {

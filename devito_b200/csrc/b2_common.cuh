@@ -130,8 +130,20 @@ class Staging {
 int grid_halo(const char *who, const char *name, const b2_dataobj *obj, const DevArray &x, int lead,
               const DevArray &u, int nd, int so, int need = -1);
 
-// NaN/Inf check of n floats (reference: errctl='max', passes/iet/errors.py:59-85); waits for the result
-int check_finite(const float *f, size_t n, bool &bad);
+// errctl (reference: errctl='max', passes/iet/errors.py:59-85): the wavefields are checked every 100th step of the
+// loop over [first, ...] and after its `last` step
+inline bool errctl_due(int time, int first, int last) { return (time - first) % 100 == 99 || time == last; }
+// NaN/Inf check of n floats of `field`, written at step `time`: B2_ERR_NAN after set_error when one is found. Waits for
+// the result.
+int check_finite(const float *f, size_t n, const char *field, int time);
+
+// Waits for the work the call queued: a launch or device error sets "<who>: device error: ..." and gives
+// B2_ERR_LAUNCH.
+int sync_call(const char *who);
+// The end of a call whose timers report the time loop as section0 only: loop_timer_start() before the loop,
+// loop_finish() after it synchronises (sync_call) and adds the loop's time to timers->section0. Null timers: no timing.
+int loop_timer_start(b2_profiler *timers);
+int loop_finish(const char *who, b2_profiler *timers);
 
 // Imaging condition over the iterated box, after the step and its injection (k_imaging, b2_runtime.cu):
 // grad -= us * (v1 - 2 v0 + v2) / dt^2, and with us2 != nullptr also - us2 * (w1 - 2 w0 + w2) / dt^2 (the TTI
@@ -174,23 +186,53 @@ int launch_imaging(const Plan &p, const DevArray &grad, int gh, const float *us,
     return launch_imaging(k);
 }
 
-// The iteration box of a linear / system call (`a`: x_m .. z_M) in the internal 3-dim convention: a 1-D or 2-D
-// grid gets leading dummy dims of extent 1. `size` = the allocated space extents, `h` the halo.
-struct Box3 {
-    int alloc[3] = {1, 1, 1}, lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0}, hal[3] = {0, 0, 0};
+// The iteration box of a call (x_m .. z_M) in the internal 3-dim convention: a 1-D or 2-D grid gets leading dummy
+// dims of extent 1 (origin 0). The plans of the wave entry points derive from it.
+struct Box {
+    int a[3] = {1, 1, 1};        // allocated extents
+    int n[3] = {1, 1, 1};        // iteration extents (<= 0: nothing to do)
+    int o[3] = {0, 0, 0};        // array index of the first iterated point
+    long long sx = 0, sy = 0;    // element strides of dim0 / dim1 (dim2 stride = 1)
+    size_t slot_elems = 0;       // elements of one time slot
+    int tsize = 3;               // time slots
+    int so = 0;                  // halo on every grid dim
 };
+
+// The box of `args` on an `nd`-dim grid (1..3) whose field has the extents `size` (time slots, then the space
+// extents) and the halo `halo` on every space dim.
 template <class Args>
-Box3 box3(const Args *a, int nd, const int *size, int h) {
-    const int lo_in[3] = {a->x_m, a->y_m, a->z_m}, hi_in[3] = {a->x_M, a->y_M, a->z_M};
-    Box3 b;
+Box make_box(const Args *args, int nd, const int *size, int halo) {
+    const int lo[3] = {args->x_m, args->y_m, args->z_m}, hi[3] = {args->x_M, args->y_M, args->z_M};
+    Box b;
+    b.tsize = size[0];
+    b.so = halo;
     for (int d = 0; d < nd; ++d) {
         const int di = 3 - nd + d;
-        b.alloc[di] = size[d];
-        b.lo[di] = lo_in[d];
-        b.hi[di] = hi_in[d];
-        b.hal[di] = h;
+        b.a[di] = size[d + 1];
+        b.n[di] = hi[d] - lo[d] + 1;
+        b.o[di] = lo[d] + halo;
     }
+    b.sy = b.a[2];
+    b.sx = (long long)b.a[1] * b.a[2];
+    b.slot_elems = (size_t)b.a[0] * b.a[1] * b.a[2];
     return b;
+}
+
+// A wave call's box against its allocation, internal dim 0, 1, 2 in turn: an empty extent sets `empty` (the call has
+// nothing to do), a box grown by `reach` cells on either side of a grid dim that leaves [0, a) refuses the call
+// (B2_ERR_INVALID after set_error naming `who`). `reach`: how far the stencil reads beyond the point it updates.
+inline int check_reach(const char *who, const Box &b, int nd, int reach, bool &empty) {
+    empty = false;
+    for (int d = 0; d < 3; ++d) {
+        if (b.n[d] <= 0) { empty = true; return B2_OK; }
+        if (d < 3 - nd) continue;                               // a dummy dim: extent 1, nothing read around it
+        if (b.o[d] - reach < 0 || b.o[d] + b.n[d] - 1 + reach >= b.a[d]) {
+            set_error("%s: iteration range [%d,%d] + reach %d leaves the allocated array (extent %d) on dim %d", who,
+                      b.o[d] - b.so, b.o[d] - b.so + b.n[d] - 1, reach, b.a[d], d - (3 - nd));
+            return B2_ERR_INVALID;
+        }
+    }
+    return B2_OK;
 }
 
 }  // namespace b2

@@ -4,16 +4,9 @@
 
 namespace b2 {
 
-struct IsoPlan {
-    // geometry (internal dims are always 3: for 2-D grids dim 0 is a dummy of extent 1)
+// The box: internal dims are always 3, for 2-D grids dim 0 is a dummy of extent 1 (radius 0).
+struct IsoPlan : Box {
     int radius[3] = {0, 0, 0};
-    int so = 0;
-    int a[3] = {1, 1, 1};        // allocated extents
-    int n[3] = {1, 1, 1};        // iteration extents
-    int o[3] = {0, 0, 0};        // array index of the first iterated point
-    long long sx = 0, sy = 0;    // element strides of dim0 / dim1 (dim2 stride = 1)
-    size_t slot_elems = 0;
-    int tsize = 3;
     float *u = nullptr;
     const float *damp = nullptr;
     const float *param = nullptr;

@@ -234,7 +234,7 @@ __global__ void k_check_finite(const float *__restrict__ f, size_t n, int *flag)
     if (bad) atomicOr(flag, 1);
 }
 
-int check_finite(const float *f, size_t n, bool &bad) {
+int check_finite(const float *f, size_t n, const char *field, int time) {
     static int *d_flag = nullptr;
     if (!d_flag) B2_CUDA(cudaMalloc(&d_flag, sizeof(int)), B2_ERR_MEMORY);
     B2_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), stream()), B2_ERR_MEMORY);
@@ -244,7 +244,37 @@ int check_finite(const float *f, size_t n, bool &bad) {
     int h = 0;
     B2_CUDA(cudaMemcpyAsync(&h, d_flag, sizeof(int), cudaMemcpyDeviceToHost, stream()), B2_ERR_MEMORY);
     B2_CUDA(cudaStreamSynchronize(stream()), B2_ERR_DEVICE);
-    bad = h != 0;
+    if (h) { set_error("NaN/Inf detected in %s at time=%d", field, time); return B2_ERR_NAN; }
+    return B2_OK;
+}
+
+int sync_call(const char *who) {
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream());
+    if (e != cudaSuccess) {
+        set_error("%s: device error: %s", who, cudaGetErrorString(e));
+        return B2_ERR_LAUNCH;
+    }
+    return B2_OK;
+}
+
+static cudaEvent_t g_loop_ev[2] = {nullptr, nullptr};     // created once (the process is bound to one device)
+
+int loop_timer_start(b2_profiler *timers) {
+    if (!timers) return B2_OK;
+    if (!g_loop_ev[1]) {
+        B2_CUDA(cudaEventCreate(&g_loop_ev[0]), B2_ERR_DEVICE);
+        B2_CUDA(cudaEventCreate(&g_loop_ev[1]), B2_ERR_DEVICE);
+    }
+    B2_CUDA(cudaEventRecord(g_loop_ev[0], stream()), B2_ERR_DEVICE);
+    return B2_OK;
+}
+
+int loop_finish(const char *who, b2_profiler *timers) {
+    if (timers) B2_CUDA(cudaEventRecord(g_loop_ev[1], stream()), B2_ERR_DEVICE);
+    if (int rc = sync_call(who)) return rc;
+    float ms = 0.f;
+    if (timers && cudaEventElapsedTime(&ms, g_loop_ev[0], g_loop_ev[1]) == cudaSuccess) timers->section0 += ms * 1e-3;
     return B2_OK;
 }
 

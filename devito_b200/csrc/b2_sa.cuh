@@ -4,16 +4,9 @@
 
 namespace b2 {
 
-struct SaPlan {
-    // geometry, internal 3-dim convention (a 2-D grid is (1, x, y) with radius 0 on dim 0)
-    int a[3];                        // allocated extents
-    int n[3];                        // iteration extents
-    int o[3];                        // array index of the first iterated point
-    int radius[3];
-    int so = 0;
-    long long sx = 0, sy = 0;
-    size_t slot_elems = 0;
-    int tsize = 0;
+// The box: a 2-D grid is (1, x, y) with radius 0 on dim 0.
+struct SaPlan : Box {
+    int radius[3] = {0, 0, 0};
     float *u = nullptr;
     float c[3][B2_MAX_RADIUS] = {};
     float dt = 0.f;

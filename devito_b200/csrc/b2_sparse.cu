@@ -10,6 +10,7 @@
 // devito/passes/iet/languages/openacc.py:79-80). One warp handles one point; lanes stride over
 // the (2r)^ndim support cells; interpolation reduces with warp shuffles.
 #include "b2_sparse.cuh"
+#include "b2_halo.cuh"
 #include <climits>
 
 namespace b2 {
@@ -200,6 +201,35 @@ int sparse_stage_in(Staging &st, const b2_sparse *s, int ndim, bool written, Spa
     out.ndim = ndim;
     out.present = true;
     return B2_OK;
+}
+
+int sparse_stage_pair(const char *who, Staging &st, const b2_sparse *src, const b2_sparse *rec, int ndim, int so,
+                      SparseDev &src_out, SparseDev &rec_out) {
+    int rc;
+    if ((rc = sparse_stage_in(st, src, ndim, false, src_out))) return rc;
+    if ((rc = sparse_stage_in(st, rec, ndim, true, rec_out))) return rc;
+    const bool src_far = src_out.present && src_out.r > so, rec_far = rec_out.present && rec_out.r > so;
+    if (src_far || rec_far) {
+        set_error("%s: sparse radius %d exceeds the halo (space_order %d)", who, src_far ? src_out.r : rec_out.r, so);
+        return B2_ERR_INVALID;
+    }
+    return B2_OK;
+}
+
+FieldGeom field_geom(const Box &b, int nd, const b2_halo_ctx *halo) {
+    FieldGeom g;
+    g.sx = b.sx;
+    g.sy = b.sy;
+    g.slot_elems = b.slot_elems;
+    g.so = b.so;
+    g.ndim = nd;
+    for (int d = 0; d < nd; ++d) {
+        const int di = 3 - nd + d;
+        g.lo[d] = b.o[di] - b.so;
+        g.hi[d] = g.lo[d] + b.n[di] - 1;
+    }
+    if (halo) { g.nb_lo = halo->rank > 0; g.nb_hi = halo->rank < halo->nranks - 1; }
+    return g;
 }
 
 int launch_inject(const SparseDev &s, const FieldGeom &g, float *f0, float *f1, int time,

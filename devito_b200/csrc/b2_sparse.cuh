@@ -15,7 +15,7 @@ struct SparseDev {
     int ndim = 3;
 };
 
-// Field geometry the sparse kernels need (internal 3-dim convention, see IsoPlan)
+// Field geometry the sparse kernels need (strides in the internal 3-dim convention of Box; bounds per grid dim)
 struct FieldGeom {
     long long sx = 0, sy = 0;
     size_t slot_elems = 0;
@@ -42,6 +42,14 @@ struct FieldGeom {
 // Checks the tables of `s` (radius, gp, the ndim weight tables, the point range against the traces) and only then
 // stages them into `st`; `written`: the traces are copied back (receivers). `out.present` stays false without points.
 int sparse_stage_in(Staging &st, const b2_sparse *s, int ndim, bool written, SparseDev &out);
+// The sources and receivers (written back) of a wave call; the support of a point reaches r cells beyond the box, so
+// an r beyond the halo `so` refuses the call (devito/operations/interpolators.py:28-37 `check_radius`).
+int sparse_stage_pair(const char *who, Staging &st, const b2_sparse *src, const b2_sparse *rec, int ndim, int so,
+                      SparseDev &src_out, SparseDev &rec_out);
+
+// The geometry of box b on an `nd`-dim grid; under x-slab decomposition (`halo`) the cells beyond x_m / x_M
+// belong to the neighbours.
+FieldGeom field_geom(const Box &b, int nd, const b2_halo_ctx *halo = nullptr);
 
 // Internal param_kind of launch_inject: the scale is a tabulated array in the field's layout, taken at the cell
 // (the self-adjoint update's C = dt^2 vp^2 / b). Not part of the C ABI.

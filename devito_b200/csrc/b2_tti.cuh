@@ -6,16 +6,9 @@ namespace b2 {
 
 // A 2-D grid (x, z) is planned as (1, x, z): extent 1 and no stencil taps on the leading dim, rotation factors
 // (0, sin theta, cos theta). Its sweeps march along the grid's x, the plan's dim 1.
-struct TtiPlan {
+struct TtiPlan : Box {
     int ndim = 3;                // 2 or 3
     int R = 4;                   // radius = space_order/2 (even)
-    int so = 8;
-    int a[3] = {1, 1, 1};
-    int n[3] = {1, 1, 1};
-    int o[3] = {0, 0, 0};
-    long long sx = 0, sy = 0;
-    size_t slot_elems = 0;
-    int tsize = 3;
     float *u = nullptr, *v = nullptr;
     const float *damp = nullptr;
     float vp = 1.f, dt = 1.f, epsilon = 0.f, delta = 0.f, theta = 0.f, phi = 0.f;
