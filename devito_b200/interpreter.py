@@ -26,9 +26,21 @@ class _Env:
         self.shape = shape
 
 
+def _subsampled(f):
+    """The factor of a function saved on a time ConditionalDimension (snapshots), else None."""
+    td = getattr(f, 'time_dim', None)
+    if getattr(f, 'is_buffered', True) or not getattr(td, 'is_Conditional', False) or not td.factor:
+        return None
+    return int(td.factor)
+
+
 def _time_index(f, idx, time):
     if idx.absolute is not None:
         return idx.absolute
+    fac = _subsampled(f)
+    if fac is not None:
+        # usave[t_sub + shift] with t_sub = time / factor
+        return time // fac + int(idx.shift)
     t = time + int(idx.shift)
     if getattr(f, 'is_buffered', False):
         return t % f.time_size
@@ -350,6 +362,9 @@ class Interpreter:
         for time in steps:
             for kind, _, obj, lhs, rhs in self.items:
                 if kind == 'eq':
+                    fac = _subsampled(lhs.function) if lhs.is_Access else None
+                    if fac is not None and time % fac:
+                        continue            # a snapshot is written where time % factor == 0 only
                     self._run_eq(obj, lhs, rhs, time, scalars, bounds)
                 elif kind == 'inject':
                     self._run_inject(obj, time, scalars, bounds)

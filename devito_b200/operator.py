@@ -30,7 +30,7 @@ from .symbolics import (Number, Add, Mul, Pow, Call, as_expr, linear_terms, NonL
 from .types import Function, TimeFunction, Constant
 from .sparse import Injection, Interpolation, SparseTimeFunction
 from .equation import Eq, FreeSurface
-from .interpreter import Interpreter
+from .interpreter import Interpreter, _subsampled
 from .parameters import configuration
 from .exceptions import InvalidArgument, ExecutionError, InvalidOperator
 from .logger import perf, warning
@@ -194,10 +194,10 @@ class Entry(NamedTuple):
     host_io: tuple          # members that may come with the caller's device buffer (struct b2_iso_args.host_io)
 
 
-_OVERRIDE_KINDS = {'wavefield': "a TimeFunction of the wavefield's space order on the same grid",
-                   'saved': "a saved TimeFunction (save=nt) of the wavefield's space order",
-                   'snapshot': "a saved TimeFunction on the same grid",
-                   'function': "a Function or an array of its allocated shape"}
+_OVERRIDE_KINDS = {'wavefield': "a float32 TimeFunction of the wavefield's space order on the same grid",
+                   'saved': "a float32 saved TimeFunction (save=nt) of the wavefield's space order",
+                   'snapshot': "a float32 saved TimeFunction on the same grid",
+                   'function': "a float32 Function or an array of its allocated shape"}
 
 
 def wave_entry(p):
@@ -288,12 +288,40 @@ class Operator:
 
     def _recognise(self):
         try:
-            return self._recognise_wave()
+            plan = self._recognise_wave()
         except _Unrecognised as wave_why:
             try:
-                return self._recognise_linear()
+                plan = self._recognise_linear()
             except _Unrecognised as lin_why:
                 raise _Unrecognised(f"{wave_why}; as a generic constant-coefficient update: {lin_why}") from None
+        self._check_dtypes(plan)
+        return plan
+
+    # the plan members that are arrays the library reads or writes
+    _ARRAY_MEMBERS = ('u', 'v', 'damp', 'snap', 'born_U', 'born_du', 'born_dv', 'born_dm', 'grad', 'usave', 'vsave')
+
+    @classmethod
+    def _check_dtypes(cls, plan):
+        """The kernels read and write float32 only: a plan whose grid, fields, parameter Functions, saved
+        fields or sparse traces and coordinates are of another dtype is not theirs to run."""
+        objs = [plan[k] for k in cls._ARRAY_MEMBERS if plan.get(k) is not None]
+        for k in ('m_role', 'b_role', 'vp_role'):
+            if plan.get(k) is not None:
+                objs.append(plan[k][1])
+        objs += list(plan.get('consts', {}).values())
+        objs = [o for o in objs if isinstance(o, Function)]
+        if np.dtype(plan['grid'].dtype) != np.float32:
+            raise _Unrecognised(f"the grid is {np.dtype(plan['grid'].dtype).name}; the kernels compute in float32")
+        for o in objs:
+            if np.dtype(o.dtype) != np.float32:
+                raise _Unrecognised(f"`{o.name}` is {np.dtype(o.dtype).name}; the kernels read float32 arrays")
+        for sf in (plan.get('src'), plan.get('rec')):
+            if sf is None:
+                continue
+            for what, dt in (('traces', sf.dtype), ('coordinates', sf.coordinates_data.dtype)):
+                if np.dtype(dt) != np.float32:
+                    raise _Unrecognised(f"the {what} of `{sf.name}` are {np.dtype(dt).name}; the kernels read "
+                                        "float32 sparse data")
 
     def _recognise_linear(self):
         """A single explicit update `f.forward|backward = sum_k c_k f[t + s_k][p + o_k]` whose
@@ -949,26 +977,30 @@ class Operator:
                     raise _Unrecognised("injection must target the updated time level")
                 ex = ex.evaluate.subs(self._subs) if self._subs else ex.evaluate
                 f2, c2, s2 = self._leaves([ex])
+                if not any(acc.function is sf for acc in f2):
+                    raise _Unrecognised("injected expression does not contain the source")
+                literal = dtsym.name not in {s.name for s in s2}
+                lits = []
                 for probe in range(2):
-                    vals, leaf = self._probe_env(rng, f2, c2, s2, grid)
-                    srcv = None
-                    for acc in f2:
-                        if acc.function is sf:
-                            srcv = vals[('f', id(sf))]
-                    if srcv is None:
-                        raise _Unrecognised("injected expression does not contain the source")
+                    # the update's leaves are in scope too, so that the role of m always has a value
+                    # (an expression without m must then fail the comparison, not the lookup)
+                    vals, leaf = self._probe_env(rng, list(funcs) + f2, list(consts) + c2, list(syms) + s2, grid)
+                    srcv = vals[('f', id(sf))]
                     dt = vals.get(('s', dtsym.name))
                     got = eval_scalar(ex, leaf)
-                    if dt is None:
-                        # `src * dt**2 / m` with a literal dt (tests/test_gpu_openacc.py:205-251)
-                        plan['inject_literal'] = True
-                        m_val = self._role_value(m_role, vals)
-                        lit = got * m_val / srcv
-                        plan['inject_dt2'] = lit
+                    if literal:
+                        # `src * dt**2 / m` with a literal dt (tests/test_gpu_openacc.py:205-251): the literal is
+                        # got * m / src, which must not depend on the probe
+                        lits.append(got * self._role_value(m_role, vals) / srcv)
                         continue
                     want = srcv * dt * dt / self._role_value(m_role, vals)
                     if abs(got - want) > 1e-9 * max(1.0, abs(want)):
                         raise _Unrecognised("injected expression is not src*dt^2/m")
+                if literal:
+                    if abs(lits[1] - lits[0]) > 1e-9 * max(abs(lits[0]), 1e-30) or not lits[0] > 0:
+                        raise _Unrecognised("injected expression with a literal dt is not src*lit/m")
+                    plan['inject_literal'] = True
+                    plan['inject_dt2'] = lits[0]
             plan['src'] = sf
         if itps:
             itp = itps[0]
@@ -1560,7 +1592,9 @@ class Operator:
             if time_M is None:
                 if not sized:
                     raise InvalidArgument("No value found for parameter time_M")
-                nt = min(f.nt if getattr(f, 'is_SparseTimeFunction', False) else f.time_size for f in sized)
+                # a snapshot on a ConditionalDimension(factor=n) bounds time by time_size * n
+                nt = min(f.nt if getattr(f, 'is_SparseTimeFunction', False) else
+                         f.time_size * (_subsampled(f) or 1) for f in sized)
                 time_M = nt - 1 - max(thi, 0)
         else:
             time_m, time_M = 0, 0
@@ -1640,6 +1674,8 @@ class Operator:
     @staticmethod
     def _override_ok(check, f, so, grid):
         """Whether `f` is what the kernel reads in a slot of this `check` (see `_OVERRIDE_KINDS`)."""
+        if np.dtype(f.dtype) != np.float32:
+            return False
         if check == 'function':
             return isinstance(f, Function)
         if not isinstance(f, TimeFunction):
@@ -1668,6 +1704,8 @@ class Operator:
             if not isinstance(obj, Function) and isinstance(val, Function):
                 raise InvalidArgument(f"array-valued `{obj.name}` needs an Operator built with a Function")
         if isinstance(val, Function):
+            if np.dtype(val.dtype) != np.float32:
+                raise InvalidArgument(f"the override of `{obj.name}` must be a float32 Function")
             return val
         if isinstance(val, np.ndarray) and val.ndim:
             raise InvalidArgument(f"an array `{obj.name}` must have the allocated shape of a Function")
@@ -1724,6 +1762,12 @@ class Operator:
         # sparse
         src = self._resolve(kwargs, p['src'], post)
         rec = self._resolve(kwargs, p['rec'], post)
+        for sf in (src, rec):
+            # a caller-built sparse table (is_foreign) carries its own float32 arrays
+            if sf is not None and not getattr(sf, 'is_foreign', False) and \
+                    (np.dtype(sf.dtype) != np.float32 or np.dtype(sf.coordinates_data.dtype) != np.float32):
+                raise InvalidArgument(f"the override of `{sf.name}` must be a float32 SparseTimeFunction "
+                                      "(traces and coordinates)")
         args['src'], args['rec'] = src, rec
         # time range (devito/types/dimension.py:279-331)
         sized = [s for s in (src, rec) if s is not None]
@@ -2057,6 +2101,8 @@ class Operator:
         if not isinstance(f, TimeFunction) or f.space_order != f0.space_order or f.grid.shape != grid.shape \
                 or f.time_size != f0.time_size:
             raise InvalidArgument("incompatible override for the updated field")
+        if np.dtype(f.dtype) != np.float32:
+            raise InvalidArgument(f"the override of `{f0.name}` must be a float32 TimeFunction")
         args['fields'] = [f]
         # scalar environment of the coefficients: spacings, dt, Constants (overridable by name)
         env = {sp.name: float(v) for sp, v in grid.spacing_map.items()}
