@@ -1829,9 +1829,10 @@ class Operator:
         out[inner] = src
         return np.ascontiguousarray(out)
 
-    def _field_obj(self, fn, dev, resident, hold, so=None, written=False, host_io_ok=False):
+    def _field_obj(self, fn, dev, resident, hold, so=None, written=False, host_io_ok=False, post=None):
         """(b2_dataobj for a dense function: resident (dmap set) or host-staged, whether it is host-staged
-        through the caller's device buffer (host_io))."""
+        through the caller's device buffer (host_io)). A resident array the call writes is marked written by a hook
+        appended to `post`, run once the call has returned, so that a view the caller keeps sees what it wrote."""
         import torch
         fo = getattr(fn, '_foreign_obj', None)
         if fo is not None:
@@ -1866,7 +1867,7 @@ class Operator:
                 distributed.register_field(st, fn.grid, dev)
             ob = L_.make_dataobj(dev_ptr=t.data_ptr(), shape=st.shape, halo=fn.halo)
             if written:
-                st.mark_device_written()
+                post.append(st.mark_device_written)
         else:
             host = st.host if written else st.host_ro
             dist_ = fn.grid.distributor if fn.grid is not None else None
@@ -2052,9 +2053,10 @@ class Operator:
         for member, w in entry.weights:
             setattr(a, member, self._w_arrays(w, hold))
         host_io = False
+        post = []
         for s in entry.arrays:
             ob, hio = self._field_obj(args[s.member], dev, res, hold, so=p['so'] if s.layout else None,
-                                      written=s.written, host_io_ok=s.member in entry.host_io)
+                                      written=s.written, host_io_ok=s.member in entry.host_io, post=post)
             setattr(a, s.member, ob.ptr)
             host_io |= hio
         for prm, val in zip(entry.params, args['params']):
@@ -2076,7 +2078,6 @@ class Operator:
             setattr(a, ax + '_M', hi)
         a.time_m, a.time_M = args['time_m'], args['time_M']
         s = self._sparse_obj(args['src'], grid, hold)
-        post = []
         r = self._sparse_obj(args['rec'], grid, hold, written=True, post=post,
                              trange=(args['time_m'], args['time_M']))
         a.src = ctypes.pointer(s) if s is not None else None
@@ -2167,7 +2168,8 @@ class Operator:
         hold = []
         a = L_.LinearArgs()
         a.ndim = nd
-        a.f = self._field_obj(args['fields'][0], dev, args['resident'], hold, written=True)[0].ptr
+        post = []
+        a.f = self._field_obj(args['fields'][0], dev, args['resident'], hold, written=True, post=post)[0].ptr
         a.halo = p['so']
         taps = (L_.Tap * len(args['taps']))()
         for i, (t, o, c) in enumerate(args['taps']):
@@ -2181,7 +2183,7 @@ class Operator:
         lo, hi = args['lo'] + [0] * (3 - nd), args['hi'] + [0] * (3 - nd)
         a.x_m, a.x_M, a.y_m, a.y_M, a.z_m, a.z_M = lo[0], hi[0], lo[1], hi[1], lo[2], hi[2]
         a.time_m, a.time_M = args['time_m'], args['time_M']
-        return self._call(L, 'b2_linear_forward', a, args, dev)
+        return self._call(L, 'b2_linear_forward', a, args, dev, post)
 
 
 # ---------------------------------------------------------------------------------------------

@@ -238,7 +238,10 @@ class SeismicModel:
         # under decomposition the maxima are collectives: every rank must take the same branch, so no rank-local
         # shortcut there
         parallel = self.grid.distributor.is_parallel
-        if not parallel and cached is not None and cached[0] == key and None not in [k[1] for k in key[:-1]]:
+        # a view of a parameter kept by the caller may have been written since without a new access
+        viewed = any(p.storage.views_held() for p in pars if hasattr(p, 'storage'))
+        if not parallel and not viewed and cached is not None and cached[0] == key and \
+                None not in [k[1] for k in key[:-1]]:
             return cached[1]
         vmax = mmax(self.vp)
         aniso = np.sqrt(1 + 2 * mmax(self.epsilon)) if 'epsilon' in self._physical_parameters else 1

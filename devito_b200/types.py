@@ -10,8 +10,13 @@ API surface mirrors what `examples/seismic` touches in the reference (SURVEY App
 Data residency: every function owns a host array and, once a CUDA operator touched it, a
 device mirror (a torch tensor used purely as an allocation).  `.data` access synchronises
 device -> host lazily; the next CUDA operator re-uploads only if the host side was exposed.
+Views the caller keeps across applies stay coherent in both directions: while a view of an
+array is alive, every apply uploads that array before it runs and downloads it after writing
+it, so an apply costs a copy of an array only while a view of it is held.
 (The reference copies every array H2D/D2H on every `apply`, devito/passes/iet/definitions.py:636-671.)
 """
+import sys
+
 import numpy as np
 
 from .symbolics import Symbol, Access, Index
@@ -356,8 +361,17 @@ class RawDeviceBuffer:
 
 
 class FieldStorage:
+    """Host array and device mirror of one dense function.
+
+    `host_valid` / `dev_valid` say which copy is current. Views handed out by the accessors may be kept by the caller
+    across applies: every NumPy view of the host array, however derived, holds a reference to it (NumPy points a
+    view's `base` at the array that owns the data, here `_host` itself), so the host array's reference count above
+    the storage's own says whether such a view is alive (`views_held`). While one is, the host array is the copy the
+    caller reads and writes at any time: `to_device` uploads it even if the device copy looks current, and
+    `mark_device_written` downloads the device copy at once."""
     raw = False          # True: device copy is a RawDeviceBuffer (IPC-exportable)
     p2p_registered = False
+    _host_refs = 0       # references to `_host` with no caller view alive; 0: a host array the caller passed in
 
     def __init__(self, shape, dtype):
         self.shape = tuple(int(s) for s in shape)
@@ -372,6 +386,12 @@ class FieldStorage:
     def _alloc_host(self):
         if self._host is not None:
             return
+        self._host = self._new_host()
+        self._host_refs = sys.getrefcount(self._host)
+
+    def _new_host(self):
+        """A zeroed host array: page-locked (`_pinned`, a torch tensor sharing its memory) for arrays of 1 MiB or
+        more when CUDA is present, else a plain NumPy array."""
         n = int(np.prod(self.shape))
         try:
             import torch
@@ -386,11 +406,14 @@ class FieldStorage:
                 except Exception:
                     pass
                 self._pinned = torch.zeros(self.shape, dtype=tdt, pin_memory=True)
-                self._host = self._pinned.numpy()
-                return
+                return self._pinned.numpy()
         except Exception:
             self._pinned = None
-        self._host = np.zeros(self.shape, dtype=self.dtype)
+        return np.zeros(self.shape, dtype=self.dtype)
+
+    def views_held(self):
+        """Whether a view of the host array is alive outside this storage."""
+        return self._host is not None and sys.getrefcount(self._host) > self._host_refs
 
     @property
     def host(self):
@@ -428,8 +451,9 @@ class FieldStorage:
         self.host_valid = True
 
     def to_device(self, device):
-        """Device tensor holding current data (upload if the host copy is newer). A function
-        whose host array was never touched is all zeros: it is created directly on the device."""
+        """Device tensor holding current data (upload if the host copy is newer, or may be: while the caller keeps a
+        view of the host array). A function whose host array was never touched is all zeros: it is created directly on
+        the device."""
         import torch
         if self.raw:
             from ._lib import lib
@@ -446,11 +470,8 @@ class FieldStorage:
                     self.dev_valid, self.host_valid = True, False
                     return self.dev
                 self.dev_valid = False
-            if not self.dev_valid:
-                self._alloc_host()
-                if L.b2_memcpy_h2d(self.dev.ptr, self._host.ctypes.data, nbytes, device.index):
-                    raise RuntimeError("host -> device copy failed")
-                self.dev_valid = True
+            if not self.dev_valid or (self.host_valid and self.views_held()):
+                self._upload()
             return self.dev
         tdt = {np.dtype(np.float32): torch.float32, np.dtype(np.int32): torch.int32,
                np.dtype(np.float64): torch.float64}[self.dtype]
@@ -465,14 +486,23 @@ class FieldStorage:
                 return self.dev
             self.dev = torch.empty(self.shape, dtype=tdt, device=device)
             self.dev_valid = False
-        if not self.dev_valid:
-            self._alloc_host()
-            if self._pinned is not None:
-                self.dev.copy_(self._pinned, non_blocking=False)
-            else:
-                self.dev.copy_(torch.from_numpy(self._host))
-            self.dev_valid = True
+        if not self.dev_valid or (self.host_valid and self.views_held()):
+            self._upload()
         return self.dev
+
+    def _upload(self):
+        """Host -> device copy of the whole array into the existing device allocation."""
+        import torch
+        self._alloc_host()
+        if isinstance(self.dev, RawDeviceBuffer):
+            from ._lib import lib
+            if lib().b2_memcpy_h2d(self.dev.ptr, self._host.ctypes.data, self._host.nbytes, self.dev.deviceid):
+                raise RuntimeError("host -> device copy failed")
+        elif self._pinned is not None:
+            self.dev.copy_(self._pinned, non_blocking=False)
+        else:
+            self.dev.copy_(torch.from_numpy(self._host))
+        self.dev_valid = True
 
     def device_scratch(self, device):
         """A device buffer of this array's size WITHOUT uploading: staging space for a host-staged apply that moves
@@ -496,9 +526,13 @@ class FieldStorage:
         return self.dev
 
     def mark_device_written(self):
+        """A kernel wrote the device copy. Called once the write is complete: a view the caller keeps is brought up to
+        date at once."""
         self.dev_valid = True
         self.host_valid = False
         self.version += 1
+        if self.views_held():
+            self.sync_to_host()
 
     def drop_device(self):
         if self.dev is not None and not self.host_valid:
