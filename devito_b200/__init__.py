@@ -33,8 +33,9 @@ class _OutOfScope:
 
 
 class CheckpointOperator(_OutOfScope):
-    _what = "pyrevolve checkpointing (devito/checkpointing/checkpoint.py); the C-ABI loop is " \
-            "restartable on [time_m, time_M] sub-ranges, which is what it needs"
+    _what = "the pyrevolve adapters (devito/checkpointing/checkpoint.py) are not provided; the checkpointed " \
+            "acoustic gradient is `AcousticWaveSolver.jacobian_adjoint(rec, checkpointing=True, n_checkpoints=...)`, " \
+            "which runs its binomial schedule (devito_b200.revolve) inside one library call"
 
 
 class DevitoCheckpoint(_OutOfScope):

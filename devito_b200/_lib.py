@@ -130,10 +130,13 @@ class LinearArgs(Structure):
 
 MAX_TAPS = 64
 
+# action kinds of b2_iso_gradient_revolve
+REVOLVE_ACTIONS = {'advance': 0, 'takeshot': 1, 'restore': 2, 'reverse': 3}
+
 _lib = None
 
 # every symbol include/b200stencil.h declares
-SYMBOLS = ['b2_iso_forward', 'b2_tti_forward', 'b2_sa_forward', 'b2_linear_forward', 'b2_system_forward', 'b2_nccl_unique_id', 'b2_halo_create',
+SYMBOLS = ['b2_iso_forward', 'b2_iso_gradient_revolve', 'b2_revolve_check', 'b2_tti_forward', 'b2_sa_forward', 'b2_linear_forward', 'b2_system_forward', 'b2_nccl_unique_id', 'b2_halo_create',
            'b2_halo_destroy', 'b2_halo_update', 'b2_device_count', 'b2_last_error', 'b2_version',
            'b2_launch_count', 'b2_last_sweep_kernel', 'b2_last_iso_coef_reuse', 'b2_kernel_timing_reset', 'b2_kernel_timing_ms',
            'b2_kernel_timing_enable', 'b2_malloc_device', 'b2_free_device', 'b2_memcpy_h2d',
@@ -159,6 +162,10 @@ def load_library():
     L = ctypes.CDLL(LIB_PATH, mode=ctypes.RTLD_GLOBAL)
     L.b2_iso_forward.argtypes = [POINTER(IsoArgs)]
     L.b2_iso_forward.restype = c_int
+    L.b2_iso_gradient_revolve.argtypes = [POINTER(IsoArgs), POINTER(IsoArgs), POINTER(c_int), c_int, c_int]
+    L.b2_iso_gradient_revolve.restype = c_int
+    L.b2_revolve_check.argtypes = [POINTER(c_int), c_int, c_int, c_int, c_int, c_int, c_int]
+    L.b2_revolve_check.restype = c_int
     L.b2_tti_forward.argtypes = [POINTER(TtiArgs)]
     L.b2_tti_forward.restype = c_int
     L.b2_sa_forward.argtypes = [POINTER(SaArgs)]

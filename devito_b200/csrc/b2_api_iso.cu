@@ -15,6 +15,7 @@
 #include <string>
 #include <chrono>
 #include <algorithm>
+#include <climits>
 
 using namespace b2;
 
@@ -481,6 +482,20 @@ static int iso_forward_two_level(const b2_iso_args *a, const IsoPlan &p, const F
     return B2_OK;
 }
 
+// One step of the single-device loop at `time` (dir +1: forward, -1: adjoint): the sweep writes level time+dir from
+// levels time and time-dir, the free-surface rows are redone when asked, then `src` is injected into the level
+// written. `se` (may be null) records an event between the sweep and the injection.
+static int iso_sweep_inject(const IsoPlan &p, const FieldGeom &g, const SparseDev &src, int time, int dir, bool fs,
+                            float scalar_scale, float dt2, StepEvents *se) {
+    const int T = p.tsize, t0 = slot(time, T), t1 = slot(time + dir, T), t2 = slot(time - dir, T);
+    int rc;
+    if ((rc = iso_step(p, t0, t2, t1, 0, p.n[0]))) return rc;
+    if (fs && (rc = iso_fs_fix(p, t0, t2, t1, 0, p.n[0]))) return rc;
+    if (se) se->next();
+    return launch_inject(src, g, p.u + (size_t)t1 * p.slot_elems, nullptr, time, p.param_kind, p.param, scalar_scale,
+                         dt2);
+}
+
 }  // namespace b2
 
 extern "C" void b2_last_call_profile(double out[5]) {
@@ -694,23 +709,27 @@ static int iso_forward_body(const b2_iso_args *a, Staging &st, SnapStreamer &str
         const int t2 = slot(time - dir, T);     // the other time level read
         const bool per_step_events = timing && (step_index++ % sample_stride == 0) && se.used + 4 <= 16384;
         if (per_step_events) { se.next(); ++nsampled; }
-        if (fused) {
-            if ((rc = halo_step_iso_fused(a->halo, p, t0, t2, t1))) return rc;
-            // the injection below must reach the copies of my boundary planes in the neighbours' halos
-            g.peer_lo = fz.peer_lo; g.peer_hi = fz.peer_hi;
-            g.off_lo = (long long)t1 * fz.slot_lo + (long long)(p.o[0] + fz.n_lo) * p.sx;
-            g.off_hi = (long long)t1 * fz.slot_hi + (long long)(p.o[0] - p.n[0]) * p.sx;
-            g.nown = p.n[0]; g.pw = p.radius[0];
-        } else if (a->halo) {
-            if ((rc = halo_exchange_and_step_iso(a->halo, p, t0, t2, t1))) return rc;
-        } else {
-            if ((rc = iso_step(p, t0, t2, t1, 0, p.n[0]))) return rc;
-        }
-        if (a->free_surface && (rc = iso_fs_fix(p, t0, t2, t1, 0, p.n[0]))) return rc;
-        if (per_step_events) se.next();
         float *f1 = p.u + (size_t)t1 * p.slot_elems;
-        if ((rc = launch_inject(src, g, f1, nullptr, time, p.param_kind, p.param, scalar_scale, dt2)))
-            return rc;
+        if (!a->halo) {
+            if ((rc = iso_sweep_inject(p, g, src, time, dir, a->free_surface, scalar_scale, dt2,
+                                       per_step_events ? &se : nullptr)))
+                return rc;
+        } else {
+            if (fused) {
+                if ((rc = halo_step_iso_fused(a->halo, p, t0, t2, t1))) return rc;
+                // the injection below must reach the copies of my boundary planes in the neighbours' halos
+                g.peer_lo = fz.peer_lo; g.peer_hi = fz.peer_hi;
+                g.off_lo = (long long)t1 * fz.slot_lo + (long long)(p.o[0] + fz.n_lo) * p.sx;
+                g.off_hi = (long long)t1 * fz.slot_hi + (long long)(p.o[0] - p.n[0]) * p.sx;
+                g.nown = p.n[0]; g.pw = p.radius[0];
+            } else if ((rc = halo_exchange_and_step_iso(a->halo, p, t0, t2, t1))) {
+                return rc;
+            }
+            if (a->free_surface && (rc = iso_fs_fix(p, t0, t2, t1, 0, p.n[0]))) return rc;
+            if (per_step_events) se.next();
+            if ((rc = launch_inject(src, g, f1, nullptr, time, p.param_kind, p.param, scalar_scale, dt2)))
+                return rc;
+        }
         if (fused) {
             // the sweep stored the boundary planes, the injection patched them: release the flags
             if ((rc = halo_fused_signal(a->halo, p.u))) return rc;
@@ -842,4 +861,271 @@ extern "C" int b2_iso_forward(const struct b2_iso_args *a) {
     g_last_profile[2] = std::chrono::duration<double, std::milli>(t1 - d2h_t0).count();
     g_last_profile[3] = std::chrono::duration<double, std::milli>(t1 - call_t0).count();
     return rc ? rc : rs;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// b2_iso_gradient_revolve: the Gradient operator with the forward wavefield recomputed from checkpoints
+// (binomial checkpointing, Griewank & Walther, ACM TOMS 26(1) 2000) instead of read from a saved (nt, x, y, z)
+// array. The forward field lives in u's 3 slots; a checkpoint holds the two levels a step reads, u[t] and u[t-1],
+// as whole allocated slots (halo included: sinc injection writes there). The actions come from the caller's
+// schedule; both plans are built once and every action runs on the library stream.
+// ---------------------------------------------------------------------------------------------------------
+static bool same_array(const b2_dataobj *x, const b2_dataobj *y) {
+    if (x == y) return true;
+    return x && y && (x->data || x->dmap) && x->data == y->data && x->dmap == y->dmap && x->nbytes == y->nbytes;
+}
+
+extern "C" int b2_revolve_check(const int *actions, int nactions, int ncheckpoints, int fwd_time_m, int fwd_time_M,
+                                int grad_time_m, int grad_time_M) {
+    const char *who = "b2_revolve_check";
+    if (ncheckpoints < 1) { set_error("%s: %d checkpoints (at least 1)", who, ncheckpoints); return B2_ERR_INVALID; }
+    if (nactions < 0 || (nactions > 0 && !actions)) { set_error("%s: no action list", who); return B2_ERR_INVALID; }
+    std::vector<int> shot((size_t)ncheckpoints);
+    std::vector<char> full((size_t)ncheckpoints, 0);
+    int cur = fwd_time_m;                 // forward time of the state in u: levels cur and cur-1 are live
+    int next = grad_time_M;               // the adjoint time the next reverse must name
+    for (int i = 0; i < nactions; ++i) {
+        const int kind = actions[3 * i], x = actions[3 * i + 1], y = actions[3 * i + 2];
+        switch (kind) {
+            case B2_REVOLVE_ADVANCE:
+                if (x != cur || y <= x || y - 1 > fwd_time_M) {
+                    set_error("%s: action %d advance(%d, %d): the forward state is at time %d, steps run up to "
+                              "time_M=%d", who, i, x, y, cur, fwd_time_M);
+                    return B2_ERR_INVALID;
+                }
+                cur = y;
+                break;
+            case B2_REVOLVE_TAKESHOT:
+            case B2_REVOLVE_RESTORE:
+                if (x < 0 || x >= ncheckpoints) {
+                    set_error("%s: action %d names checkpoint %d of %d", who, i, x, ncheckpoints);
+                    return B2_ERR_INVALID;
+                }
+                if (kind == B2_REVOLVE_TAKESHOT) {
+                    if (y != cur) {
+                        set_error("%s: action %d takeshot(%d, %d): the forward state is at time %d", who, i, x, y, cur);
+                        return B2_ERR_INVALID;
+                    }
+                    shot[x] = cur;
+                    full[x] = 1;
+                } else {
+                    if (!full[x]) { set_error("%s: action %d restores the empty checkpoint %d", who, i, x); return B2_ERR_INVALID; }
+                    cur = shot[x];
+                }
+                break;
+            case B2_REVOLVE_REVERSE:
+                if (x != next || x < grad_time_m) {
+                    set_error("%s: action %d reverse(%d): the adjoint steps run once each from %d down to %d, the "
+                              "next is %d", who, i, x, grad_time_M, grad_time_m, next);
+                    return B2_ERR_INVALID;
+                }
+                if (x != cur && x != cur - 1) {
+                    set_error("%s: action %d reverse(%d) needs u[%d], the forward state holds levels %d and %d", who, i,
+                              x, x, cur - 1, cur);
+                    return B2_ERR_INVALID;
+                }
+                --next;
+                break;
+            default:
+                set_error("%s: action %d has the unknown kind %d", who, i, kind);
+                return B2_ERR_INVALID;
+        }
+    }
+    if (next >= grad_time_m) {
+        set_error("%s: the actions reverse down to time %d, not to time_m=%d", who, next + 1, grad_time_m);
+        return B2_ERR_INVALID;
+    }
+    return B2_OK;
+}
+
+// What the two argument blocks may be: everything the two loops share (medium, box, time step) is the same.
+static int revolve_args_check(const b2_iso_args *f, const b2_iso_args *g) {
+    const char *who = "b2_iso_gradient_revolve";
+    if (!f || !g || !f->u || !g->u) { set_error("%s: NULL args", who); return B2_ERR_INVALID; }
+    const b2_iso_args *both[2] = {f, g};
+    for (const b2_iso_args *a : both) {
+        const char *which = a == f ? "fwd" : "grad";
+        if (a->ndim != 3) { set_error("%s: %s: the imaging condition is 3-D only", who, which); return B2_ERR_INVALID; }
+        if (a->radius < 1 || a->radius > B2_MAX_RADIUS || a->radius > a->space_order) {
+            set_error("%s: %s: unsupported radius %d (space_order %d)", who, which, a->radius, a->space_order);
+            return B2_ERR_INVALID;
+        }
+        if (a->halo || a->ot4 || a->free_surface || a->born_U || a->born_dm || a->snap || a->host_io || a->rec) {
+            set_error("%s: %s: not combined with halo exchange, OT4, a free surface, Born modelling, snapshots, "
+                      "host_io or receivers", who, which);
+            return B2_ERR_INVALID;
+        }
+    }
+    if (f->adjoint || f->grad || f->usave) {
+        set_error("%s: fwd must describe the forward operator (no adjoint, grad or usave)", who);
+        return B2_ERR_INVALID;
+    }
+    if (!g->adjoint || !g->grad) { set_error("%s: grad must describe the Gradient operator (adjoint, grad)", who); return B2_ERR_INVALID; }
+    if (!same_array(g->usave, f->u)) {
+        set_error("%s: grad's usave must be fwd's u (the forward field is recomputed into it)", who);
+        return B2_ERR_INVALID;
+    }
+    if (same_array(g->u, f->u)) { set_error("%s: the adjoint field must not be the forward field", who); return B2_ERR_INVALID; }
+    if (!f->u->size || f->u->size[0] != 3) {
+        set_error("%s: fwd's u must be buffered with 3 time slots", who);
+        return B2_ERR_INVALID;
+    }
+    const int fb[6] = {f->x_m, f->x_M, f->y_m, f->y_M, f->z_m, f->z_M}, gb[6] = {g->x_m, g->x_M, g->y_m, g->y_M, g->z_m, g->z_M};
+    // the two sweeps share the update-coefficient tables: one medium, one box, one time step
+    if (f->space_order != g->space_order || f->radius != g->radius || f->dt != g->dt || f->vp != g->vp ||
+        f->param_kind != g->param_kind || !same_array(f->damp, g->damp) || !same_array(f->param, g->param) ||
+        memcmp(fb, gb, sizeof fb)) {
+        set_error("%s: fwd and grad must share space order, radius, dt, vp, damp, the parameter array and the "
+                  "iteration box", who);
+        return B2_ERR_INVALID;
+    }
+    return B2_OK;
+}
+
+static int iso_revolve_body(const b2_iso_args *f, const b2_iso_args *ga, const int *act, int nact, int nck,
+                            Staging &st) {
+    const char *who = "b2_iso_gradient_revolve";
+    const int so = f->space_order;
+    int rc;
+    DevArray *u, *v, *damp = nullptr, *param = nullptr, *grad;
+    SparseDev src, none, asrc, anone;
+    if ((rc = st.array(f->u, 4, true, u))) return rc;
+    if ((rc = st.array(ga->u, 4, true, v))) return rc;
+    if (f->damp && (rc = st.array(f->damp, 3, false, damp))) return rc;
+    if (f->param_kind != B2_PARAM_SCALAR) {
+        if (!f->param) { set_error("%s: param array missing", who); return B2_ERR_INVALID; }
+        if ((rc = st.array(f->param, 3, false, param))) return rc;
+    }
+    if ((rc = sparse_stage_pair(who, st, f->src, nullptr, 3, so, src, none))) return rc;
+    if ((rc = sparse_stage_pair(who, st, ga->src, nullptr, 3, so, asrc, anone))) return rc;
+    if ((rc = st.array(ga->grad, 3, true, grad))) return rc;
+    for (int d = 1; d < 4; ++d)
+        if (v->size[d] != u->size[d]) { set_error("%s: the adjoint field must have u's space layout", who); return B2_ERR_INVALID; }
+    const int gh = grid_halo(who, "grad", ga->grad, *grad, 0, *u, 3, so);
+    if (gh < 0) return B2_ERR_INVALID;
+
+    IsoPlan pf, pa;
+    const b2_iso_args *args[2] = {f, ga};
+    IsoPlan *plans[2] = {&pf, &pa};
+    DevArray *fields[2] = {u, v};
+    for (int i = 0; i < 2; ++i) {
+        IsoPlan &p = *plans[i];
+        const b2_iso_args *a = args[i];
+        static_cast<Box &>(p) = make_box(a, 3, fields[i]->size, so);
+        bool empty;
+        if ((rc = check_reach(who, p, 3, a->radius, empty))) return rc;
+        if (empty) return B2_OK;
+        for (int d = 0; d < 3; ++d) {
+            p.radius[d] = a->radius;
+            if (!a->w[d]) { set_error("%s: weights for dim %d missing", who, d); return B2_ERR_INVALID; }
+            for (int k = 0; k <= a->radius; ++k) p.w[d][k] = a->w[d][k];
+        }
+        p.u = (float *)fields[i]->d;
+        p.damp = damp ? (const float *)damp->d : nullptr;
+        p.param = param ? (const float *)param->d : nullptr;
+        p.param_kind = a->param_kind;
+        p.vp = a->vp;
+        p.dt = a->dt;
+        // the second plan re-tabulates the shared coefficient tables with the same medium, box and dt
+        if ((rc = iso_plan_init(p, a->kernel))) return rc;
+    }
+
+    // the checkpoints, once per call: two whole slots each
+    const size_t slot_bytes = pf.slot_elems * sizeof(float);
+    std::vector<float *> ck((size_t)nck);
+    for (int k = 0; k < nck; ++k) {
+        DevArray *x;
+        if ((rc = st.scratch(2 * slot_bytes, x))) return rc;
+        ck[k] = (float *)x->d;
+    }
+    auto level = [&](int time) { return pf.u + (size_t)slot(time, 3) * pf.slot_elems; };
+    const FieldGeom gf = field_geom(pf, 3), gg = field_geom(pa, 3);
+    const float dt2 = f->dt * f->dt, scalar_scale = dt2 * f->vp * f->vp;
+    bool two_level = false;
+    if ((rc = two_level_wanted(f, pf, *u, src, gf, false, false, two_level))) return rc;
+    // the sweeps that ran, in order of first use, space-separated: forward ones, then after ';' the adjoint one
+    std::string fwd_k, adj_k;
+    auto add_kernel = [](std::string &s) {
+        const std::string k = b2_last_sweep_kernel();
+        if (k.empty() || (" " + s + " ").find(" " + k + " ") != std::string::npos) return;
+        s += (s.empty() ? "" : " ") + k;
+    };
+    std::vector<int> shot((size_t)nck);
+    int cur = f->time_m;
+    // errctl on the forward steps keeps b2_iso_forward's cadence: every 100th forward time counted from time_m, and
+    // the last forward time the schedule reaches (a recomputed time is checked again)
+    int fwd_last = f->time_m;
+    for (int i = 0; i < nact; ++i)
+        if (act[3 * i] == B2_REVOLVE_ADVANCE) fwd_last = std::max(fwd_last, act[3 * i + 2] - 1);
+    // the level each slot of u holds (INT_MIN: none known): a restore copies only the levels not already in place,
+    // e.g. the ones the last advance left behind
+    int held[3] = {INT_MIN, INT_MIN, INT_MIN};
+    held[slot(cur, 3)] = cur;
+    held[slot(cur - 1, 3)] = cur - 1;
+    if ((rc = loop_timer_start(ga->timers))) return rc;
+    for (int i = 0; i < nact; ++i) {
+        const int kind = act[3 * i], x = act[3 * i + 1], y = act[3 * i + 2];
+        if (kind == B2_REVOLVE_ADVANCE) {
+            if (two_level && y - x >= 2) {
+                b2_iso_args r = *f;
+                r.time_m = x;
+                r.time_M = y - 1;
+                int nsampled = 0;
+                if ((rc = iso_forward_two_level(&r, pf, gf, src, none, scalar_scale, dt2, nullptr, 1, nsampled)))
+                    return rc;
+                held[0] = held[1] = held[2] = INT_MIN;
+                held[slot(y, 3)] = y;
+                held[slot(y - 1, 3)] = y - 1;
+            } else {
+                for (int time = x; time < y; ++time) {
+                    if ((rc = iso_sweep_inject(pf, gf, src, time, 1, false, scalar_scale, dt2, nullptr))) return rc;
+                    held[slot(time + 1, 3)] = time + 1;
+                    if (f->errctl && errctl_due(time, f->time_m, fwd_last) &&
+                        (rc = check_finite(level(time + 1), pf.slot_elems, "u", time)))
+                        return rc;
+                }
+            }
+            add_kernel(fwd_k);
+            cur = y;
+        } else if (kind == B2_REVOLVE_TAKESHOT || kind == B2_REVOLVE_RESTORE) {
+            const bool take = kind == B2_REVOLVE_TAKESHOT;
+            if (!take) cur = shot[x];
+            for (int j = 0; j < 2; ++j) {
+                float *c = ck[x] + (size_t)j * pf.slot_elems, *l = level(cur - j);
+                if (!take && held[slot(cur - j, 3)] == cur - j) continue;
+                B2_CUDA(cudaMemcpyAsync(take ? c : l, take ? l : c, slot_bytes, cudaMemcpyDeviceToDevice, stream()),
+                        B2_ERR_MEMORY);
+                held[slot(cur - j, 3)] = cur - j;
+            }
+            if (take) shot[x] = cur;
+        } else {
+            // one adjoint step, then grad -= u[x] * v.dt2 with u[x] live in its slot
+            const int T = pa.tsize;
+            if ((rc = iso_sweep_inject(pa, gg, asrc, x, -1, false, scalar_scale, dt2, nullptr))) return rc;
+            if ((rc = launch_imaging(pa, *grad, gh, level(x), pa.u, nullptr, nullptr, slot(x, T), slot(x - 1, T),
+                                     slot(x + 1, T))))
+                return rc;
+            add_kernel(adj_k);
+            if (ga->errctl && errctl_due(x, ga->time_m, ga->time_m) &&
+                (rc = check_finite(pa.u + (size_t)slot(x - 1, T) * pa.slot_elems, pa.slot_elems, "v", x)))
+                return rc;
+        }
+    }
+    note_sweep_kernel("%s;%s", fwd_k.c_str(), adj_k.c_str());
+    return loop_finish(who, ga->timers);
+}
+
+extern "C" int b2_iso_gradient_revolve(const struct b2_iso_args *fwd, const struct b2_iso_args *grad,
+                                       const int *actions, int nactions, int ncheckpoints) {
+    int rc;
+    if ((rc = revolve_args_check(fwd, grad))) return rc;
+    if ((rc = b2_revolve_check(actions, nactions, ncheckpoints, fwd->time_m, fwd->time_M, grad->time_m, grad->time_M)))
+        return rc;
+    if (grad->time_M < grad->time_m) return B2_OK;
+    std::lock_guard<std::mutex> api_lock(api_mutex());
+    if ((rc = use_device(fwd->deviceid))) return rc;
+    note_sweep_kernel("");
+    Staging st;
+    rc = iso_revolve_body(fwd, grad, actions, nactions, ncheckpoints, st);
+    return st.finish(rc);
 }

@@ -106,6 +106,7 @@ struct DevArray {
     bool owned = false;      // we allocated it: released when the call ends
     bool written = false;    // the call writes it: copied back to `h` (see Staging::finish)
     bool host_io = false;    // ... even though not owned: the caller's own device buffer next to its host array
+    bool pooled = true;      // an owned buffer goes back to the staging pool (false: freed outright)
     int ndim = 0;
     int size[4] = {1, 1, 1, 1};
 };
@@ -116,6 +117,9 @@ class Staging {
     // Stages `obj` (`ndim` extents): resident arrays (dmap) are used in place, host arrays are copied in (copy_in)
     // to a buffer of the staging pool. `out` is set even when this fails, and finish() releases what it holds.
     int array(const b2_dataobj *obj, int ndim, bool written, DevArray *&out, bool copy_in = true);
+    // Device scratch of `nbytes` for the call alone (uninitialised, never copied): freed by finish(), not pooled, so
+    // that the memory it held is free again when the call returns.
+    int scratch(size_t nbytes, DevArray *&out);
     // Ends the call: the written arrays go back to the host iff `code` is B2_OK or B2_ERR_NAN, every staged buffer
     // is released whatever the code. Returns `code`, or the first copy-back error when `code` is B2_OK.
     int finish(int code);

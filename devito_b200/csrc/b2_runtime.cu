@@ -190,6 +190,22 @@ int Staging::array(const b2_dataobj *obj, int ndim, bool written, DevArray *&out
     return B2_OK;
 }
 
+int Staging::scratch(size_t nbytes, DevArray *&out) {
+    DevArray &x = arrays_.emplace_back();
+    out = &x;
+    x.nbytes = nbytes;
+    x.pooled = false;
+    if (cudaMalloc(&x.d, nbytes) != cudaSuccess) {
+        cudaGetLastError();                        // not sticky: later calls must not see it
+        x.d = nullptr;
+        set_error("device scratch of %zu bytes: out of memory", nbytes);
+        return B2_ERR_MEMORY;
+    }
+    x.owned = true;
+    ++g_staged_outstanding;
+    return B2_OK;
+}
+
 int Staging::finish(int code) {
     cudaError_t e = cudaSuccess;
     if (code == B2_OK || code == B2_ERR_NAN)
@@ -203,7 +219,8 @@ int Staging::finish(int code) {
     if (e == cudaSuccess) e = s;
     for (DevArray &x : arrays_)
         if (x.owned) {
-            pool_release(x.d, x.nbytes);
+            if (x.pooled) pool_release(x.d, x.nbytes);
+            else cudaFree(x.d);
             --g_staged_outstanding;
         }
     arrays_.clear();

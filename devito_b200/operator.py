@@ -1711,13 +1711,15 @@ class Operator:
             raise InvalidArgument(f"an array `{obj.name}` must have the allocated shape of a Function")
         return float(val.data if isinstance(val, Constant) else val)
 
-    def _prepare(self, kwargs):
+    def _prepare(self, kwargs, omit=()):
         p, entry = self._plan, self._entry
         grid = p['grid']
         args = OrderedDict()
         hold = []          # keep ctypes/ndarray objects alive during the call
         post = args['post'] = []     # run after the C call (write-back of ndarray overrides)
         for s in entry.arrays:
+            if s.member in omit:
+                continue
             f = args[s.member] = self._resolve(kwargs, s.obj, post)
             if not self._override_ok(s.check, f, p['so'], grid):
                 raise InvalidArgument(f"the override of `{s.obj.name}` must be {_OVERRIDE_KINDS[s.check]}")
@@ -1772,7 +1774,7 @@ class Operator:
         # time range (devito/types/dimension.py:279-331)
         sized = [s for s in (src, rec) if s is not None]
         sized += [f for f in args['fields'] if not f.is_buffered]
-        sized += [args[s.member] for s in entry.arrays if s.check == 'saved']
+        sized += [args[s.member] for s in entry.arrays if s.check == 'saved' and s.member not in omit]
         time_m = kwargs.pop('time_m', None)
         time_M = kwargs.pop('time_M', kwargs.pop('time', None))
         if time_m is None:
@@ -2042,7 +2044,15 @@ class Operator:
 
     def _apply_wave(self, **kwargs):
         L = L_.lib()
-        args, hold = self._prepare(dict(kwargs))
+        hold = []          # alive until the call returns
+        a, args, dev, post = self._marshal_wave(kwargs, hold)
+        return self._call(L, self._entry.symbol, a, args, dev, post)
+
+    def _marshal_wave(self, kwargs, hold, omit=()):
+        """The entry point's argument block for an apply with `kwargs`: (block, prepared arguments, device, post-call
+        hooks). `hold` keeps what the block points into alive; the array members in `omit` are left NULL."""
+        args, held = self._prepare(dict(kwargs), omit)
+        hold.extend(held)
         p, entry = self._plan, self._entry
         grid = p['grid']
         dev = self._device(args)
@@ -2055,6 +2065,8 @@ class Operator:
         host_io = False
         post = []
         for s in entry.arrays:
+            if s.member in omit:
+                continue
             ob, hio = self._field_obj(args[s.member], dev, res, hold, so=p['so'] if s.layout else None,
                                       written=s.written, host_io_ok=s.member in entry.host_io, post=post)
             setattr(a, s.member, ob.ptr)
@@ -2090,7 +2102,7 @@ class Operator:
             # injection used a literal dt**2 (not the `dt` symbol): it must agree with runtime dt
             if abs(p['inject_dt2'] - a.dt * a.dt) > 1e-5 * p['inject_dt2']:
                 raise InvalidArgument("literal dt in the injected expression differs from runtime dt")
-        return self._call(L, entry.symbol, a, args, dev, post)
+        return a, args, dev, post
 
     # -- generic constant-coefficient update ------------------------------------------------------
     def _prepare_linear(self, kwargs):

@@ -1,6 +1,14 @@
 """Isotropic acoustic modelling (mirror of examples/seismic/acoustic/operators.py:50-187 and
 wavesolver.py:11-156): forward and adjoint operators (gradient/Born are SURVEY §8f)."""
-from .. import Eq, FreeSurface, Inc, Function, Operator, TimeFunction, solve
+import ctypes
+import time as _time
+from types import SimpleNamespace
+
+import numpy as np
+
+from .. import Eq, FreeSurface, Inc, Function, Operator, TimeFunction, solve, InvalidArgument
+from .. import _lib as L_
+from ..revolve import schedule, default_n_checkpoints
 from ..tools import memoized_meth
 
 __all__ = ['laplacian', 'iso_stencil', 'ForwardOperator', 'AdjointOperator', 'GradientOperator',
@@ -95,7 +103,8 @@ def BornOperator(model, geometry, space_order=4, kernel='OT2', **kwargs):
 
 
 class AcousticWaveSolver:
-    """wavesolver.py:11-120 (`forward` only)."""
+    """wavesolver.py:11-230: forward, adjoint, Born (`jacobian`) and gradient (`jacobian_adjoint`, with or without
+    checkpointing)."""
 
     def __init__(self, model, geometry, kernel='OT2', space_order=4, **kwargs):
         self.model = model
@@ -136,8 +145,19 @@ class AcousticWaveSolver:
         return GradientOperator(self.model, save=save, geometry=self.geometry, kernel=self.kernel,
                                 space_order=self.space_order, **self._kwargs)
 
-    def jacobian_adjoint(self, rec, u, src=None, v=None, grad=None, model=None, **kwargs):
-        """wavesolver.py:158-230 (without checkpointing): gradient of the data misfit w.r.t. m."""
+    def jacobian_adjoint(self, rec, u=None, src=None, v=None, grad=None, model=None, checkpointing=False,
+                         n_checkpoints=None, **kwargs):
+        """wavesolver.py:158-230: gradient of the data misfit w.r.t. m. Without `checkpointing`, `u` is the saved
+        forward wavefield (`forward(save=True)`). With it, `u` is not needed: one library call recomputes the forward
+        field from `n_checkpoints` device checkpoints of two wavefield slots each (binomial checkpointing,
+        devito_b200/revolve.py) while it runs the adjoint; `src` drives the forward run (default: the geometry's).
+        `n_checkpoints=None` takes as many as fit in 90 % of the free device memory, at most one per time step."""
+        if checkpointing:
+            return self._jacobian_adjoint_revolve(rec, src=src, v=v, grad=grad, model=model,
+                                                  n_checkpoints=n_checkpoints, **kwargs)
+        if u is None:
+            raise TypeError("jacobian_adjoint() needs the saved forward wavefield `u` (forward(save=True)) unless "
+                            "checkpointing=True")
         dt = kwargs.pop('dt', self.dt)
         grad = grad or Function(name='grad', grid=self.model.grid)
         v = v or TimeFunction(name='v', grid=self.model.grid, time_order=2, space_order=self.space_order)
@@ -145,6 +165,85 @@ class AcousticWaveSolver:
         kwargs.update(model.physical_params(**kwargs))
         summary = self.op_grad().apply(rec=rec, grad=grad, v=v, u=u, dt=dt, **kwargs)
         return grad, summary
+
+    def _revolve_setup(self, rec, src=None, v=None, grad=None, model=None, n_checkpoints=None, **kwargs):
+        """The two argument blocks of b2_iso_gradient_revolve (the forward operator's and the Gradient operator's,
+        marshalled like their applies; the Gradient's usave, damp and parameter point at the forward block's arrays)
+        and its action list. Refuses what the entry point does not run before touching the device."""
+        if n_checkpoints is not None and int(n_checkpoints) < 1:
+            raise ValueError(f"n_checkpoints must be at least 1, got {n_checkpoints}")
+        op_g = self.op_grad(save=True)          # OT4: the Gradient operator's NotImplementedError
+        if self.model.grid.distributor.is_parallel:
+            raise InvalidArgument("the checkpointed gradient does not run on a decomposed grid in this version")
+        op_f = self.op_fwd(save=False)
+        for op in (op_f, op_g):
+            if op.backend != 'cuda-sm90a':
+                raise InvalidArgument(f"operator `{op.name}` is not on the CUDA path: {op._why_not}")
+        dt = kwargs.pop('dt', self.dt)
+        u = TimeFunction(name='u', grid=self.model.grid, time_order=2, space_order=self.space_order)
+        grad = grad or Function(name='grad', grid=self.model.grid)
+        v = v or TimeFunction(name='v', grid=self.model.grid, time_order=2, space_order=self.space_order)
+        model = model or self.model
+        kwargs.update(model.physical_params(**kwargs))
+        hold = []
+        af, args_f, dev, post_f = op_f._marshal_wave(dict(kwargs, src=src or self.geometry.src, u=u, dt=dt), hold)
+        ag, args_g, _, post_g = op_g._marshal_wave(dict(kwargs, rec=rec, v=v, grad=grad, dt=dt), hold,
+                                                   omit=('usave',))
+        af.rec = None                           # the forward run records nothing
+        ag.usave, ag.damp, ag.param = af.u, af.damp, af.param
+        # schedule step i <-> forward state at time tf + i (levels tf + i, tf + i - 1) and adjoint time tg + i
+        tf, tg = args_f['time_m'], args_g['time_m']
+        nsteps = args_g['time_M'] - tg + 1
+        if tf - tg not in (0, 1):
+            raise InvalidArgument(f"the forward loop starts at time {tf}, the adjoint one at {tg}: the adjoint step at "
+                                  "time t needs u[t] among the two levels of forward state t")
+        if n_checkpoints is None and nsteps < 1:
+            n_checkpoints = 1                   # nothing to reverse: the call returns without device work
+        if n_checkpoints is None:
+            import torch
+            free = torch.cuda.mem_get_info(dev)[0]
+            # what the call itself copies in (host-staged arrays) is not free for checkpoints
+            free -= sum(o.contents.nbytes for o in (af.u, af.damp, af.param, ag.u, ag.grad)
+                        if o and not o.contents.dmap)
+            slot = int(np.prod(u.storage.shape[1:])) * np.dtype(np.float32).itemsize
+            n_checkpoints = default_n_checkpoints(nsteps, free, slot)
+            if n_checkpoints < 1:
+                raise InvalidArgument("no device memory is left for a checkpoint (two wavefield slots)")
+        n_checkpoints = int(n_checkpoints)
+        sched = schedule(nsteps, n_checkpoints)
+        flat = []
+        for act in sched:
+            kind = L_.REVOLVE_ACTIONS[act[0]]
+            if act[0] == 'advance':
+                flat += [kind, tf + act[1], tf + act[2]]
+            elif act[0] == 'takeshot':
+                flat += [kind, act[1], tf + act[2]]
+            elif act[0] == 'restore':
+                flat += [kind, act[1], 0]
+            else:
+                flat += [kind, tg + act[1], 0]
+        actions = (ctypes.c_int * max(len(flat), 1))(*flat)
+        return SimpleNamespace(op=op_g, fwd=af, grad=ag, args=args_g, dev=dev, post=post_f + args_f['post'] + post_g + args_g['post'],
+                               actions=actions, nactions=len(sched), n_checkpoints=n_checkpoints, schedule=sched,
+                               nsteps=nsteps, hold=hold, grad_fn=grad)
+
+    def _jacobian_adjoint_revolve(self, rec, **kwargs):
+        return self._revolve_run(self._revolve_setup(rec, **kwargs))
+
+    def _revolve_run(self, c):
+        """One call of b2_iso_gradient_revolve with what `_revolve_setup` built: (grad, summary)."""
+        L = L_.lib()
+        c.fwd.deviceid = c.grad.deviceid = c.dev
+        timers = L_.Profiler()
+        c.grad.timers = ctypes.pointer(timers)
+        t0 = _time.perf_counter()
+        rc = L.b2_iso_gradient_revolve(ctypes.byref(c.fwd), ctypes.byref(c.grad), c.actions, c.nactions,
+                                       c.n_checkpoints)
+        t_wall = _time.perf_counter() - t0
+        for fn in c.post:
+            fn()
+        summary = c.op._finish(rc, L, timers, c.args, t_wall)
+        return c.grad_fn, summary
 
     jacobian_adjoint.__name__ = 'jacobian_adjoint'
     gradient = jacobian_adjoint

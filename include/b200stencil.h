@@ -163,6 +163,39 @@ struct b2_iso_args {
 };
 int b2_iso_forward(const struct b2_iso_args *a);
 
+/* ---- the acoustic gradient with binomial checkpointing (the reference's `jacobian_adjoint(checkpointing=True)`,
+ *      examples/seismic/acoustic/wavesolver.py:196-210) ------------------------------------------------------------
+ * Runs the Gradient operator `grad` (adjoint != 0, with `grad`; `src` = the receiver data injected into the adjoint
+ * field grad->u) while the forward operator `fwd` (adjoint 0, `src`, u buffered with 3 time slots) recomputes the
+ * forward wavefield from `ncheckpoints` device checkpoints instead of reading a saved (nt, x, y, z) array: grad->usave
+ * must be fwd->u (the same struct, or one with the same data, dmap and nbytes). `actions` holds `nactions` triples
+ * {kind, a, b}, in absolute time indices of the two operators:
+ *   B2_REVOLVE_ADVANCE  {t0, t1}: forward steps time = t0 .. t1-1 (t0 = the current forward time; the sweeps, the two-
+ *                                 level pass and the injection of b2_iso_forward)
+ *   B2_REVOLVE_TAKESHOT {k, t}  : copy u[t] and u[t-1] (whole allocated slots, halo included) into checkpoint k
+ *                                 (t = the current forward time)
+ *   B2_REVOLVE_RESTORE  {k, -}  : copy them back; the current forward time becomes t
+ *   B2_REVOLVE_REVERSE  {t, -}  : one adjoint step at time t with its injection, then grad -= u[t] * v.dt2, u[t] read
+ *                                 from its slot of u (t = the current forward time or the one before)
+ * The reverse steps name grad->time_M down to grad->time_m, once each. The forward state at entry is fwd->time_m
+ * (levels time_m and time_m-1 in u). Every array is staged once, both plans are built once and the checkpoints
+ * (2 slots each) are allocated for the call and freed on return. 3-D only; a halo context, OT4, a free surface, Born,
+ * snapshots, host_io or receivers (`rec`) in either block, a usave that is not fwd's u, fwd and grad that differ in
+ * space order, radius, dt, vp, damp, the parameter array or the iteration box, or a malformed action list return
+ * 210. errctl checks u after every forward step at a time with (time - fwd->time_m) % 100 == 99 or at the last
+ * forward time the schedule reaches (again when that time is recomputed), and v on the adjoint steps as
+ * b2_iso_forward does. The loop time goes to grad->timers->section0.
+ * b2_last_sweep_kernel then reports the forward sweeps that ran (space-separated, in order of first use), ';', the
+ * adjoint one, e.g. "iso_tma2<4,scalar> iso_tma<4,scalar>;iso_tma<4,scalar>". */
+enum { B2_REVOLVE_ADVANCE = 0, B2_REVOLVE_TAKESHOT = 1, B2_REVOLVE_RESTORE = 2, B2_REVOLVE_REVERSE = 3 };
+int b2_iso_gradient_revolve(const struct b2_iso_args *fwd, const struct b2_iso_args *grad, const int *actions,
+                            int nactions, int ncheckpoints);
+/* Host only, no device needed: 0 when `actions` is a schedule b2_iso_gradient_revolve accepts for these time ranges,
+ * else 210 with the first fault in b2_last_error (out-of-range times or checkpoints, a restore of an empty
+ * checkpoint, a reverse step out of order or without its forward level live, steps left unreversed). */
+int b2_revolve_check(const int *actions, int nactions, int ncheckpoints, int fwd_time_m, int fwd_time_M,
+                     int grad_time_m, int grad_time_M);
+
 /* ---- TTI centred forward (replaces generated `ForwardTTI`,
  *      examples/seismic/tti/operators.py:186-247, 431-480), 2-D and 3-D ----------------------- */
 struct b2_tti_args {
