@@ -14,7 +14,7 @@ import numpy as np
 
 from .exceptions import BackendUnavailable
 
-__all__ = ['lib', 'have_lib', 'have_gpu', 'Dataobj', 'Profiler', 'Sparse', 'IsoArgs', 'TtiArgs', 'SaArgs', 'Tap', 'LinearArgs',
+__all__ = ['lib', 'have_lib', 'have_gpu', 'Dataobj', 'Profiler', 'Sparse', 'IsoArgs', 'TtiArgs', 'SaArgs', 'ViscoArgs', 'Tap', 'LinearArgs',
            'SysTap', 'SysStage', 'SysInject', 'SysInterp', 'SystemArgs',
            'make_dataobj', 'ForeignDataobj', 'ForeignSparse', 'nccl_library_path', 'LIB_PATH']
 
@@ -87,6 +87,19 @@ class SaArgs(Structure):
                 ('halo', c_void_p), ('free_surface', c_int), ('timers', POINTER(Profiler))]
 
 
+class ViscoArgs(Structure):
+    _fields_ = [('ndim', c_int), ('space_order', c_int), ('radius', c_int),
+                ('c', POINTER(c_float) * 3),
+                ('u', POINTER(Dataobj)), ('r', POINTER(Dataobj)), ('b', POINTER(Dataobj)), ('b_value', c_float),
+                ('vp', POINTER(Dataobj)), ('vp_value', c_float), ('qp', POINTER(Dataobj)), ('qp_value', c_float),
+                ('damp', POINTER(Dataobj)), ('f0', c_float), ('dt', c_float),
+                ('x_m', c_int), ('x_M', c_int), ('y_m', c_int), ('y_M', c_int),
+                ('z_m', c_int), ('z_M', c_int), ('time_m', c_int), ('time_M', c_int),
+                ('src', POINTER(Sparse)), ('rec', POINTER(Sparse)), ('rec_toff', c_int),
+                ('adjoint', c_int), ('errctl', c_int), ('deviceid', c_int), ('kernel', c_int),
+                ('halo', c_void_p), ('free_surface', c_int), ('timers', POINTER(Profiler))]
+
+
 class Tap(Structure):
     _fields_ = [('tshift', c_int), ('off', c_int * 3), ('coef', c_float)]
 
@@ -136,7 +149,7 @@ REVOLVE_ACTIONS = {'advance': 0, 'takeshot': 1, 'restore': 2, 'reverse': 3}
 _lib = None
 
 # every symbol include/b200stencil.h declares
-SYMBOLS = ['b2_iso_forward', 'b2_iso_gradient_revolve', 'b2_revolve_check', 'b2_tti_forward', 'b2_sa_forward', 'b2_linear_forward', 'b2_system_forward', 'b2_nccl_unique_id', 'b2_halo_create',
+SYMBOLS = ['b2_iso_forward', 'b2_iso_gradient_revolve', 'b2_revolve_check', 'b2_tti_forward', 'b2_sa_forward', 'b2_visco_forward', 'b2_linear_forward', 'b2_system_forward', 'b2_nccl_unique_id', 'b2_halo_create',
            'b2_halo_destroy', 'b2_halo_update', 'b2_device_count', 'b2_last_error', 'b2_version',
            'b2_launch_count', 'b2_last_sweep_kernel', 'b2_last_iso_coef_reuse', 'b2_kernel_timing_reset', 'b2_kernel_timing_ms',
            'b2_kernel_timing_enable', 'b2_malloc_device', 'b2_free_device', 'b2_memcpy_h2d',
@@ -170,6 +183,8 @@ def load_library():
     L.b2_tti_forward.restype = c_int
     L.b2_sa_forward.argtypes = [POINTER(SaArgs)]
     L.b2_sa_forward.restype = c_int
+    L.b2_visco_forward.argtypes = [POINTER(ViscoArgs)]
+    L.b2_visco_forward.restype = c_int
     L.b2_linear_forward.argtypes = [POINTER(LinearArgs)]
     L.b2_linear_forward.restype = c_int
     L.b2_system_forward.argtypes = [POINTER(SystemArgs)]

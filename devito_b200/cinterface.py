@@ -149,7 +149,7 @@ def _body(plan, distributed):
     L.append(f"  struct b2_{plan['kind']}_args a;")
     L.append("  memset(&a, 0, sizeof(a));")
     for k, v in entry.flags.items():
-        L.append(f"  a.{k} = {int(v)};")
+        L.append(f"  a.{k} = {_flit(v) if isinstance(v, float) else int(v)};")
     for member, _ in entry.weights:
         for d in range(nd):
             L.append(f"  a.{member}[{d}] = {member}_{'xyz'[d]};")

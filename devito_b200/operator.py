@@ -18,6 +18,7 @@ over the C ABI in include/b200stencil.h (one FFI crossing per `apply`, like the 
 interpreter.  The recognised path NEVER falls back to the CPU.
 """
 import ctypes
+import itertools
 import os
 import time as _time
 from collections import OrderedDict
@@ -156,6 +157,11 @@ class _Unrecognised(Exception):
     pass
 
 
+class _NotVisco(_Unrecognised):
+    """Two updates that do not have the shape of the SLS pair (the second reads the first only at the level the
+    first writes): left to the TTI and Born recognisers."""
+
+
 # ---------------------------------------------------------------------------------------------
 # the argument block of a wave operator's C entry point
 # ---------------------------------------------------------------------------------------------
@@ -187,7 +193,7 @@ class Entry(NamedTuple):
     plugin (refplugin.py) need to know about the call of a recognised wave operator."""
     symbol: str             # b2_<kind>_forward, taking a struct b2_<kind>_args
     struct: type            # its ctypes mirror
-    flags: dict             # integer members fixed by the plan
+    flags: dict             # members fixed by the plan (integers; f0 of the viscoacoustic update)
     weights: list           # (member, per-dimension weight lists)
     arrays: list            # Slots, in the order they are marshalled
     params: list            # Params
@@ -203,7 +209,8 @@ _OVERRIDE_KINDS = {'wavefield': "a float32 TimeFunction of the wavefield's space
 def wave_entry(p):
     """The `Entry` of a recognised wave plan (kind 'iso', 'tti' or 'sa')."""
     kind = p['kind']
-    slots = [('u', True, False, 'wavefield'), ('v', True, False, 'wavefield'), ('damp', False, True, 'function'),
+    slots = [('u', True, False, 'wavefield'), ('v', True, False, 'wavefield'), ('r', True, False, 'wavefield'),
+             ('damp', False, True, 'function'),
              ('snap', True, False, 'snapshot'), ('born_U', True, False, 'wavefield'),
              ('born_du', True, False, 'wavefield'), ('born_dv', True, False, 'wavefield'),
              ('born_dm', False, False, 'function'), ('grad', True, False, 'function'),
@@ -214,6 +221,8 @@ def wave_entry(p):
         params = [Param('param', 'vp', obj, 1.0, role.startswith('m_'), True)]
     elif kind == 'sa':
         params = [Param(k, k + '_value', p[k + '_role'][1], 1.0, False, True) for k in ('b', 'vp')]
+    elif kind == 'visco':
+        params = [Param(k, k + '_value', p[k + '_role'][1], 1.0, False, True) for k in ('b', 'vp', 'qp')]
     else:
         params = [Param(n + '_arr', n, p['consts'].get(n), 1.0 if n == 'vp' else 0.0, False, False)
                   for n in ('vp', 'epsilon', 'delta', 'theta', 'phi')]
@@ -223,8 +232,10 @@ def wave_entry(p):
         flags.update(free_surface=int(bool(p.get('free_surface'))), ot4=int(bool(p.get('ot4'))))
         if p.get('snap') is not None:
             flags.update(snap_factor=p['snap_factor'], snap_toff=p['snap_toff'])
+    if kind == 'visco':
+        flags.update(f0=float(p['f0']))
     weights = [(k, p[k]) for k in ('w', 'w2', 'w1', 'c') if k in p]
-    struct = {'iso': L_.IsoArgs, 'tti': L_.TtiArgs, 'sa': L_.SaArgs}[kind]
+    struct = {'iso': L_.IsoArgs, 'tti': L_.TtiArgs, 'sa': L_.SaArgs, 'visco': L_.ViscoArgs}[kind]
     return Entry(f'b2_{kind}_forward', struct, flags, weights, arrays, params,
                  ('u', 'damp', 'param') if kind == 'iso' else ())
 
@@ -298,14 +309,14 @@ class Operator:
         return plan
 
     # the plan members that are arrays the library reads or writes
-    _ARRAY_MEMBERS = ('u', 'v', 'damp', 'snap', 'born_U', 'born_du', 'born_dv', 'born_dm', 'grad', 'usave', 'vsave')
+    _ARRAY_MEMBERS = ('u', 'v', 'r', 'damp', 'snap', 'born_U', 'born_du', 'born_dv', 'born_dm', 'grad', 'usave', 'vsave')
 
     @classmethod
     def _check_dtypes(cls, plan):
         """The kernels read and write float32 only: a plan whose grid, fields, parameter Functions, saved
         fields or sparse traces and coordinates are of another dtype is not theirs to run."""
         objs = [plan[k] for k in cls._ARRAY_MEMBERS if plan.get(k) is not None]
-        for k in ('m_role', 'b_role', 'vp_role'):
+        for k in ('m_role', 'b_role', 'vp_role', 'qp_role'):
             if plan.get(k) is not None:
                 objs.append(plan[k][1])
         objs += list(plan.get('consts', {}).values())
@@ -431,6 +442,13 @@ class Operator:
             return plan
         if snaps:
             raise _Unrecognised("snapshots are on the fast path next to the single-field acoustic update only")
+        if len(updates) == 2 and not incs:
+            try:
+                return self._recognise_visco(updates, injs, itps)
+            except _NotVisco:
+                pass            # not the shape of the SLS pair: the TTI / Born recognisers below decide
+            except _Unrecognised as visco_why:
+                raise _Unrecognised(f"as the SLS viscoacoustic pair: {visco_why}") from None
         if len(updates) == 2 and (self._dirn != 1 or incs):
             if any(_space_offsets(e.lhs, None)[0] != -1 for _, e in updates):
                 raise _Unrecognised("the TTI imaging condition needs the backward (adjoint) pair")
@@ -756,7 +774,7 @@ class Operator:
         scale = max(abs(v) for v in pred.values())
         return set(got) == set(pred) and all(abs(got[k] - pred[k]) <= 1e-9 * scale for k in pred)
 
-    def _attach_sa_sparse(self, plan, injs, itps, funcs, consts, syms):
+    def _attach_sa_sparse(self, plan, injs, itps, funcs, consts, syms, scale=None, what="src*dt^2*vp^2/b"):
         """Injection `src * dt^2 * vp^2 / b` into the level written (operators.py:101, :149), checked at random
         values; receivers / the adjoint source as for the acoustic update."""
         grid, dtsym = plan['grid'], plan['dt']
@@ -797,12 +815,120 @@ class Operator:
                     if n.is_Constant:
                         return vals[id(n)]
                     return dt if n.name == dtsym.name else spc[n.name]
-                want = vals[id(sf)] * dt * dt * vals[id(plan['vp_role'][1])] ** 2 / vals[id(plan['b_role'][1])]
+                vp_, b_ = vals[id(plan['vp_role'][1])], vals[id(plan['b_role'][1])]
+                want = vals[id(sf)] * dt * dt * (vp_ ** 2 / b_ if scale is None else scale(vp_, b_))
                 if abs(eval_scalar(ex, leaf) - want) > 1e-9 * abs(want):
-                    raise _Unrecognised("injected expression is not src*dt^2*vp^2/b")
+                    raise _Unrecognised(f"injected expression is not {what}")
             plan['src'] = sf
         if itps:
             self._attach_sparse(plan, [], itps, [plan['u']], funcs, consts, syms, None)
+
+    def _recognise_visco(self, updates, injs, itps):
+        """The reference's second-order SLS viscoacoustic pair (examples/seismic/viscoacoustic/operators.py:124-192,
+        kernel='sls', time_order=2): r.forward|backward, then p.forward|backward reading r at the level just written.
+        The radius and weights follow from the support of p; the roles of the parameter leaves (b, vp, qp and the
+        damping mask) are tried in turn, f0 is solved from the coefficient of r[t], and each candidate is checked by
+        comparing EVERY coefficient of both equations with `predict_visco` at probe values that vary linearly in
+        space (`_sa_probe`), so that where b, rho and tt are sampled changes the prediction."""
+        (r, e1), (p, e2) = updates
+        dirn = self._dirn
+        reads = lambda e, f: [k for k in (_space_offsets(a, None) for a in e.rhs.evaluate.preorder()
+                                          if a.is_Access and a.function is f) if k is not None]
+        r_in_p = reads(e2, r)
+        if not r_in_p or any(k[0] != dirn for k in r_in_p) or any(k[0] == dirn for k in reads(e1, p)):
+            raise _NotVisco("the second update does not read the first at the level just written")
+        grid = p.grid
+        nd = grid.dim
+        if nd not in (2, 3):
+            raise _Unrecognised("only 2-D/3-D grids")
+        so = p.space_order
+        if r.space_order != so or r.grid is not grid or r.time_size != p.time_size:
+            raise _Unrecognised("p and r differ in space order, grid or time slots")
+        keyed = []
+        for e in (e1, e2):
+            k_ = {}
+            for acc, coef in self._coeffs(e.rhs, [p, r]).items():
+                k = _space_offsets(acc, None)
+                if k is None:
+                    raise _Unrecognised("non-affine wavefield access")
+                k_[('p' if acc.function is p else 'r',) + k] = coef
+            keyed.append(k_)
+        reach = max((max(abs(o) for o in k[2]) for k in keyed[1] if k[0] == 'p'), default=0)
+        if reach % 2 == 0:
+            raise _Unrecognised("support is not that of nested half-node first derivatives")
+        R = (reach + 1) // 2
+        if 2 * R > so or R > 8:
+            raise _Unrecognised(f"radius {2 * R - 1} does not fit the halo of space_order {so}")
+        funcs, consts, syms = self._leaves(list(keyed[0].values()) + list(keyed[1].values()))
+        for a in funcs:
+            if getattr(a.function, 'is_TimeFunction', False):
+                raise _Unrecognised("a third wavefield in the coefficients")
+        dtsym = grid.stepping_dim.spacing
+        if dtsym.name not in {s.name for s in syms}:
+            raise _Unrecognised("no time spacing in the update")
+        known = {dtsym.name} | {sp.name for sp in grid.spacing_map}
+        for sym in syms:
+            if sym.name not in known:
+                raise _Unrecognised(f"unknown symbol {sym.name} in the update")
+        c = [sa_weights(R, h) for h in self._spacing_values(grid)]
+        fcands = [('f', a.function) for a in funcs]
+        cands = fcands + [('c', cst) for cst in consts]
+        rng = np.random.default_rng(1357)
+        probes = [self._sa_probe(rng, cands, grid) for _ in range(3)]
+        found = None
+        for roles in itertools.permutations(cands, 3):
+            for d_role in [x for x in fcands if all(x is not y for y in roles)] + [None]:
+                used = {id(x[1]) for x in roles + (d_role,) if x is not None}
+                if used != {id(x[1]) for x in cands}:
+                    continue
+                f0 = self._visco_f0(keyed, probes[0], roles, d_role, nd, dirn)
+                if f0 is not None and all(self._visco_matches(keyed, pr, roles, d_role, f0, c, R, nd, dirn)
+                                          for pr in probes):
+                    found = roles + (d_role, f0)
+                    break
+            if found:
+                break
+        if found is None:
+            raise _Unrecognised("coefficients are not those of the SLS update for any roles of b, vp, qp and damp")
+        b_role, vp_role, qp_role, d_role, f0 = found
+        plan = {'kind': 'visco', 'u': p, 'r': r, 'grid': grid, 'so': so, 'R': R, 'c': c, 'b_role': b_role,
+                'vp_role': vp_role, 'qp_role': qp_role, 'damp': d_role[1] if d_role else None,
+                'f0': float(np.float32(f0)), 'dt': dtsym, 'src': None, 'rec': None, 'rec_toff': 0,
+                'adjoint': dirn == -1}
+        self._attach_sa_sparse(plan, injs, itps, funcs, consts, syms, scale=lambda vp, b: vp * vp,
+                               what="src*dt^2/m")
+        return plan
+
+    @staticmethod
+    def _visco_f0(keyed, probe, roles, d_role, nd, dirn):
+        """f0 from the coefficient damp (1 - dt/t_s) of r[t] in the memory-variable update, or None."""
+        value, leaf, dt = probe
+        zero = (0,) * nd
+        coef = keyed[0].get(('r', 0, zero))
+        damp = value(d_role[1], zero) if d_role else 1.0
+        if coef is None:
+            return None
+        den = 1.0 - eval_scalar(coef, leaf) / damp
+        qp = value(roles[2][1], zero)
+        if den <= 0 or qp <= 0:
+            return None
+        t_s = dt / den
+        f0 = (np.sqrt(1.0 + 1.0 / qp ** 2) - 1.0 / qp) / t_s
+        return f0 if np.isfinite(f0) and f0 > 0 else None
+
+    def _visco_matches(self, keyed, probe, roles, d_role, f0, c, R, nd, dirn):
+        value, leaf, dt = probe
+        b_role, vp_role, qp_role = roles
+        zero = (0,) * nd
+        pred = predict_visco(c, R, nd, lambda off: value(b_role[1], off), lambda off: value(vp_role[1], off),
+                             lambda off: value(qp_role[1], off),
+                             (lambda off: value(d_role[1], off)) if d_role else (lambda off: 1.0), f0, dt, dirn)
+        for got_k, want in zip(keyed, pred):
+            got = {k: eval_scalar(v, leaf) for k, v in got_k.items()}
+            scale = max(abs(v) for v in want.values())
+            if set(got) != set(want) or any(abs(got[k] - want[k]) > 1e-9 * scale for k in want):
+                return False
+        return True
 
     def _recognise_ot4(self, u, keyed, star, R):
         """The reference's 4th-order-in-time acoustic update (examples/seismic/acoustic/operators.py:
@@ -1727,6 +1853,8 @@ class Operator:
         if grid.distributor.is_parallel:
             if p['kind'] == 'sa':
                 raise InvalidArgument("the self-adjoint update does not run on a decomposed grid in this version")
+            if p['kind'] == 'visco':
+                raise InvalidArgument("the SLS viscoacoustic update does not run on a decomposed grid in this version")
             if p['kind'] == 'tti' and grid.dim == 2:
                 raise InvalidArgument("2-D TTI modelling does not run on a decomposed grid in this version")
             if p['kind'] == 'tti' and p.get('adjoint'):
@@ -2021,6 +2149,11 @@ class Operator:
         if p['kind'] == 'sa':
             # per axis 2R fluxes of R multiply-adds and a multiply, then R outer multiply-adds; the update 6
             return float(nd * (2 * R * (2 * R + 1) + 2 * R) + 6), 24.0
+        if p['kind'] == 'visco':
+            # the nested operator as for 'sa'; the epilogue of b2_visco_point.cuh 16 (forward) or the mix 8 and the
+            # update 6 (adjoint); bytes of DESIGN §3.3k
+            lap = nd * (2 * R * (2 * R + 1) + 2 * R)
+            return (float(lap + 14), 64.0) if p.get('adjoint') else (float(lap + 16), 44.0)
         star = 1 + nd * R * 3                       # centre mul + per tap pair: add, multiply-add
         if p['kind'] == 'iso':
             arr = p['m_role'][0].endswith('_f')
@@ -2222,6 +2355,65 @@ def predict_sa(c, R, nd, bval, vp, w, dt, dirn):
                     key = (0, unit(d, m))
                     out[key] = out.get(key, 0.0) + C * a * bq * sgn * c[d][i - 1]
     return out
+
+
+# ---------------------------------------------------------------------------------------------
+# the SLS viscoacoustic pair as linear coefficients (float64) — used only by the recogniser
+# ---------------------------------------------------------------------------------------------
+def nested_taps(c, R, nd, bval):
+    """{offset: coefficient} of L(f) = sum_d sum_k c_k (F_d(p+(k-1)) - F_d(p-k)), F_d(q) = b(q) sum_i c_i (f(q+i) -
+    f(q-i+1)) at the output point; `bval(offset)` is b at that offset from it."""
+    out = {}
+
+    def unit(d, o):
+        e = [0] * nd
+        e[d] = o
+        return tuple(e)
+    for d in range(nd):
+        for j in range(-R, R):
+            a = c[d][j] if j >= 0 else -c[d][-j - 1]
+            bq = bval(unit(d, j))
+            for i in range(1, R + 1):
+                for m, sgn in ((j + i, 1.0), (j - i + 1, -1.0)):
+                    key = unit(d, m)
+                    out[key] = out.get(key, 0.0) + a * bq * sgn * c[d][i - 1]
+    return out
+
+
+def predict_visco(c, R, nd, bval, vpval, qpval, dval, f0, dt, dirn):
+    """({(field, time_shift, offsets): coefficient} of the memory-variable update, ... of the pressure update) of the
+    reference's sls_2nd_order (tests/visco_ref.py states the scheme). The parameters are callables of the offset from
+    the output point; the adjoint applies L to (1+tt) rho p and rho r[t-1], so there tt and rho are taken at the
+    nodes."""
+    zero = (0,) * nd
+
+    def relax(off):
+        q = qpval(off)
+        t_s = (np.sqrt(1.0 + 1.0 / q ** 2) - 1.0 / q) / f0
+        return t_s, 1.0 / (f0 ** 2 * t_s * t_s) - 1.0
+    t_s, tt = relax(zero)
+    damp = dval(zero)
+    m = 1.0 / vpval(zero) ** 2
+    e = (1.0 - damp) / dt
+    W = damp / (m / dt ** 2 + e)
+    L = nested_taps(c, R, nd, bval)
+    eq1 = {('r', 0, zero): damp * (1.0 - dt / t_s)}
+    eq2 = {}
+    if dirn == 1:
+        rho = 1.0 / bval(zero)
+        for off, w in L.items():
+            eq1[('p', 0, off)] = damp * dt * tt / t_s * rho * w
+            eq2[('p', 0, off)] = W * rho * (1.0 + tt) * w
+        eq2[('r', 1, zero)] = -W
+    else:
+        eq1[('p', 0, zero)] = -damp * dt * tt / t_s
+        for off, w in L.items():
+            rho = 1.0 / bval(off)
+            eq2[('p', 0, off)] = W * rho * (1.0 + relax(off)[1]) * w
+            eq2[('r', -1, off)] = W * rho * w
+    eq2[('p', 0, zero)] = eq2.get(('p', 0, zero), 0.0) + W * (2.0 * m / dt ** 2 + e)
+    eq2[('p', -dirn, zero)] = -W * m / dt ** 2
+    return eq1, eq2
 
 
 # ---------------------------------------------------------------------------------------------

@@ -11,3 +11,4 @@ from .tti import ForwardOperator as TTIForwardOperator  # noqa: F401
 from .self_adjoint import (SaIsoAcousticWaveSolver, IsoFwdOperator, IsoAdjOperator, setup_w_over_q,  # noqa: F401
                            acoustic_sa_setup)
 from .self_adjoint import iso_stencil as sa_iso_stencil  # noqa: F401
+from .viscoacoustic import ViscoacousticWaveSolver  # noqa: F401

@@ -285,7 +285,7 @@ def damp_profile(shape, padsizes, spacing, abc_type="damp", x_range=None):
 def demo_model(preset, **kwargs):
     """Preset models with the reference's names and defaults
     (examples/seismic/preset_models.py:20-238): `constant-isotropic`, `constant-tti`,
-    `layers-isotropic`, `layers-tti`."""
+    `layers-isotropic`, `layers-tti`, `layers-viscoacoustic`."""
     space_order = kwargs.pop('space_order', 2)
     shape = kwargs.pop('shape', (101, 101))
     spacing = kwargs.pop('spacing', tuple(10. for _ in shape))
@@ -328,4 +328,16 @@ def demo_model(preset, **kwargs):
         return SeismicModel(space_order=space_order, vp=v, origin=origin, shape=shape, dtype=dtype,
                             spacing=spacing, nbl=nbl, epsilon=.1 * (v - vp_top), delta=.05 * (v - vp_top),
                             theta=.5 * (v - vp_top), phi=phi, bcs="damp", **kwargs)
+    if p == 'layers-viscoacoustic':
+        vp_top = kwargs.pop('vp_top', 1.5)
+        vp_bottom = kwargs.pop('vp_bottom', 3.5)
+        v = np.empty(shape, dtype=dtype)
+        v[:] = vp_top
+        vp_i = np.linspace(vp_top, vp_bottom, nlayers)
+        for i in range(1, nlayers):
+            v[..., i * int(shape[-1] / nlayers):] = vp_i[i]
+        qp = (3.516 * ((v * 1000.) ** 2.2) * 10 ** (-6)).astype(dtype)     # Li's empirical formula
+        b = (1.0 / (0.31 * (1e3 * v) ** 0.25)).astype(dtype)               # Gardner's density, not normalised
+        return SeismicModel(space_order=space_order, vp=v, qp=qp, b=b, nbl=nbl, dtype=dtype, origin=origin,
+                            shape=shape, spacing=spacing, **kwargs)
     raise ValueError(f"unknown or unsupported preset {preset!r}")

@@ -300,6 +300,53 @@ struct b2_sa_args {
 };
 int b2_sa_forward(const struct b2_sa_args *a);
 
+/* ---- second-order SLS viscoacoustic modelling (replaces the generated `ForwardOperator` / `AdjointOperator` of
+ *      examples/seismic/viscoacoustic at kernel='sls', time_order=2, operators.py:124-192) ------------------------
+ * With L(f) = sum_d sum_k c_d[k-1] (F_d(p + (k-1) e_d) - F_d(p - k e_d)), F_d(q) = b(q) sum_k c_d[k-1] (f(q + k e_d) -
+ * f(q - (k-1) e_d)) (the nested operator of b2_sa_forward, b at the nodes), t_s = (sqrt(1 + 1/qp^2) - 1/qp) / f0,
+ * tt = 1/(f0^2 t_s^2) - 1, m = 1/vp^2, rho = 1/b and damp the "mask" profile (NULL: 1):
+ *   r[t+1] = damp solve(r.dt - (tt/t_s) rho L(p) + r/t_s, r[t+1])
+ *   p[t+1] = damp solve(m p.dt2 - rho (1+tt) L(p) + r[t+1] + (1-damp) p.dt, p[t+1])
+ * with r.dt, p.dt the first-order forward differences (f[t+1] - f[t]) / dt and .dt.T = (f[t-1] - f[t]) / dt; then p[t+1][cell] += w.w.w * src[t][p] * dt^2 vp^2 and rec[t][p] samples p[t + rec_toff].
+ * With `adjoint` time runs from time_M down to time_m:
+ *   r[t-1] = damp solve(r.dt.T + (tt/t_s) p + r/t_s, r[t-1])
+ *   p[t-1] = damp solve(m p.dt2 - L((1+tt) rho p) - L(rho r[t-1]) + (1-damp) p.dt.T, p[t-1])
+ * `src` (the receiver data) is injected into p[t-1] with the same scale and `rec` (the adjoint source) samples p[t].
+ * p (`u`) and r have the same layout. Not combined with halo exchange or a free surface (210). kernel 0 runs the
+ * 2.5-D TMA sweep k_visco_tma<R> when the layout qualifies (3-D, radius 2 or 4, z extent and z start multiples of 4,
+ * 16-byte aligned arrays), else the one-thread-per-point kernel; kernel 2 on a layout that does not qualify returns
+ * 210. b2_last_sweep_kernel reports "visco_tma<R>" or "visco_generic", with "+adj" on adjoint calls. */
+struct b2_visco_args {
+    int ndim;                         /* 2 or 3                                                      */
+    int space_order;                  /* halo width of p / r / b / vp / qp / damp                    */
+    int radius;                       /* R <= space_order/2 (the nested stencil reaches 2R-1 points)  */
+    const float *c[3];                /* per-dim weights incl. 1/h: c[d][0..radius-1]                */
+    struct b2_dataobj *u;             /* p: (tsize, x+2so, y+2so[, z+2so]); tsize 3 or nt (save=True) */
+    struct b2_dataobj *r;             /* the memory variable, p's layout                             */
+    struct b2_dataobj *b;             /* buoyancy array, or NULL -> b_value                          */
+    float b_value;
+    struct b2_dataobj *vp;            /* velocity array, or NULL -> vp_value                         */
+    float vp_value;
+    struct b2_dataobj *qp;            /* quality-factor array, or NULL -> qp_value                   */
+    float qp_value;
+    struct b2_dataobj *damp;          /* mask profile, or NULL -> 1                                  */
+    float f0;                         /* reference frequency of the relaxation times                 */
+    float dt;
+    int x_m, x_M, y_m, y_M, z_m, z_M; /* for ndim==2 the z entries are ignored                       */
+    int time_m, time_M;
+    struct b2_sparse *src;            /* injected into the level written                             */
+    struct b2_sparse *rec;            /* samples p[t] (rec_toff 0) or the level written              */
+    int rec_toff;
+    int adjoint;
+    int errctl;                       /* !=0: NaN check of p and r every 100 steps -> return 100      */
+    int deviceid;
+    int kernel;                       /* 0 auto, 1 generic, 2 TMA (210 if the layout does not take it) */
+    b2_halo_ctx *halo;                /* must be NULL                                                */
+    int free_surface;                 /* must be 0                                                   */
+    struct b2_profiler *timers;       /* may be NULL; section0 accumulates the loop time             */
+};
+int b2_visco_forward(const struct b2_visco_args *a);
+
 /* ---- generic explicit update with constant coefficients --------------------------------------
  * Any Operator whose single equation is  f[t + wshift][p] = sum_k coef_k * f[t + tshift_k][p + off_k]
  * with coefficients that do not depend on position (Constants, spacings, dt) — e.g. the reference's
@@ -442,7 +489,7 @@ void   b2_kernel_timing_enable(int on);
  * selected at run time (layout checks, B2_* switches): this tells which one computed the answer. A TTI Born call
  * appends the path of its source term: "+born_v4" (float4 along z) or "+born_s" (one point per thread); a TTI
  * adjoint call appends "+adj" to the variant that ran its sweep. b2_sa_forward reports "sa_tma<R>" or "sa_generic", with "+adj" on
- * adjoint calls. */
+ * adjoint calls; b2_visco_forward "visco_tma<R>" or "visco_generic", with "+adj" on adjoint calls. */
 const char *b2_last_sweep_kernel(void);
 /* number of x-planes of the last b2_iso_forward call whose update coefficient A = 1/(m/dt^2 + damp/dt) the
  * TMA sweep took from the one tile it pins per CTA instead of streaming it: the planes of the update box whose
