@@ -98,6 +98,18 @@ inline int env_int(const char *name, int dflt) {
 // ring-buffer slot of time level `time` in an array of T slots
 inline int slot(int time, int T) { return ((time % T) + T) % T; }
 
+// TMA tensor map over a dense f32 array of `rank` (3 or 4) dims, extents `dims` innermost first (z, y, x[, t]), box
+// (bz, by, 1[, 1]). B2_ERR_DEVICE after set_error naming `who` when the driver cannot encode it.
+int encode_tmap(CUtensorMap *tm, const void *base, int rank, const int *dims, int bz, int by, const char *who);
+
+// One buffer of device scratch that a sweep file keeps across calls (released with the process).
+struct ScratchSlot {
+    float *p = nullptr;
+    size_t elems = 0;
+};
+// `*out` = slot s holding `elems` floats, re-allocated when its size differs (uninitialised then)
+int cached_scratch(ScratchSlot &s, size_t elems, float **out);
+
 // A dense f32/i32 array made device-visible: either resident (dmap) or staged by us.
 struct DevArray {
     void *d = nullptr;       // device pointer

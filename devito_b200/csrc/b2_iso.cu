@@ -729,48 +729,6 @@ k_iso_coef(const float *__restrict__ damp, const float *__restrict__ param, int 
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *,
-                                    const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                    const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled get_encode() {
-    static PFN_encodeTiled fn = nullptr;
-    if (fn) return fn;
-    void *p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-        return nullptr;
-    fn = reinterpret_cast<PFN_encodeTiled>(p);
-    return fn;
-}
-
-// tensor map over a (t?, x, y, z) f32 array; box = (bz, by, 1[, 1])
-static int make_tmap(CUtensorMap *tm, const void *base, int rank, const int *dims_zyxt,
-                     int bz, int by) {
-    PFN_encodeTiled enc = get_encode();
-    if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return B2_ERR_DEVICE; }
-    cuuint64_t gdim[4];
-    cuuint64_t gstr[3];
-    cuuint32_t box[4] = {(cuuint32_t)bz, (cuuint32_t)by, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    cuuint64_t stride = 4;
-    for (int i = 0; i < rank; ++i) {
-        gdim[i] = (cuuint64_t)dims_zyxt[i];
-        stride *= gdim[i];
-        if (i < rank - 1) gstr[i] = stride;
-    }
-    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void *>(base),
-                     gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled failed (%d) rank=%d box=(%d,%d)", (int)r, rank, bz, by);
-        return B2_ERR_DEVICE;
-    }
-    return B2_OK;
-}
-
 // tile configuration per radius (TY, TZ4) and coefficient kind (ARR: an array vp|m streams a third tile):
 // sized so that the Q-stage plane ring plus the (R+1)-stage tile ring fit the 227 KB of shared memory of one SM.
 // so=8 with a scalar vp: 16 x 128, so that every TMA box row and every warp's store is 512 contiguous bytes
@@ -783,21 +741,8 @@ template <> struct TileOf<4, true> { static constexpr int TY = 32, TZ4 = 16; };
 template <bool ARR> struct TileOf<6, ARR> { static constexpr int TY = 16, TZ4 = 16; };
 template <bool ARR> struct TileOf<8, ARR> { static constexpr int TY = 8, TZ4 = 16; };
 
-// scratch for the coefficient arrays, cached across calls (re-allocated when the size changes)
-static float *g_coef[3] = {nullptr, nullptr, nullptr};     // A, B (TMA path), W (OT4)
-static size_t g_coef_elems[3] = {0, 0, 0};
-
-static int coef_buffer(int which, size_t elems, float **out) {
-    if (g_coef_elems[which] != elems) {
-        if (g_coef[which]) cudaFree(g_coef[which]);
-        g_coef[which] = nullptr;
-        g_coef_elems[which] = 0;
-        B2_CUDA(cudaMalloc(&g_coef[which], elems * sizeof(float)), B2_ERR_MEMORY);
-        g_coef_elems[which] = elems;
-    }
-    *out = g_coef[which];
-    return B2_OK;
-}
+// scratch for the coefficient arrays, cached across calls: A, B (TMA path), W (OT4)
+static ScratchSlot g_coef[3];
 
 // rows [y0, y1) of the planes [x0, x1) (allocated indices): the y-skewed streamed loop tabulates row blocks
 __global__ void __launch_bounds__(256)
@@ -917,10 +862,10 @@ int iso_coef_reuse_count() {
 
 static int iso_coef_tabulate(IsoPlan &p) {
     int rc;
-    if ((rc = coef_buffer(0, p.slot_elems, &p.coefA))) return rc;
+    if ((rc = cached_scratch(g_coef[0], p.slot_elems, &p.coefA))) return rc;
     p.coefB = nullptr;
     if (p.param_kind != B2_PARAM_SCALAR)
-        if ((rc = coef_buffer(1, p.slot_elems, &p.coefB))) return rc;
+        if ((rc = cached_scratch(g_coef[1], p.slot_elems, &p.coefB))) return rc;
     if (p.defer_coef) return B2_OK;          // the caller tabulates plane ranges itself
     return iso_coef_tabulate_all(p);
 }
@@ -934,11 +879,11 @@ static int plan_tma(IsoPlan &p) {
     const int dims4[4] = {p.a[2], p.a[1], p.a[0], p.tsize};
     const int dims3[3] = {p.a[2], p.a[1], p.a[0]};
     int rc;
-    if ((rc = make_tmap(&p.tm_uh, p.u, 4, dims4, 4 * TZ4 + 2 * RZ, TY + 2 * R))) return rc;
-    if ((rc = make_tmap(&p.tm_uc, p.u, 4, dims4, 4 * TZ4, TY))) return rc;
-    if ((rc = make_tmap(&p.tm_damp, p.coefA, 3, dims3, 4 * TZ4, TY))) return rc;
+    if ((rc = encode_tmap(&p.tm_uh, p.u, 4, dims4, 4 * TZ4 + 2 * RZ, TY + 2 * R, "iso"))) return rc;
+    if ((rc = encode_tmap(&p.tm_uc, p.u, 4, dims4, 4 * TZ4, TY, "iso"))) return rc;
+    if ((rc = encode_tmap(&p.tm_damp, p.coefA, 3, dims3, 4 * TZ4, TY, "iso"))) return rc;
     if (arr) {
-        if ((rc = make_tmap(&p.tm_par, p.coefB, 3, dims3, 4 * TZ4, TY))) return rc;
+        if ((rc = encode_tmap(&p.tm_par, p.coefB, 3, dims3, 4 * TZ4, TY, "iso"))) return rc;
     } else {
         p.tm_par = p.tm_damp;
     }
@@ -969,7 +914,7 @@ int iso_plan_init(IsoPlan &p, int kernel) {
             }
         }
         p.use_tma = false;
-        return coef_buffer(2, p.slot_elems, &p.ot4W);
+        return cached_scratch(g_coef[2], p.slot_elems, &p.ot4W);
     }
     if (kernel == 2 && !ok) {
         set_error("iso: TMA kernel forced but layout does not qualify (radius=%d a2=%d o2=%d)", R,
@@ -1192,10 +1137,10 @@ int iso2_prepare(const IsoPlan &p, float *scratch[2]) {
     const int dims4s[4] = {p.a[2], p.a[1], p.a[0], 2};
     const int dims3[3] = {p.a[2], p.a[1], p.a[0]};
     int rc;
-    if ((rc = make_tmap(&g_s2_tm_uh, p.u, 4, dims4, C::BZ, C::BY))) return rc;
-    if ((rc = make_tmap(&g_s2_tm_uh_s, g_s2, 4, dims4s, C::BZ, C::BY))) return rc;
-    if ((rc = make_tmap(&g_s2_tm_uc, p.u, 4, dims4, C::EZ, C::EY))) return rc;
-    if ((rc = make_tmap(&g_s2_tm_a, p.coefA, 3, dims3, C::EZ, C::EY))) return rc;
+    if ((rc = encode_tmap(&g_s2_tm_uh, p.u, 4, dims4, C::BZ, C::BY, "iso"))) return rc;
+    if ((rc = encode_tmap(&g_s2_tm_uh_s, g_s2, 4, dims4s, C::BZ, C::BY, "iso"))) return rc;
+    if ((rc = encode_tmap(&g_s2_tm_uc, p.u, 4, dims4, C::EZ, C::EY, "iso"))) return rc;
+    if ((rc = encode_tmap(&g_s2_tm_a, p.coefA, 3, dims3, C::EZ, C::EY, "iso"))) return rc;
     scratch[0] = g_s2;
     scratch[1] = g_s2 + p.slot_elems;
     return B2_OK;

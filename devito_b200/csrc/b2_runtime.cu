@@ -231,6 +231,52 @@ int Staging::finish(int code) {
     return code;
 }
 
+int cached_scratch(ScratchSlot &s, size_t elems, float **out) {
+    if (s.elems != elems) {
+        if (s.p) cudaFree(s.p);
+        s.p = nullptr;
+        s.elems = 0;
+        B2_CUDA(cudaMalloc(&s.p, elems * sizeof(float)), B2_ERR_MEMORY);
+        s.elems = elems;
+    }
+    *out = s.p;
+    return B2_OK;
+}
+
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
+                                    const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+int encode_tmap(CUtensorMap *tm, const void *base, int rank, const int *dims, int bz, int by, const char *who) {
+    static PFN_encodeTiled enc = nullptr;     // the driver entry point, looked up on first use
+    if (!enc) {
+        void *fp = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess) {
+            set_error("%s: cuTensorMapEncodeTiled entry point not available", who);
+            return B2_ERR_DEVICE;
+        }
+        enc = reinterpret_cast<PFN_encodeTiled>(fp);
+    }
+    cuuint64_t gdim[4], gstr[3];
+    cuuint32_t box[4] = {(cuuint32_t)bz, (cuuint32_t)by, 1, 1}, estr[4] = {1, 1, 1, 1};
+    cuuint64_t stride = 4;
+    for (int i = 0; i < rank; ++i) {
+        gdim[i] = (cuuint64_t)dims[i];
+        stride *= gdim[i];
+        if (i < rank - 1) gstr[i] = stride;
+    }
+    const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void *>(base), gdim, gstr,
+                           box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("%s: cuTensorMapEncodeTiled failed (%d) rank=%d box=(%d,%d)", who, (int)r, rank, bz, by);
+        return B2_ERR_DEVICE;
+    }
+    return B2_OK;
+}
+
 int grid_halo(const char *who, const char *name, const b2_dataobj *obj, const DevArray &x, int lead,
               const DevArray &u, int nd, int so, int need) {
     const int n0 = u.size[1] - 2 * so;                   // the grid's extent on the first space dim

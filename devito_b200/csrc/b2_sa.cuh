@@ -16,14 +16,14 @@ struct SaPlan : Box {
     // library scratch: C = dt^2 vp^2 / b, and b expanded when it is a scalar
     float *C = nullptr, *b = nullptr;
     bool adjoint = false;
-    // k_sa_tma<R> (3-D, R in {2, 4}, z rows and the box start 16-byte aligned): tensor maps of the haloed u[t] plane
+    // sa_tma<R> (3-D, R in {2, 4}, z rows and the box start 16-byte aligned): tensor maps of the haloed u[t] plane
     // (all slots; the slot is a coordinate) and of the haloed b plane
     bool use_tma = false;
     CUtensorMap tm_u, tm_b;
 };
 
 // Checks the layout, allocates the scratch and tabulates C (and b) over the whole allocated slot.
-// kernel: 0 auto (k_sa_tma<R> when the layout qualifies, else k_sa_generic), 1 generic, 2 TMA (210 with a message
+// kernel: 0 auto (sa_tma<R> when the layout qualifies, else k_sa_generic), 1 generic, 2 TMA (210 with a message
 // when the layout does not qualify).
 int sa_plan_init(SaPlan &p, int kernel);
 

@@ -1349,34 +1349,6 @@ k_tti_coef(const float *__restrict__ damp, float m_dt2, float inv_dt, float *__r
     for (; i < n; i += stride) A[i] = 1.0f / (m_dt2 + (damp ? damp[i] * inv_dt : 0.f));
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *,
-                                    const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                    const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static int tti_make_tmap(CUtensorMap *tm, const void *base, const int *a, int tsize, int bz, int by) {
-    static PFN_encodeTiled enc = nullptr;
-    if (!enc) {
-        void *fp = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &q) != cudaSuccess ||
-            q != cudaDriverEntryPointSuccess) {
-            set_error("cuTensorMapEncodeTiled entry point not available");
-            return B2_ERR_DEVICE;
-        }
-        enc = reinterpret_cast<PFN_encodeTiled>(fp);
-    }
-    cuuint64_t gdim[4] = {(cuuint64_t)a[2], (cuuint64_t)a[1], (cuuint64_t)a[0], (cuuint64_t)tsize};
-    cuuint64_t gstr[3] = {gdim[0] * 4, gdim[0] * gdim[1] * 4, gdim[0] * gdim[1] * gdim[2] * 4};
-    cuuint32_t box[4] = {(cuuint32_t)bz, (cuuint32_t)by, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void *>(base), gdim, gstr, box,
-                     estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (tti) failed: %d", (int)r); return B2_ERR_DEVICE; }
-    return B2_OK;
-}
-
 static bool tti_use_ws(int R);
 constexpr int kTtiWsTY = 24;
 template <int R> struct TtiTile;
@@ -1391,19 +1363,7 @@ template <> struct TtiArrTile<4> { static constexpr int TY = 20; };
 
 // scratch cached across calls
 // 0: A, 1-2: Gz(u), Gz(v) (two-pass), 3-8: per-point tables, 9-10: the adjoint's mixes
-static float *g_tti_scratch[11] = {};
-static size_t g_tti_scratch_elems[11] = {};
-static int tti_scratch(int which, size_t elems, float **out) {
-    if (g_tti_scratch_elems[which] != elems) {
-        if (g_tti_scratch[which]) cudaFree(g_tti_scratch[which]);
-        g_tti_scratch[which] = nullptr;
-        g_tti_scratch_elems[which] = 0;
-        B2_CUDA(cudaMalloc(&g_tti_scratch[which], elems * sizeof(float)), B2_ERR_MEMORY);
-        g_tti_scratch_elems[which] = elems;
-    }
-    *out = g_tti_scratch[which];
-    return B2_OK;
-}
+static ScratchSlot g_tti_scratch[11];
 
 // the per-point tables of k_tti_tables (array-valued parameters)
 static int tti_tables(TtiPlan &p) {
@@ -1411,7 +1371,7 @@ static int tti_tables(TtiPlan &p) {
     B2_SM_COUNT(sms);
     float **t[6] = {&p.tCx, &p.tCy, &p.tCz, &p.tE2, &p.tSD, &p.tMD};
     for (int i = p.ndim == 2; i < 6; ++i)      // a 2-D plan has no rotation factor on its dummy dim: tCx stays NULL
-        if ((rc = tti_scratch(3 + i, p.slot_elems, t[i]))) return rc;
+        if ((rc = cached_scratch(g_tti_scratch[3 + i], p.slot_elems, t[i]))) return rc;
     k_tti_tables<<<sms * 8, 256, 0, stream()>>>(p.vp_a, p.eps_a, p.delta_a, p.theta_a, p.phi_a, p.vp, p.epsilon,
                                                  p.delta, p.theta, p.phi, 1.0f / (p.dt * p.dt), p.tCx, p.tCy, p.tCz,
                                                  p.tE2, p.tSD, p.tMD, p.slot_elems, p.ndim == 2);
@@ -1423,9 +1383,10 @@ static int tti_tables(TtiPlan &p) {
 // tensor maps of the 2-D sweep over the field pair (u, v) of `tsize` slots: boxes of one row segment
 static int tti2d_maps(const TtiPlan &p, const float *u, const float *v, int tsize, TtiPlan &out) {
     constexpr int BOXZ = Tti2dCfg<2, false>::BOXZ;
+    const int dims[4] = {p.a[2], p.a[1], p.a[0], tsize};
     int rc;
-    if ((rc = tti_make_tmap(&out.tm_u, u, p.a, tsize, BOXZ, 1))) return rc;
-    return tti_make_tmap(&out.tm_v, v, p.a, tsize, BOXZ, 1);
+    if ((rc = encode_tmap(&out.tm_u, u, 4, dims, BOXZ, 1, "tti"))) return rc;
+    return encode_tmap(&out.tm_v, v, 4, dims, BOXZ, 1, "tti");
 }
 
 static int tti_plan_init_2d(TtiPlan &p, int kernel) {
@@ -1440,10 +1401,10 @@ static int tti_plan_init_2d(TtiPlan &p, int kernel) {
     int rc;
     if (p.has_arrays && (rc = tti_tables(p))) return rc;
     if (!ok) {
-        if ((rc = tti_scratch(1, p.slot_elems, &p.gzu))) return rc;
-        return tti_scratch(2, p.slot_elems, &p.gzv);
+        if ((rc = cached_scratch(g_tti_scratch[1], p.slot_elems, &p.gzu))) return rc;
+        return cached_scratch(g_tti_scratch[2], p.slot_elems, &p.gzv);
     }
-    if ((rc = tti_scratch(0, p.slot_elems, &p.coefA))) return rc;
+    if ((rc = cached_scratch(g_tti_scratch[0], p.slot_elems, &p.coefA))) return rc;
     B2_SM_COUNT(sms);
     const float inv_dt = 1.0f / p.dt;
     if (p.has_arrays)
@@ -1456,8 +1417,9 @@ static int tti_plan_init_2d(TtiPlan &p, int kernel) {
     if ((rc = tti2d_maps(p, p.u, p.v, p.tsize, p))) return rc;
     if (p.has_arrays) {       // sin(th), cos(th) of `Gzz_centered_2d`
         constexpr int BOXZ = Tti2dCfg<2, false>::BOXZ;
-        if ((rc = tti_make_tmap(&p.tm_cy, p.tCy, p.a, 1, BOXZ, 1))) return rc;
-        if ((rc = tti_make_tmap(&p.tm_cz, p.tCz, p.a, 1, BOXZ, 1))) return rc;
+        const int dims1[4] = {p.a[2], p.a[1], p.a[0], 1};
+        if ((rc = encode_tmap(&p.tm_cy, p.tCy, 4, dims1, BOXZ, 1, "tti"))) return rc;
+        if ((rc = encode_tmap(&p.tm_cz, p.tCz, 4, dims1, BOXZ, 1, "tti"))) return rc;
     }
     return B2_OK;
 }
@@ -1489,7 +1451,7 @@ int tti_plan_init(TtiPlan &p, int kernel) {
     B2_SM_COUNT(sms);
     auto tables = [&]() -> int { return tti_tables(p); };
     if (ok) {
-        if ((rc = tti_scratch(0, p.slot_elems, &p.coefA))) return rc;
+        if ((rc = cached_scratch(g_tti_scratch[0], p.slot_elems, &p.coefA))) return rc;
         const float inv_dt = 1.0f / p.dt;
         int ty;
         if (p.arr_fused) {
@@ -1504,17 +1466,18 @@ int tti_plan_init(TtiPlan &p, int kernel) {
         count_launch();
         B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
         p.tm_rows = ty + 2 * p.R;
-        if ((rc = tti_make_tmap(&p.tm_u, p.u, p.a, p.tsize, 72, ty + 2 * p.R))) return rc;
-        if ((rc = tti_make_tmap(&p.tm_v, p.v, p.a, p.tsize, 72, ty + 2 * p.R))) return rc;
+        const int dims[4] = {p.a[2], p.a[1], p.a[0], p.tsize}, dims1[4] = {p.a[2], p.a[1], p.a[0], 1};
+        if ((rc = encode_tmap(&p.tm_u, p.u, 4, dims, 72, ty + 2 * p.R, "tti"))) return rc;
+        if ((rc = encode_tmap(&p.tm_v, p.v, 4, dims, 72, ty + 2 * p.R, "tti"))) return rc;
         if (p.arr_fused) {  // boxes of the Gz tile (TY + R rows) over the factor tables
-            if ((rc = tti_make_tmap(&p.tm_cx, p.tCx, p.a, 1, 72, ty + p.R))) return rc;
-            if ((rc = tti_make_tmap(&p.tm_cy, p.tCy, p.a, 1, 72, ty + p.R))) return rc;
-            if ((rc = tti_make_tmap(&p.tm_cz, p.tCz, p.a, 1, 72, ty + p.R))) return rc;
+            if ((rc = encode_tmap(&p.tm_cx, p.tCx, 4, dims1, 72, ty + p.R, "tti"))) return rc;
+            if ((rc = encode_tmap(&p.tm_cy, p.tCy, 4, dims1, 72, ty + p.R, "tti"))) return rc;
+            if ((rc = encode_tmap(&p.tm_cz, p.tCz, 4, dims1, 72, ty + p.R, "tti"))) return rc;
         }
         return B2_OK;
     }
-    if ((rc = tti_scratch(1, p.slot_elems, &p.gzu))) return rc;
-    if ((rc = tti_scratch(2, p.slot_elems, &p.gzv))) return rc;
+    if ((rc = cached_scratch(g_tti_scratch[1], p.slot_elems, &p.gzu))) return rc;
+    if ((rc = cached_scratch(g_tti_scratch[2], p.slot_elems, &p.gzv))) return rc;
     if (p.has_arrays && (rc = tables())) return rc;
     return B2_OK;
 }
@@ -1530,16 +1493,16 @@ int tti_plan_retarget(const TtiPlan &p, float *u, float *v, TtiPlan &out) {
     }
     int rc;
     if (p.use_2d) return tti2d_maps(p, u, v, p.tsize, out);
-    if ((rc = tti_make_tmap(&out.tm_u, u, p.a, p.tsize, 72, p.tm_rows))) return rc;
-    if ((rc = tti_make_tmap(&out.tm_v, v, p.a, p.tsize, 72, p.tm_rows))) return rc;
-    return B2_OK;
+    const int dims[4] = {p.a[2], p.a[1], p.a[0], p.tsize};
+    if ((rc = encode_tmap(&out.tm_u, u, 4, dims, 72, p.tm_rows, "tti"))) return rc;
+    return encode_tmap(&out.tm_v, v, 4, dims, 72, p.tm_rows, "tti");
 }
 
 int tti_plan_adjoint(const TtiPlan &p, TtiPlan &out) {
     float *a = nullptr, *b = nullptr;
     int rc;
-    if ((rc = tti_scratch(9, p.slot_elems, &a))) return rc;
-    if ((rc = tti_scratch(10, p.slot_elems, &b))) return rc;
+    if ((rc = cached_scratch(g_tti_scratch[9], p.slot_elems, &a))) return rc;
+    if ((rc = cached_scratch(g_tti_scratch[10], p.slot_elems, &b))) return rc;
     out = p;                // tables, A and two-pass scratch shared; u / v stay p / r
     out.ma = a;
     out.mb = b;
@@ -1548,8 +1511,9 @@ int tti_plan_adjoint(const TtiPlan &p, TtiPlan &out) {
     if (p.use_fused) {      // one slot each (cudaMalloc'ed, so 16-byte aligned): the sweep reads slot 0 of the maps
         // the scalar so=8 adjoint sweeps with k_tti_fused<4> where the forward takes k_tti_ws (its own tile height)
         if (!p.arr_fused) out.tm_rows = (p.R == 2 ? TtiTile<2>::TY : TtiTile<4>::TY) + 2 * p.R;
-        if ((rc = tti_make_tmap(&out.tm_u, a, p.a, 1, 72, out.tm_rows))) return rc;
-        if ((rc = tti_make_tmap(&out.tm_v, b, p.a, 1, 72, out.tm_rows))) return rc;
+        const int dims1[4] = {p.a[2], p.a[1], p.a[0], 1};
+        if ((rc = encode_tmap(&out.tm_u, a, 4, dims1, 72, out.tm_rows, "tti"))) return rc;
+        if ((rc = encode_tmap(&out.tm_v, b, 4, dims1, 72, out.tm_rows, "tti"))) return rc;
     }
     return B2_OK;
 }

@@ -18,14 +18,14 @@ struct ViscoPlan : Box {
     float *K[VK_NTAB] = {};
     float *b = nullptr, *s = nullptr;
     bool adjoint = false;
-    // k_visco_tma<R> (3-D, R in {2, 4}, z rows and the box start 16-byte aligned): tensor maps of the haloed plane of
+    // visco_tma<R> (3-D, R in {2, 4}, z rows and the box start 16-byte aligned): tensor maps of the haloed plane of
     // the field L is applied to (p, every slot, the slot a coordinate; or s) and of the haloed b plane
     bool use_tma = false;
     CUtensorMap tm_f, tm_b;
 };
 
 // Checks the layout, allocates the scratch and tabulates the tables (and b) over the whole allocated slot.
-// kernel: 0 auto (k_visco_tma<R> when the layout qualifies, else k_visco_generic), 1 generic, 2 TMA (210 with a
+// kernel: 0 auto (visco_tma<R> when the layout qualifies, else k_visco_generic), 1 generic, 2 TMA (210 with a
 // message when the layout does not qualify).
 int visco_plan_init(ViscoPlan &p, int kernel);
 

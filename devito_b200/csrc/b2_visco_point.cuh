@@ -1,12 +1,14 @@
 // One-point form of the second-order SLS viscoacoustic update (b2_visco_forward).
 //
 // `__host__ __device__`, like b2_sa_point.cuh, so that tests/support/emu_visco.cu can run the same code (the tables,
-// the adjoint's mix and the point body) on the CPU and compare it with the float64 restatement without a GPU. The scheme is the reference's `sls_2nd_order`
-// (examples/seismic/viscoacoustic/operators.py:124-192). With the nested operator of the self-adjoint update
+// the adjoint's mix and the point body) on the CPU and compare it with the float64 restatement without a GPU. The
+// scheme is the reference's `sls_2nd_order` (examples/seismic/viscoacoustic/operators.py:124-192). With the nested
+// operator of the self-adjoint update
 //
 //   F_d(q) = b(q) * sum_k c_k [f(q + k e_d) - f(q - (k-1) e_d)],   L(f)(p) = sum_d sum_k c_k [F_d(p + (k-1) e_d) - F_d(p - k e_d)]
 //
-// (b at the nodes, c_k = the half-node first-derivative weights divided by h_d) and the per-point tables of
+// (b at the nodes, c_k = the half-node first-derivative weights divided by h_d), whose code both updates share
+// (nested_div of b2_nested_point.cuh here, k_nested_tma of b2_nested.cuh in the TMA sweep), and the per-point tables of
 // k_visco_coef (t_s, tt from qp and f0, m = 1/vp^2, damp the "mask" profile, e = (1 - damp) / dt):
 //
 //   Kd = damp,  Kg = dt damp / t_s,  Kt = tt,  W = damp / (m/dt^2 + e),  Wm = W m / dt^2
@@ -20,7 +22,7 @@
 //   s      = ((1 + Kt) p[t] + r[t-1]) / b                                        (everywhere)
 //   p[t-1] = W L(s) + Wm (2 p[t] - p[t+1]) + (Kd - Wm) p[t]
 #pragma once
-#include "b2_common.cuh"
+#include "b2_nested_point.cuh"
 #include <cmath>
 
 namespace b2 {
@@ -51,26 +53,6 @@ B2_VISCO_HD long long visco_index(const ViscoK &k, int x, int y, int z) {
     return (long long)(k.o0 + x) * k.sx + (long long)(k.o1 + y) * k.sy + (k.o2 + z);
 }
 
-// F_d at node q along stride s
-B2_VISCO_HD float visco_flux(const ViscoK &k, const float *__restrict__ c, int R, long long q, long long s) {
-    float acc = 0.f;
-    for (int i = 1; i <= R; ++i) acc += c[i - 1] * (k.f[q + i * s] - k.f[q - (i - 1) * s]);
-    return k.b[q] * acc;
-}
-
-B2_VISCO_HD float visco_div(const ViscoK &k, long long idx) {
-    float acc = 0.f;
-    const long long st[3] = {k.sx, k.sy, 1};
-    for (int d = 0; d < 3; ++d) {
-        const int R = k.r[d];
-        const long long s = st[d];
-        for (int i = 1; i <= R; ++i)
-            acc += k.c[d][i - 1] *
-                   (visco_flux(k, k.c[d], R, idx + (i - 1) * s, s) - visco_flux(k, k.c[d], R, idx - i * s, s));
-    }
-    return acc;
-}
-
 // the epilogue shared by both sweeps: given L at the point, the tables and the levels read, write the point
 B2_VISCO_HD void visco_update(const ViscoK &k, long long idx, float lap, float bc) {
     const float kd = k.K[VK_D][idx], w = k.K[VK_W][idx], wm = k.K[VK_WM][idx];
@@ -88,7 +70,7 @@ B2_VISCO_HD void visco_update(const ViscoK &k, long long idx, float lap, float b
 
 B2_VISCO_HD void visco_point(const ViscoK &k, int x, int y, int z) {
     const long long idx = visco_index(k, x, y, z);
-    visco_update(k, idx, visco_div(k, idx), k.b[idx]);
+    visco_update(k, idx, nested_div(k.f, k.b, k.sx, k.sy, k.r, k.c, idx), k.b[idx]);
 }
 
 // The adjoint's pointwise pass (k_visco_adj_mix) over the whole allocated slot.

@@ -269,7 +269,7 @@ int b2_tti_forward(const struct b2_tti_args *a);
  * at the cell, and rec[t][p] samples u[t + rec_toff]. With `adjoint` the same formula writes u[t-1] from u[t] and
  * u[t+1], time runs from time_M down to time_m, `src` (the receiver data) is injected into u[t-1] with the same scale
  * and `rec` (the adjoint source) samples u[t] (rec_toff 0) or u[t-1] (rec_toff != 0).
- * Not combined with halo exchange or a free surface (210). kernel 0 runs the 2.5-D TMA sweep k_sa_tma<R> when the
+ * Not combined with halo exchange or a free surface (210). kernel 0 runs the 2.5-D TMA sweep sa_tma<R> when the
  * layout qualifies (3-D, radius 2 or 4, z extent and z start multiples of 4, 16-byte aligned arrays), else the
  * one-thread-per-point kernel; kernel 2 on a layout that does not qualify returns 210.
  * b2_last_sweep_kernel reports "sa_tma<R>" or "sa_generic", with "+adj" on adjoint calls. */
@@ -313,7 +313,7 @@ int b2_sa_forward(const struct b2_sa_args *a);
  *   p[t-1] = damp solve(m p.dt2 - L((1+tt) rho p) - L(rho r[t-1]) + (1-damp) p.dt.T, p[t-1])
  * `src` (the receiver data) is injected into p[t-1] with the same scale and `rec` (the adjoint source) samples p[t].
  * p (`u`) and r have the same layout. Not combined with halo exchange or a free surface (210). kernel 0 runs the
- * 2.5-D TMA sweep k_visco_tma<R> when the layout qualifies (3-D, radius 2 or 4, z extent and z start multiples of 4,
+ * 2.5-D TMA sweep visco_tma<R> when the layout qualifies (3-D, radius 2 or 4, z extent and z start multiples of 4,
  * 16-byte aligned arrays), else the one-thread-per-point kernel; kernel 2 on a layout that does not qualify returns
  * 210. b2_last_sweep_kernel reports "visco_tma<R>" or "visco_generic", with "+adj" on adjoint calls. */
 struct b2_visco_args {

@@ -3,7 +3,7 @@
 
 At so=8 on 1024^3 (944^3 + 40 absorbing cells per side) with array b, vp and w/Q, it calls `b2_sa_forward` on
 device-resident arrays (u, b, vp, w/Q: 4.3 GB per level or field), forward and adjoint, with the TMA sweep
-(`k_sa_tma<4>`, kernel=0) and the one-thread-per-point kernel (`k_sa_generic`, kernel=1) alternated in the same run,
+(`sa_tma<4>`, kernel=0) and the one-thread-per-point kernel (`k_sa_generic`, kernel=1) alternated in the same run,
 STEPS steps each after a warm-up call. It prints one JSON line with, per kernel and direction:
 - the per-step time of each direction (host clock around the blocking call / the number of steps);
 - the mean device time per sweep launch (CUDA events around every launch, `b2_kernel_timing_ms`) and the variant that

@@ -3,7 +3,7 @@
 
 At so=8 on 1024^3 (absorbing layers included) with array vp, b, qp and the mask damping, it calls `b2_visco_forward`
 on device-resident arrays (p, r: three levels each; vp, b, qp, damp: 4.5 GB per level or field), forward and
-adjoint, with the TMA sweep (`k_visco_tma<4>`, kernel=0) and the one-thread-per-point kernel (`k_visco_generic`,
+adjoint, with the TMA sweep (`visco_tma<4>`, kernel=0) and the one-thread-per-point kernel (`k_visco_generic`,
 kernel=1) alternated in the same run, STEPS steps each after a warm-up call. The library adds five tables and, on
 the adjoint, s: 72 GB in all with the arrays above, within the 80 GB of an H100. It prints one JSON line with, per
 kernel and direction:

@@ -63,7 +63,7 @@ TILES = {
     # b2_tti.cu TtiTile<R>::TY, kTtiWsTY, TtiArrTile<R>::TY; TZ: TtiCfg / TtiWsCfg
     'tti_fused<2>': (32, 64), 'tti_fused<4>': (28, 64), 'tti_ws<pf1>': (24, 64),
     'tti_arr_ct2<2>': (30, 64), 'tti_arr_ct2<4>': (20, 64),
-    # b2_sa.cu SaTmaCfg<R>
+    # b2_nested.cuh NestedCfg<R> (the SA sweep k_nested_tma<R, SaEpi>)
     'sa_tma<2>': (16, 64), 'sa_tma<4>': (16, 64),
 }
 TTI_SA_TILES = {name: t for name, t in TILES.items() if name.startswith(('tti_', 'sa_'))}

@@ -114,7 +114,7 @@ def _check(key, sweep, box, **kw):
 
 
 CASES = [
-    # (so, arrays, adjoint, nd, kernel=): kernel 0 picks k_sa_tma<R> on these 3-D so=4 / so=8 layouts (z extent and z
+    # (so, arrays, adjoint, nd, kernel=): kernel 0 picks sa_tma<R> on these 3-D so=4 / so=8 layouts (z extent and z
     # start multiples of 4), k_sa_generic otherwise; the (37, 45, 68) grid cuts into 3 x 2 yz-tiles of 16 x 64, the
     # last of each partial, and the interior box shifts and shortens them
     (4, True, False, 3, 0), (8, True, False, 3, 0), (4, True, True, 3, 0), (8, True, True, 3, 0),

@@ -48,7 +48,7 @@ def _struct(src, head):
 
 def kernel_tiles():
     """(TY, TZ) per sweep name, as the CUDA sources define them"""
-    iso, tti, sa = _source('b2_iso.cu'), _source('b2_tti.cu'), _source('b2_sa.cu')
+    iso, tti, nested = _source('b2_iso.cu'), _source('b2_tti.cu'), _source('b2_nested.cuh')
     out = {}
     for r in (2, 4, 6, 8):
         for param in ('scalar', 'vp', 'm'):
@@ -66,12 +66,13 @@ def kernel_tiles():
         (ty,) = _ints(_struct(tti, rf'struct TtiArrTile<{r}>'), 'TY')
         out[f'tti_arr_ct2<{r}>'] = (ty, tz)
     out['tti_ws<pf1>'] = (int(re.search(r'constexpr int kTtiWsTY = (\d+);', tti).group(1)), tz_ws)
-    ty, tz = _ints(_struct(sa, r'template <int R> struct SaTmaCfg'), 'TY', 'TZ')
+    ty, tz = _ints(_struct(nested, r'template <int R> struct NestedCfg'), 'TY', 'TZ')
     out['sa_tma<2>'] = out['sa_tma<4>'] = (ty, tz)
     return out
 
 
-def test_tiles_match_the_kernels():
+def test_tiles_match_the_kernel_sources():
+    """the iso and TTI tiles of their sweep files, and the SA tile of the nested-operator sweep (b2_nested.cuh)"""
     assert kernel_tiles() == KC.TILES
 
 
