@@ -431,7 +431,10 @@ class Operator:
                 except _Unrecognised as sa_why:
                     raise _Unrecognised(f"{iso_why}; as the self-adjoint update: {sa_why}") from None
             if incs:
-                self._attach_imaging(plan, incs[0])
+                if plan['grid'].dim != 3:
+                    raise _Unrecognised("imaging condition is 3-D only")
+                plan['grad'] = incs[0].lhs.function
+                (plan['usave'],) = self._imaging(plan, incs[0], [plan['u']], 7)
             plan['free_surface'] = bool(fss)
             if fss and plan.get('ot4'):
                 raise _Unrecognised("a free surface under the OT4 kernel is not on the fast path yet")
@@ -454,7 +457,11 @@ class Operator:
                 raise _Unrecognised("the TTI imaging condition needs the backward (adjoint) pair")
             plan = self._recognise_tti_adjoint(updates, injs, itps)
             if incs:
-                self._attach_tti_imaging(plan, incs[0])
+                saved = self._imaging(plan, incs[0], [plan['u'], plan['v']], 17)
+                if any(s.grid is not plan['grid'] for s in saved):
+                    raise _Unrecognised("the forward wavefields must be saved (save=nt) and read at (time, x, y, z)")
+                plan['grad'] = incs[0].lhs.function
+                plan['usave'], plan['vsave'] = saved
             return plan
         if len(updates) == 2:
             try:
@@ -536,6 +543,18 @@ class Operator:
             raise _Unrecognised("update has a source term that is not a sparse injection")
         return terms
 
+    def _taps(self, rhs, fields, tags=None):
+        """{tap: coefficient} of an update linear in `fields`. A tap is the access's (time_shift, offsets), led by
+        the entry of `tags` that belongs to the field read when `tags` (one per field) is given."""
+        tag = {id(f): t for f, t in zip(fields, tags or ())}
+        out = {}
+        for acc, coef in self._coeffs(rhs, fields).items():
+            k = _space_offsets(acc, None)
+            if k is None:
+                raise _Unrecognised("non-affine wavefield access")
+            out[(tag[id(acc.function)],) + k if tags else k] = coef
+        return out
+
     @staticmethod
     def _leaves(exprs):
         """Non-wavefield leaves of the coefficient expressions."""
@@ -587,14 +606,8 @@ class Operator:
         if so % 2 or so < 2 or so // 2 > 8:
             raise _Unrecognised(f"space_order {so} unsupported")
         R = so // 2
-        terms = self._coeffs(eq.rhs, [u])
         # the stencil support must be exactly the (2R*nd + 1)-point star at t plus the centre at t-1
-        keyed = {}
-        for acc, coef in terms.items():
-            k = _space_offsets(acc, None)
-            if k is None:
-                raise _Unrecognised("non-affine wavefield access")
-            keyed[k] = coef
+        keyed = self._taps(eq.rhs, [u])
         zero = (0,) * nd
         star = {(0, zero)}
         for d in range(nd):
@@ -673,33 +686,54 @@ class Operator:
         if nd not in (2, 3):
             raise _Unrecognised("only 2-D/3-D grids")
         so = u.space_order
-        terms = self._coeffs(eq.rhs, [u])
-        keyed = {}
-        for acc, coef in terms.items():
-            k = _space_offsets(acc, None)
-            if k is None:
-                raise _Unrecognised("non-affine wavefield access")
-            keyed[k] = coef
+        keyed = self._taps(eq.rhs, [u])
         dirn = self._dirn
         zero = (0,) * nd
-        reach = max((max(abs(o) for o in k[1]) for k in keyed), default=0)
-        if reach % 2 == 0:
-            raise _Unrecognised("support is not that of nested half-node first derivatives")
-        R = (reach + 1) // 2
-        if 2 * R > so or R > 8:
-            raise _Unrecognised(f"radius {2 * R - 1} does not fit the halo of space_order {so}")
+        R, leaves, c, fcands, cands, probes = self._nested_front(
+            [k[1] for k in keyed], keyed.values(), grid, so, 2468)
         star = {(0, zero), (-dirn, zero)}
         for d in range(nd):
-            for s in range(-reach, reach + 1):
+            for s in range(1 - 2 * R, 2 * R):
                 o = [0] * nd
                 o[d] = s
                 star.add((0, tuple(o)))
         if set(keyed) != star:
             raise _Unrecognised("stencil support is not the star of radius 2R-1 plus the centre of the other level")
-        funcs, consts, syms = self._leaves(keyed.values())
+
+        def match(roles, w_role):
+            b, vp = (x[1] for x in roles)
+            for value, leaf, dt in probes:
+                pred = predict_sa(c, R, nd, lambda off: value(b, off), value(vp, zero),
+                                  value(w_role[1], zero) if w_role else 0.0, dt, dirn)
+                if not self._nested_matches([(keyed, pred)], leaf):
+                    return None
+            return roles + (w_role,)
+        found = self._find_roles(cands, fcands, 2, match)
+        if found is None:
+            raise _Unrecognised("coefficients are not those of the self-adjoint update for any roles of "
+                                "b, vp and w/Q")
+        b_role, vp_role, w_role = found
+        plan = {'kind': 'sa', 'u': u, 'grid': grid, 'so': so, 'R': R, 'c': c,
+                'b_role': b_role, 'vp_role': vp_role, 'damp': w_role[1] if w_role else None,
+                'dt': grid.stepping_dim.spacing, 'src': None, 'rec': None, 'rec_toff': 0, 'adjoint': dirn == -1}
+        self._attach_sa_sparse(plan, injs, itps, *leaves)
+        return plan
+
+    def _nested_front(self, offsets, exprs, grid, so, seed):
+        """What recognising the self-adjoint update and the SLS pair shares, both applying the nested operator L:
+        L's radius R from the reach of the wavefield's tap `offsets`; the leaves of the coefficient expressions
+        `exprs`, which read no other wavefield, dt and no unknown symbol; L's weights c; the candidates for the
+        parameter roles (the Functions, then all); and three probes drawn from `seed`."""
+        reach = max((max(abs(o) for o in off) for off in offsets), default=0)
+        if reach % 2 == 0:
+            raise _Unrecognised("support is not that of nested half-node first derivatives")
+        R = (reach + 1) // 2
+        if 2 * R > so or R > 8:
+            raise _Unrecognised(f"radius {2 * R - 1} does not fit the halo of space_order {so}")
+        funcs, consts, syms = self._leaves(exprs)
         for a in funcs:
             if getattr(a.function, 'is_TimeFunction', False):
-                raise _Unrecognised("a second wavefield in the coefficients")
+                raise _Unrecognised("another wavefield in the coefficients")
         dtsym = grid.stepping_dim.spacing
         if dtsym.name not in {s.name for s in syms}:
             raise _Unrecognised("no time spacing in the update")
@@ -707,39 +741,37 @@ class Operator:
         for sym in syms:
             if sym.name not in known:
                 raise _Unrecognised(f"unknown symbol {sym.name} in the update")
-        hs = self._spacing_values(grid)
-        c = [sa_weights(R, h) for h in hs]
+        c = [sa_weights(R, h) for h in self._spacing_values(grid)]
         fcands = [('f', a.function) for a in funcs]
-        ccands = [('c', cst) for cst in consts]
-        cands = fcands + ccands
-        rng = np.random.default_rng(2468)
+        cands = fcands + [('c', cst) for cst in consts]
+        rng = np.random.default_rng(seed)
         probes = [self._sa_probe(rng, cands, grid) for _ in range(3)]
-        found = None
-        for b_role in cands:
-            for vp_role in cands:
-                if vp_role is b_role:
-                    continue
-                for w_role in [r for r in fcands if r is not b_role and r is not vp_role] + [None]:
-                    used = {id(r[1]) for r in (b_role, vp_role, w_role) if r is not None}
-                    if used != {id(r[1]) for r in cands}:
-                        continue
-                    if all(self._sa_matches(keyed, pr, b_role, vp_role, w_role, c, R, nd, dirn, dtsym)
-                           for pr in probes):
-                        found = (b_role, vp_role, w_role)
-                        break
-                if found:
-                    break
-            if found:
-                break
-        if found is None:
-            raise _Unrecognised("coefficients are not those of the self-adjoint update for any roles of "
-                                "b, vp and w/Q")
-        b_role, vp_role, w_role = found
-        plan = {'kind': 'sa', 'u': u, 'grid': grid, 'so': so, 'R': R, 'c': c,
-                'b_role': b_role, 'vp_role': vp_role, 'damp': w_role[1] if w_role else None,
-                'dt': dtsym, 'src': None, 'rec': None, 'rec_toff': 0, 'adjoint': dirn == -1}
-        self._attach_sa_sparse(plan, injs, itps, funcs, consts, syms)
-        return plan
+        return R, (funcs, consts, syms), c, fcands, cands, probes
+
+    @staticmethod
+    def _find_roles(cands, fcands, n, match):
+        """The first result of `match(roles, damping role)` that is not None: `roles` are n distinct candidates in
+        the order of `itertools.permutations`, the damping role is a Function of `fcands` outside them or None, and
+        every candidate has a role."""
+        every = {id(x[1]) for x in cands}
+        for roles in itertools.permutations(cands, n):
+            for d_role in [x for x in fcands if all(x is not y for y in roles)] + [None]:
+                if {id(x[1]) for x in roles + (d_role,) if x is not None} == every:
+                    found = match(roles, d_role)
+                    if found is not None:
+                        return found
+        return None
+
+    @staticmethod
+    def _nested_matches(pairs, leaf):
+        """Whether, for each (keyed coefficient expressions, predicted coefficients) of `pairs`, the taps are the
+        predicted ones and each coefficient evaluated at `leaf` is within 1e-9 times the largest predicted one."""
+        for keyed, pred in pairs:
+            got = {k: eval_scalar(v, leaf) for k, v in keyed.items()}
+            scale = max(abs(v) for v in pred.values())
+            if set(got) != set(pred) or not all(abs(got[k] - pred[k]) <= 1e-9 * scale for k in pred):
+                return False
+        return True
 
     def _sa_probe(self, rng, cands, grid):
         """Probe values: a Function is base + grad . offset (linear in space), a Constant one number."""
@@ -763,42 +795,20 @@ class Operator:
                 return value(n.function, k[1] if k is not None else (0,) * grid.dim)
             if n.is_Constant:
                 return value(n, (0,) * grid.dim)
-            return spc[n.name]           # _recognise_sa refused every other symbol
+            return spc[n.name]           # _nested_front refused every other symbol
         return value, leaf, dt
-
-    def _sa_matches(self, keyed, probe, b_role, vp_role, w_role, c, R, nd, dirn, dtsym):
-        value, leaf, dt = probe
-        got = {k: eval_scalar(v, leaf) for k, v in keyed.items()}
-        pred = predict_sa(c, R, nd, lambda off: value(b_role[1], off), value(vp_role[1], (0,) * nd),
-                          value(w_role[1], (0,) * nd) if w_role else 0.0, dt, dirn)
-        scale = max(abs(v) for v in pred.values())
-        return set(got) == set(pred) and all(abs(got[k] - pred[k]) <= 1e-9 * scale for k in pred)
 
     def _attach_sa_sparse(self, plan, injs, itps, funcs, consts, syms, scale=None, what="src*dt^2*vp^2/b"):
         """Injection `src * dt^2 * vp^2 / b` into the level written (operators.py:101, :149), checked at random
         values; receivers / the adjoint source as for the acoustic update."""
         grid, dtsym = plan['grid'], plan['dt']
         if injs:
-            inj = injs[0]
-            sf = inj.sfunction
-            if not isinstance(sf, SparseTimeFunction) or sf.interpolation not in ('linear', 'sinc'):
-                raise _Unrecognised("unsupported sparse function for injection")
-            self._check_radius(sf, [plan['u']])
-            if [id(a.function) for a in inj.fields] != [id(plan['u'])]:
-                raise _Unrecognised("injection target differs from the updated field")
-            a, ex = inj.fields[0], inj.exprs[0]
-            k = _space_offsets(a, None)
-            if k is None or k[0] != self._dirn or any(k[1]):
-                raise _Unrecognised("injection must target the updated time level")
-            ex = ex.evaluate.subs(self._subs) if self._subs else ex.evaluate
-            f2, c2, s2 = self._leaves([ex])
+            sf, ((ex, (f2, c2, s2)),) = self._injection(injs[0], [plan['u']])
             if dtsym.name not in {s.name for s in s2}:
                 raise _Unrecognised("injected expression has no time spacing")
             for sym in s2:
                 if sym.name != dtsym.name and sym.name not in {sp.name for sp in grid.spacing_map}:
                     raise _Unrecognised(f"unknown symbol {sym.name} in the injected expression")
-            if not any(acc.function is sf for acc in f2):
-                raise _Unrecognised("injected expression does not contain the source")
             rng = np.random.default_rng(8642)
             roles = [plan['b_role'], plan['vp_role']]
             known = {id(o) for _, o in roles} | {id(sf)}
@@ -844,59 +854,29 @@ class Operator:
         so = p.space_order
         if r.space_order != so or r.grid is not grid or r.time_size != p.time_size:
             raise _Unrecognised("p and r differ in space order, grid or time slots")
-        keyed = []
-        for e in (e1, e2):
-            k_ = {}
-            for acc, coef in self._coeffs(e.rhs, [p, r]).items():
-                k = _space_offsets(acc, None)
-                if k is None:
-                    raise _Unrecognised("non-affine wavefield access")
-                k_[('p' if acc.function is p else 'r',) + k] = coef
-            keyed.append(k_)
-        reach = max((max(abs(o) for o in k[2]) for k in keyed[1] if k[0] == 'p'), default=0)
-        if reach % 2 == 0:
-            raise _Unrecognised("support is not that of nested half-node first derivatives")
-        R = (reach + 1) // 2
-        if 2 * R > so or R > 8:
-            raise _Unrecognised(f"radius {2 * R - 1} does not fit the halo of space_order {so}")
-        funcs, consts, syms = self._leaves(list(keyed[0].values()) + list(keyed[1].values()))
-        for a in funcs:
-            if getattr(a.function, 'is_TimeFunction', False):
-                raise _Unrecognised("a third wavefield in the coefficients")
-        dtsym = grid.stepping_dim.spacing
-        if dtsym.name not in {s.name for s in syms}:
-            raise _Unrecognised("no time spacing in the update")
-        known = {dtsym.name} | {sp.name for sp in grid.spacing_map}
-        for sym in syms:
-            if sym.name not in known:
-                raise _Unrecognised(f"unknown symbol {sym.name} in the update")
-        c = [sa_weights(R, h) for h in self._spacing_values(grid)]
-        fcands = [('f', a.function) for a in funcs]
-        cands = fcands + [('c', cst) for cst in consts]
-        rng = np.random.default_rng(1357)
-        probes = [self._sa_probe(rng, cands, grid) for _ in range(3)]
-        found = None
-        for roles in itertools.permutations(cands, 3):
-            for d_role in [x for x in fcands if all(x is not y for y in roles)] + [None]:
-                used = {id(x[1]) for x in roles + (d_role,) if x is not None}
-                if used != {id(x[1]) for x in cands}:
-                    continue
-                f0 = self._visco_f0(keyed, probes[0], roles, d_role, nd, dirn)
-                if f0 is not None and all(self._visco_matches(keyed, pr, roles, d_role, f0, c, R, nd, dirn)
-                                          for pr in probes):
-                    found = roles + (d_role, f0)
-                    break
-            if found:
-                break
+        keyed = [self._taps(e.rhs, [p, r], ('p', 'r')) for e in (e1, e2)]
+        R, leaves, c, fcands, cands, probes = self._nested_front(
+            [k[2] for k in keyed[1] if k[0] == 'p'], list(keyed[0].values()) + list(keyed[1].values()), grid, so, 1357)
+        at = lambda value, role: (lambda off: value(role[1], off)) if role else (lambda off: 1.0)
+
+        def match(roles, d_role):
+            f0 = self._visco_f0(keyed, probes[0], roles, d_role, nd, dirn)
+            if f0 is None:
+                return None
+            for value, leaf, dt in probes:
+                pred = predict_visco(c, R, nd, *(at(value, x) for x in roles), at(value, d_role), f0, dt, dirn)
+                if not self._nested_matches(zip(keyed, pred), leaf):
+                    return None
+            return roles + (d_role, f0)
+        found = self._find_roles(cands, fcands, 3, match)
         if found is None:
             raise _Unrecognised("coefficients are not those of the SLS update for any roles of b, vp, qp and damp")
         b_role, vp_role, qp_role, d_role, f0 = found
         plan = {'kind': 'visco', 'u': p, 'r': r, 'grid': grid, 'so': so, 'R': R, 'c': c, 'b_role': b_role,
                 'vp_role': vp_role, 'qp_role': qp_role, 'damp': d_role[1] if d_role else None,
-                'f0': float(np.float32(f0)), 'dt': dtsym, 'src': None, 'rec': None, 'rec_toff': 0,
-                'adjoint': dirn == -1}
-        self._attach_sa_sparse(plan, injs, itps, funcs, consts, syms, scale=lambda vp, b: vp * vp,
-                               what="src*dt^2/m")
+                'f0': float(np.float32(f0)), 'dt': grid.stepping_dim.spacing, 'src': None, 'rec': None,
+                'rec_toff': 0, 'adjoint': dirn == -1}
+        self._attach_sa_sparse(plan, injs, itps, *leaves, scale=lambda vp, b: vp * vp, what="src*dt^2/m")
         return plan
 
     @staticmethod
@@ -915,20 +895,6 @@ class Operator:
         t_s = dt / den
         f0 = (np.sqrt(1.0 + 1.0 / qp ** 2) - 1.0 / qp) / t_s
         return f0 if np.isfinite(f0) and f0 > 0 else None
-
-    def _visco_matches(self, keyed, probe, roles, d_role, f0, c, R, nd, dirn):
-        value, leaf, dt = probe
-        b_role, vp_role, qp_role = roles
-        zero = (0,) * nd
-        pred = predict_visco(c, R, nd, lambda off: value(b_role[1], off), lambda off: value(vp_role[1], off),
-                             lambda off: value(qp_role[1], off),
-                             (lambda off: value(d_role[1], off)) if d_role else (lambda off: 1.0), f0, dt, dirn)
-        for got_k, want in zip(keyed, pred):
-            got = {k: eval_scalar(v, leaf) for k, v in got_k.items()}
-            scale = max(abs(v) for v in want.values())
-            if set(got) != set(want) or any(abs(got[k] - want[k]) > 1e-9 * scale for k in want):
-                return False
-        return True
 
     def _recognise_ot4(self, u, keyed, star, R):
         """The reference's 4th-order-in-time acoustic update (examples/seismic/acoustic/operators.py:
@@ -1084,27 +1050,35 @@ class Operator:
         if so < sf.r:
             raise ValueError(f"Space order {so} too small for interpolation r {sf.r}")
 
+    def _injection(self, inj, fields):
+        """The checks every injection passes, whatever value it injects: a SparseTimeFunction with linear or sinc
+        interpolation that fits the halo, injected once into each of `fields` at the level written, each expression
+        containing the source. Returns the source and, per target, the evaluated expression and its leaves."""
+        sf = inj.sfunction
+        if not isinstance(sf, SparseTimeFunction) or sf.interpolation not in ('linear', 'sinc'):
+            raise _Unrecognised("unsupported sparse function for injection")
+        self._check_radius(sf, fields)
+        if sorted(id(a.function) for a in inj.fields) != sorted(id(f) for f in fields):
+            raise _Unrecognised("injection targets differ from the updated fields")
+        targets = []
+        for a, ex in zip(inj.fields, inj.exprs):
+            k = _space_offsets(a, None)
+            if k is None or k[0] != self._dirn or any(k[1]):
+                raise _Unrecognised("injection must target the updated time level")
+            ex = ex.evaluate.subs(self._subs) if self._subs else ex.evaluate
+            leaves = self._leaves([ex])
+            if not any(acc.function is sf for acc in leaves[0]):
+                raise _Unrecognised("injected expression does not contain the source")
+            targets.append((ex, leaves))
+        return sf, targets
+
     def _attach_sparse(self, plan, injs, itps, fields, funcs, consts, syms, m_role):
         grid = plan['grid']
         dtsym = plan['dt']
         rng = np.random.default_rng(4321)
         if injs:
-            inj = injs[0]
-            sf = inj.sfunction
-            if not isinstance(sf, SparseTimeFunction) or sf.interpolation not in ('linear', 'sinc'):
-                raise _Unrecognised("unsupported sparse function for injection")
-            self._check_radius(sf, fields)
-            tgt = {id(f) for f in fields}
-            if {id(a.function) for a in inj.fields} != tgt:
-                raise _Unrecognised("injection targets differ from the updated fields")
-            for a, ex in zip(inj.fields, inj.exprs):
-                k = _space_offsets(a, None)
-                if k is None or k[0] != self._dirn or any(k[1]):
-                    raise _Unrecognised("injection must target the updated time level")
-                ex = ex.evaluate.subs(self._subs) if self._subs else ex.evaluate
-                f2, c2, s2 = self._leaves([ex])
-                if not any(acc.function is sf for acc in f2):
-                    raise _Unrecognised("injected expression does not contain the source")
+            sf, targets = self._injection(injs[0], fields)
+            for ex, (f2, c2, s2) in targets:
                 literal = dtsym.name not in {s.name for s in s2}
                 lits = []
                 for probe in range(2):
@@ -1177,16 +1151,10 @@ class Operator:
         if plan.get('ot4') or plan.get('adjoint'):
             raise _Unrecognised("Born is on the fast path for the forward OT2 update only")
         grid = plan['grid']
-        terms = self._coeffs(eqU.rhs, [u, U])
-        ku = {}
-        for acc, coef in self._coeffs(equ.rhs, [u]).items():
-            ku[_space_offsets(acc, None)] = coef
-        kU, kq = {}, {}
-        for acc, coef in terms.items():
-            k = _space_offsets(acc, None)
-            if k is None:
-                raise _Unrecognised("non-affine wavefield access")
-            (kU if acc.function is U else kq)[k] = coef
+        tU = self._taps(eqU.rhs, [u, U], ('u', 'U'))
+        ku = self._taps(equ.rhs, [u])
+        kU = {k[1:]: coef for k, coef in tU.items() if k[0] == 'U'}
+        kq = {k[1:]: coef for k, coef in tU.items() if k[0] == 'u'}
         zero = (0, 0, 0)
         if set(kU) != set(ku) or set(kq) != {(1, zero), (0, zero), (-1, zero)}:
             raise _Unrecognised("second update is not the background stencil plus a centred u.dt2 term")
@@ -1225,69 +1193,13 @@ class Operator:
         plan['born_dm'] = dm
         return plan
 
-    def _attach_imaging(self, plan, inc):
-        """`Inc(grad, -u * v.dt2)` next to the adjoint update = the reference's Gradient operator
-        (examples/seismic/acoustic/operators.py:190-232)."""
-        v = plan['u']
+    def _imaging(self, plan, inc, fields, seed):
+        """`Inc(g, -sum_i s_i * f_i.dt2)` next to the adjoint update of `fields`, each s_i a forward wavefield saved
+        (save=nt) and read at (time, x, y, z): the reference's Gradient operator (examples/seismic/acoustic/
+        operators.py:190-232) for one field, its `GradientTTI` (tti/operators.py `JacobianAdjOperator`) for the TTI
+        pair. The coefficients are checked at values drawn from `seed`. Returns the s_i, in the order of `fields`."""
         grid = plan['grid']
-        lhs = inc.lhs
-        if not (lhs.is_Access and isinstance(lhs.function, Function) and not lhs.function.is_TimeFunction):
-            raise _Unrecognised("increment target is not a Function")
-        if grid.dim != 3 or lhs.function.grid is not grid:
-            raise _Unrecognised("imaging condition is 3-D only")
-        k = _space_offsets(lhs, None)
-        if k is None or any(k[1]):
-            raise _Unrecognised("increment target accessed off-centre")
-        rhs = inc.rhs.evaluate
-        if self._subs:
-            rhs = rhs.subs(self._subs)
-        try:
-            terms, rest = linear_terms(rhs, lambda a: a.function is v)
-        except NonLinear as e:
-            raise _Unrecognised(f"increment is not linear in the adjoint wavefield: {e}") from None
-        if not (rest.is_Number and float(rest.value) == 0.0):
-            raise _Unrecognised("increment has terms without the adjoint wavefield")
-        keyed = {}
-        for acc, coef in terms.items():
-            kk = _space_offsets(acc, None)
-            if kk is None or any(kk[1]):
-                raise _Unrecognised("increment reads the adjoint wavefield off-centre")
-            keyed[kk[0]] = coef
-        if set(keyed) != {-1, 0, 1}:
-            raise _Unrecognised("increment is not u * v.dt2")
-        funcs, consts, syms = self._leaves(keyed.values())
-        saved = [a for a in funcs if getattr(a.function, 'is_TimeFunction', False)]
-        if len(saved) != 1 or len(funcs) != 1 or consts:
-            raise _Unrecognised("increment must multiply v.dt2 by one saved wavefield")
-        us = saved[0]
-        ku = _space_offsets(us, None)
-        if us.function.is_buffered or ku is None or ku[0] != 0 or any(ku[1]) or \
-                us.function.space_order != v.space_order:
-            raise _Unrecognised("the forward wavefield must be saved (save=nt) and read at (time, x, y, z)")
-        rng = np.random.default_rng(7)
-        dtname = plan['dt'].name
-        for probe in range(2):
-            uval, dt = rng.uniform(0.5, 2.0), rng.uniform(0.5, 2.0)
-
-            def leaf(n):
-                if n.is_Access:
-                    return uval
-                if n.name == dtname:
-                    return dt
-                raise _Unrecognised(f"unknown symbol {n.name} in the increment")
-            c = {t: eval_scalar(e, leaf) for t, e in keyed.items()}
-            want = {-1: -uval / dt ** 2, 0: 2 * uval / dt ** 2, 1: -uval / dt ** 2}
-            for t in want:
-                if abs(c[t] - want[t]) > 1e-9 * abs(want[t]):
-                    raise _Unrecognised("increment is not -u * v.dt2")
-        plan['grad'] = lhs.function
-        plan['usave'] = us.function
-
-    def _attach_tti_imaging(self, plan, inc):
-        """`Inc(dm, -(u0 * p.dt2 + v0 * r.dt2))` next to the adjoint TTI pair = the reference's `GradientTTI`
-        (tti/operators.py `JacobianAdjOperator`): u0, v0 saved forward wavefields read at (time, x, y, z)."""
-        p, r = plan['u'], plan['v']
-        grid = plan['grid']
+        form = ' + '.join(f'saved * {f.name}.dt2' for f in fields)
         lhs = inc.lhs
         if not (lhs.is_Access and isinstance(lhs.function, Function) and not lhs.function.is_TimeFunction):
             raise _Unrecognised("increment target is not a Function")
@@ -1299,38 +1211,40 @@ class Operator:
         rhs = inc.rhs.evaluate
         if self._subs:
             rhs = rhs.subs(self._subs)
+        ids = {id(f) for f in fields}
         try:
-            terms, rest = linear_terms(rhs, lambda a: a.function is p or a.function is r)
+            terms, rest = linear_terms(rhs, lambda a: id(a.function) in ids)
         except NonLinear as e:
             raise _Unrecognised(f"increment is not linear in the adjoint wavefields: {e}") from None
         if not (rest.is_Number and float(rest.value) == 0.0):
             raise _Unrecognised("increment has terms without the adjoint wavefields")
-        keyed = {id(p): {}, id(r): {}}
+        keyed = {id(f): {} for f in fields}
         for acc, coef in terms.items():
             kk = _space_offsets(acc, None)
             if kk is None or any(kk[1]):
                 raise _Unrecognised("increment reads an adjoint wavefield off-centre")
             keyed[id(acc.function)][kk[0]] = coef
         saved = []
-        for f in (p, r):
+        for f in fields:
             if set(keyed[id(f)]) != {-1, 0, 1}:
-                raise _Unrecognised("increment is not u0 * p.dt2 + v0 * r.dt2 (both fields, second derivative)")
+                raise _Unrecognised(f"increment is not -({form})")
             funcs, consts, _ = self._leaves(keyed[id(f)].values())
             sv = [a for a in funcs if getattr(a.function, 'is_TimeFunction', False)]
             if len(sv) != 1 or len(funcs) != 1 or consts:
-                raise _Unrecognised("each term of the increment must multiply f.dt2 by one saved wavefield")
+                raise _Unrecognised(f"each term of the increment must multiply {f.name}.dt2 by one saved wavefield")
             us = sv[0]
             ku = _space_offsets(us, None)
             if us.function.is_buffered or ku is None or ku[0] != 0 or any(ku[1]) or \
-                    us.function.space_order != p.space_order or us.function.grid is not grid:
-                raise _Unrecognised("the forward wavefields must be saved (save=nt) and read at (time, x, y, z)")
+                    us.function.space_order != plan['u'].space_order:
+                raise _Unrecognised("the forward wavefield must be saved (save=nt) and read at (time, x, y, z)")
             saved.append(us.function)
-        if saved[0] is saved[1]:
-            raise _Unrecognised("the two terms of the increment must use the two saved wavefields")
-        rng = np.random.default_rng(17)
+        if len({id(s) for s in saved}) != len(saved):
+            raise _Unrecognised("the terms of the increment must use distinct saved wavefields")
+        rng = np.random.default_rng(seed)
         dtname = plan['dt'].name
         for probe in range(2):
-            val = {id(saved[0]): rng.uniform(0.5, 2.0), id(saved[1]): rng.uniform(2.5, 4.0)}
+            # saved field i is drawn in [0.5 + 2i, 2 + 2i], so a term that multiplies the wrong field cannot match
+            val = {id(s): rng.uniform(0.5 + 2 * i, 2.0 + 2 * i) for i, s in enumerate(saved)}
             dt = rng.uniform(0.5, 2.0)
 
             def leaf(n):
@@ -1339,17 +1253,18 @@ class Operator:
                 if n.name == dtname:
                     return dt
                 raise _Unrecognised(f"unknown symbol {n.name} in the increment")
-            for f, sfn in ((p, saved[0]), (r, saved[1])):
+            for f, s in zip(fields, saved):
                 c = {t: eval_scalar(e, leaf) for t, e in keyed[id(f)].items()}
-                s_ = val[id(sfn)]
+                s_ = val[id(s)]
                 want = {-1: -s_ / dt ** 2, 0: 2 * s_ / dt ** 2, 1: -s_ / dt ** 2}
                 for t in want:
                     if abs(c[t] - want[t]) > 1e-9 * abs(want[t]):
-                        raise _Unrecognised("increment is not -(u0 * p.dt2 + v0 * r.dt2)")
-        plan['grad'] = lhs.function
-        plan['usave'], plan['vsave'] = saved
+                        raise _Unrecognised(f"increment is not -({form})")
+        return saved
 
     # -- TTI -------------------------------------------------------------------------------------
+    _TTI_PARAMS = ('vp', 'epsilon', 'delta', 'theta', 'phi')
+
     def _recognise_tti_adjoint(self, updates, injs, itps):
         """The reference's centred-TTI adjoint `AdjointTTI` (tti/operators.py `AdjointOperator`, `kernel_centered(...,
         forward=False)`): (p.backward, r.backward) from H0 = Gh(e2 p + sd r), Hz = Gzz(sd p + r), e2 and sd sampled at
@@ -1366,20 +1281,9 @@ class Operator:
         if so != v.space_order or so % 4 or so // 2 > 8:
             raise _Unrecognised(f"TTI needs space_order multiple of 4 (got {so})")
         R = so // 2
-        tu = self._coeffs(equ.rhs, [u, v])
-        tv = self._coeffs(eqv.rhs, [u, v])
-
-        def keyed(terms):
-            out = {}
-            for acc, coef in terms.items():
-                k = _space_offsets(acc, None)
-                if k is None:
-                    raise _Unrecognised("non-affine wavefield access")
-                out[('u' if acc.function is u else 'v',) + k] = coef
-            return out
-        ku, kv = keyed(tu), keyed(tv)
+        ku, kv = (self._taps(e.rhs, [u, v], ('u', 'v')) for e in (equ, eqv))
         funcs, consts, syms = self._leaves(list(ku.values()) + list(kv.values()))
-        pnames = ('vp', 'epsilon', 'delta', 'theta', 'phi')
+        pnames = self._TTI_PARAMS
         byname = {c.name: c for c in consts if c.name in pnames}
         damp = None
         for a in funcs:
@@ -1413,37 +1317,7 @@ class Operator:
         w1 = [half_node_first_derivative_weights(so, h) for h in hs]
         rng = np.random.default_rng(99)
         for probe in range(2):
-            # parameters get a random value AND a random spatial gradient, so that the comparison
-            # also checks WHERE each factor is sampled (the reference samples the rotation factors
-            # at the shifted points of the outer derivative, tti/operators.py:92-102)
-            base = {n: rng.uniform(0.2, 0.8) for n in pnames}
-            gradv = {n: (rng.uniform(-0.02, 0.02, size=nd) if isinstance(byname.get(n), Function) else np.zeros(nd))
-                     for n in pnames}
-            if 'phi' not in byname:
-                base['phi'] = 0.0
-            dt = rng.uniform(0.5, 2.0)
-            dval = rng.uniform(0.5, 2.0) if damp is not None else 0.0
-            spv = {sp.name: float(v) for sp, v in grid.spacing_map.items()}
-
-            def P(name, off):
-                return float(base[name] + np.dot(gradv[name], off))
-
-            def leaf(n):
-                if n.is_Access:
-                    f = n.function
-                    if f is damp:
-                        return dval
-                    k = _space_offsets(n, None)
-                    if k is None:
-                        raise _Unrecognised("non-affine parameter access")
-                    return P(f.name, k[1])
-                if n.is_Constant:
-                    return P(n.name, (0,) * nd)
-                if n.name == dtsym.name:
-                    return dt
-                if n.name in spv:
-                    return spv[n.name]
-                raise _Unrecognised(f"unknown symbol {n.name}")
+            P, leaf, dt, dval, _ = self._tti_probe(rng, byname, damp, grid)
             pu, pv = predict_tti(w2, w1, R, P, dval, dt, adjoint=adjoint, nd=nd)
             for got, pred, nm in ((ku, pu, 'u'), (kv, pv, 'v')):
                 keys = set(got) | set(pred)
@@ -1458,6 +1332,47 @@ class Operator:
                 'm_role': m_role, 'adjoint': adjoint}
         self._attach_sparse(plan, injs, itps, [u, v], funcs, consts, syms, plan['m_role'])
         return plan
+
+    def _tti_probe(self, rng, byname, damp, grid, dm=None):
+        """Values for one probe of the TTI recognisers. Each parameter gets a random value AND, if `byname` has it
+        as a Function, a random spatial gradient, so that the comparison also checks WHERE each factor is sampled
+        (the reference samples the rotation factors at the shifted points of the outer derivative,
+        tti/operators.py:92-102). dt, then damp and (TTI Born) dm at the centre, are drawn after them.
+        Returns `P(name, offset)`, `leaf`, dt and the values of damp (0 without it) and dm."""
+        nd = grid.dim
+        base = {n: rng.uniform(0.2, 0.8) for n in self._TTI_PARAMS}
+        gradv = {n: (rng.uniform(-0.02, 0.02, size=nd) if isinstance(byname.get(n), Function) else np.zeros(nd))
+                 for n in self._TTI_PARAMS}
+        if 'phi' not in byname:
+            base['phi'] = 0.0
+        dt = rng.uniform(0.5, 2.0)
+        dval = rng.uniform(0.5, 2.0) if damp is not None else 0.0
+        dmv = rng.uniform(0.5, 2.0) if dm is not None else None
+        spv = {sp.name: float(v) for sp, v in grid.spacing_map.items()}
+        dtname = grid.stepping_dim.spacing.name
+
+        def P(name, off):
+            return float(base[name] + np.dot(gradv[name], off))
+
+        def leaf(n):
+            if n.is_Access:
+                f = n.function
+                if f is damp:
+                    return dval
+                if f is dm:
+                    return dmv
+                k = _space_offsets(n, None)
+                if k is None:
+                    raise _Unrecognised("non-affine parameter access")
+                return P(f.name, k[1])
+            if n.is_Constant:
+                return P(n.name, (0,) * nd)
+            if n.name == dtname:
+                return dt
+            if n.name in spv:
+                return spv[n.name]
+            raise _Unrecognised(f"unknown symbol {n.name}")
+        return P, leaf, dt, dval, dmv
 
     def _recognise_tti_born(self, updates, injs, itps):
         """The reference's centred-TTI linearised-modelling operator `BornTTI` (examples/seismic/tti/operators.py:
@@ -1482,34 +1397,21 @@ class Operator:
         for f, _ in lin:
             if f.grid is not grid or f.space_order != so:
                 raise _Unrecognised("TTI Born: the linearised fields need the background grid and space order")
-        ku0 = {}
-        for acc, coef in self._coeffs(bg[0][1].rhs, [u0, v0]).items():
-            ku0[(0 if acc.function is u0 else 1,) + _space_offsets(acc, None)] = coef
-        kv0 = {}
-        for acc, coef in self._coeffs(bg[1][1].rhs, [u0, v0]).items():
-            kv0[(0 if acc.function is u0 else 1,) + _space_offsets(acc, None)] = coef
-        # split each linearised equation into taps on the linearised pair and on the background pair
+        ku0, kv0 = (self._taps(e.rhs, [u0, v0], (0, 1)) for _, e in bg)
+        # split each linearised equation into taps on the linearised pair (tagged 'a', 'b') and on the background
+        # pair (0, 1)
         (fa, ea), (fb, eb) = lin
-        ta = self._coeffs(ea.rhs, [fa, fb, u0, v0])
-        tb = self._coeffs(eb.rhs, [fa, fb, u0, v0])
+        ta, tb = (self._taps(e.rhs, [fa, fb, u0, v0], ('a', 'b', 0, 1)) for e in (ea, eb))
 
-        def split(terms, du, dv):
-            own, ext = {}, {}
-            for acc, coef in terms.items():
-                k = _space_offsets(acc, None)
-                if k is None:
-                    raise _Unrecognised("non-affine wavefield access")
-                f = acc.function
-                if f is du or f is dv:
-                    own[(0 if f is du else 1,) + k] = coef
-                else:
-                    ext[(0 if f is u0 else 1,) + k] = coef
+        def split(keyed, du):
+            own = {(int(k[0] != du),) + k[1:]: coef for k, coef in keyed.items() if k[0] in ('a', 'b')}
+            ext = {k: coef for k, coef in keyed.items() if k[0] in (0, 1)}
             return own, ext
         # du is the field whose equation carries the background u0 taps; dv the v0 ones
         cand = []
-        for du, edu, dv, edv, tdu, tdv in ((fa, ea, fb, eb, ta, tb), (fb, eb, fa, ea, tb, ta)):
-            own_u, ext_u = split(tdu, du, dv)
-            own_v, ext_v = split(tdv, du, dv)
+        for du, dv, tdu, tdv, tag in ((fa, fb, ta, tb, 'a'), (fb, fa, tb, ta, 'b')):
+            own_u, ext_u = split(tdu, tag)
+            own_v, ext_v = split(tdv, tag)
             if set(own_u) == set(ku0) and set(own_v) == set(kv0):
                 cand.append((du, dv, own_u, ext_u, own_v, ext_v))
         if not cand:
@@ -1518,7 +1420,6 @@ class Operator:
         for c in cand[0][2:]:
             allc += list(c.values())
         funcs, csts, syms = self._leaves(allc)
-        pnames = ('vp', 'epsilon', 'delta', 'theta', 'phi')
         known = {id(c) for c in consts.values()}
         if damp is not None:
             known.add(id(damp))
@@ -1530,7 +1431,7 @@ class Operator:
             raise _Unrecognised("TTI Born: cannot identify the model perturbation dm (the linearised pair must use the "
                                 "background parameters)")
         dm = next(iter(extra.values()))
-        if getattr(dm, 'is_TimeFunction', False) or dm.name in pnames:
+        if getattr(dm, 'is_TimeFunction', False) or dm.name in self._TTI_PARAMS:
             raise _Unrecognised("TTI Born: cannot identify the model perturbation dm")
         for ex in allc:
             for n in ex.preorder():
@@ -1538,45 +1439,20 @@ class Operator:
                     k = _space_offsets(n, None)
                     if k is None or any(k[1]):
                         raise _Unrecognised("dm accessed off-centre")
-        dtsym = plan['dt']
-        spv = {sp.name: float(v) for sp, v in grid.spacing_map.items()}
         zero = (0,) * grid.dim
         rng = np.random.default_rng(2718)
         errors = []
         for du, dv, own_u, ext_u, own_v, ext_v in cand:
             try:
                 for probe in range(2):
-                    base = {n: rng.uniform(0.2, 0.8) for n in pnames}
-                    gradv = {n: (rng.uniform(-0.02, 0.02, size=grid.dim) if isinstance(consts.get(n), Function)
-                                 else np.zeros(grid.dim)) for n in pnames}
-                    if 'phi' not in consts:
-                        base['phi'] = 0.0
-                    dt = rng.uniform(0.5, 2.0)
-                    dval = rng.uniform(0.5, 2.0) if damp is not None else 0.0
-                    dmv = rng.uniform(0.5, 2.0)
-
-                    def leaf(n):
-                        if n.is_Access:
-                            f = n.function
-                            if f is damp:
-                                return dval
-                            if f is dm:
-                                return dmv
-                            return float(base[f.name] + np.dot(gradv[f.name], _space_offsets(n, None)[1]))
-                        if n.is_Constant:
-                            return base[n.name]
-                        if n.name == dtsym.name:
-                            return dt
-                        if n.name in spv:
-                            return spv[n.name]
-                        raise _Unrecognised(f"unknown symbol {n.name}")
+                    P, leaf, dt, dval, dmv = self._tti_probe(rng, consts, damp, grid, dm)
                     for got, want in ((own_u, ku0), (own_v, kv0)):
                         for k, c in want.items():
                             w = eval_scalar(c, leaf)
                             if abs(eval_scalar(got[k], leaf) - w) > 1e-9 * max(1.0, abs(w)):
                                 raise _Unrecognised(f"the linearised pair is not updated with the background stencil "
                                                     f"(tap {k})")
-                    vp = base['vp']
+                    vp = P('vp', zero)
                     den = 1.0 / (vp * vp) / dt ** 2 + dval / dt
                     for ext, src in ((ext_u, 0), (ext_v, 1)):
                         want = {(src, 1, zero): -dmv / dt ** 2 / den, (src, 0, zero): 2 * dmv / dt ** 2 / den,
@@ -2341,19 +2217,8 @@ def predict_sa(c, R, nd, bval, vp, w, dt, dirn):
     zero = (0,) * nd
     C = dt * dt * vp * vp / bval(zero)
     out = {(0, zero): 2.0 - dt * w, (-dirn, zero): dt * w - 1.0}
-
-    def unit(d, o):
-        e = [0] * nd
-        e[d] = o
-        return tuple(e)
-    for d in range(nd):
-        for j in range(-R, R):
-            a = c[d][j] if j >= 0 else -c[d][-j - 1]
-            bq = bval(unit(d, j))
-            for i in range(1, R + 1):
-                for m, sgn in ((j + i, 1.0), (j - i + 1, -1.0)):
-                    key = (0, unit(d, m))
-                    out[key] = out.get(key, 0.0) + C * a * bq * sgn * c[d][i - 1]
+    for off, v in nested_taps(c, R, nd, bval).items():
+        out[(0, off)] = out.get((0, off), 0.0) + C * v
     return out
 
 
