@@ -14,10 +14,15 @@
 //   __device__ void operator()(float4 acc, const float *U, int ucol, int bcol, long long off, int zcnt) const
 // acc: L at the thread's four points; U: the ring slot of their plane (f at U + ucol, b at U + bcol); off: the global
 // index of the first point; zcnt: how many of the four lie in the box (1..4; the sweep calls it only when some do).
+//
+// The host side the two updates share: the plan base NestedPlan, its set-up nested_plan_init (kernel choice, TMA
+// eligibility, b expanded into scratch, the tensor maps), and the launches launch_nested_tma and
+// launch_nested_generic. What is left to an update is its own arrays, tables, epilogue and injection scale.
 #pragma once
 #include "b2_common.cuh"
 #include "b2_ptx.cuh"
 #include <algorithm>
+#include <initializer_list>
 
 namespace b2 {
 
@@ -227,11 +232,61 @@ int nested_maps(const Box &p, const float *f, int fslots, const float *b, CUtens
     return encode_tmap(&tm_b, b, 3, dims, Cf::BZB, Cf::BYB, who);
 }
 
-// One sweep of k_nested_tma<R, Epi> over box p with the weights c (c[d][k-1] = c_k / h_d), f at slot `slot0` of tm_f.
-// The variant is noted as "<name>_tma<R>" (b2_last_sweep_kernel), with "+adj" when `adjoint`.
+// What the plans of the self-adjoint update (SaPlan) and the SLS update (ViscoPlan) share. The box: a 2-D grid is
+// (1, x, y) with radius 0 on dim 0.
+struct NestedPlan : Box {
+    int radius[3] = {0, 0, 0};
+    float c[3][B2_MAX_RADIUS] = {};          // c[d][k-1] = c_k / h_d
+    float dt = 0.f;
+    bool adjoint = false;
+    // b and vp: an array in the wavefield's space layout, or the scalar next to it
+    const float *b_arr = nullptr, *vp_arr = nullptr;
+    float b_value = 1.f, vp_value = 1.f;
+    float *b = nullptr;                      // b_arr, or library scratch that the update's table kernel fills
+    // <name>_tma<R> (3-D, R in {2, 4}, z rows and the box start 16-byte aligned): tensor maps of the haloed plane of
+    // the field f that L is applied to (every slot f has, the slot a coordinate) and of the haloed b plane
+    bool use_tma = false;
+    CUtensorMap tm_f, tm_b;
+};
+
+// The plan set-up both updates share, once p's box, radius, weights and parameters are set. Checks `kernel` (0 auto:
+// the TMA sweep when the layout qualifies, 1 generic, 2 TMA: 210 with a message when it does not), points p.b at b_arr
+// or at the scratch `bslot`, which the caller's table kernel fills with b_value, and encodes the maps of the TMA sweep
+// over f (`fslots` slots). `aligned`: the caller's arrays that the sweep accesses 16 bytes at a time (b is checked
+// here; library scratch comes from cudaMalloc and is aligned). Messages start with `who`.
+inline int nested_plan_init(NestedPlan &p, int kernel, const char *who, ScratchSlot &bslot,
+                            std::initializer_list<const void *> aligned, const float *f, int fslots) {
+    if (kernel != 0 && kernel != 1 && kernel != 2) {
+        set_error("%s: unknown kernel %d", who, kernel);
+        return B2_ERR_INVALID;
+    }
+    // the TMA sweep: 3-D, R in {2, 4} on every axis, z rows and the box start 16-byte aligned (the conditions of
+    // k_iso_tma: so % 4 == 0 and nz % 4 == 0 make the row pitch a multiple of 4 floats)
+    const int R = p.radius[2];
+    bool ok = p.radius[0] == R && p.radius[1] == R && (R == 2 || R == 4);
+    ok = ok && p.a[2] % 4 == 0 && p.o[2] % 4 == 0 && p.slot_elems % 4 == 0 && (uintptr_t)p.b_arr % 16 == 0;
+    for (const void *x : aligned) ok = ok && (uintptr_t)x % 16 == 0;
+    if (kernel == 2 && !ok) {
+        set_error("%s: TMA kernel forced but the layout does not qualify (3-D, radius 2 or 4, z extent and z start "
+                  "multiples of 4, 16-byte aligned arrays; radius=%d a2=%d o2=%d)", who, R, p.a[2], p.o[2]);
+        return B2_ERR_INVALID;
+    }
+    int rc;
+    if (p.b_arr) {
+        p.b = const_cast<float *>(p.b_arr);
+    } else if ((rc = cached_scratch(bslot, p.slot_elems, &p.b))) {
+        return rc;
+    }
+    p.use_tma = ok && kernel != 1;
+    if (!p.use_tma) return B2_OK;
+    return R == 2 ? nested_maps<2>(p, f, fslots, p.b, p.tm_f, p.tm_b, who)
+                  : nested_maps<4>(p, f, fslots, p.b, p.tm_f, p.tm_b, who);
+}
+
+// One sweep of k_nested_tma<R, Epi> over plan p's box with its weights and maps, f at slot `slot0` of tm_f. The
+// variant is noted as "<name>_tma<R>" (b2_last_sweep_kernel), with "+adj" on the adjoint.
 template <int R, class Epi>
-int launch_nested_tma(const Box &p, const float (*c)[B2_MAX_RADIUS], const CUtensorMap &tm_f, const CUtensorMap &tm_b,
-                      int slot0, const Epi &epi, const char *name, bool adjoint) {
+int launch_nested_tma(const NestedPlan &p, int slot0, const Epi &epi, const char *name) {
     using Cf = NestedCfg<R>;
     auto kern = k_nested_tma<R, Epi>;
     static bool attr_set = false;           // the shared-memory size is opted into before the first launch
@@ -257,14 +312,39 @@ int launch_nested_tma(const Box &p, const float (*c)[B2_MAX_RADIUS], const CUten
     k.lx = std::min(choose_chunk_len(sms, k.ntz * k.nty, p.n[0], 4 * R - 2, 32), p.n[0]);
     k.slot0 = slot0;
     for (int i = 0; i < R; ++i) {
-        k.cx[i] = c[0][i];
-        k.cy[i] = c[1][i];
-        k.cz[i] = c[2][i];
+        k.cx[i] = p.c[0][i];
+        k.cy[i] = p.c[1][i];
+        k.cz[i] = p.c[2][i];
     }
     const int ntx = (p.n[0] + k.lx - 1) / k.lx;
     timing_begin();
-    note_sweep_kernel("%s_tma<%d>%s", name, R, adjoint ? "+adj" : "");
-    kern<<<k.ntz * k.nty * ntx, Cf::TY * Cf::TZ4 + 32, Cf::SMEM, stream()>>>(tm_f, tm_b, args);
+    note_sweep_kernel("%s_tma<%d>%s", name, R, p.adjoint ? "+adj" : "");
+    kern<<<k.ntz * k.nty * ntx, Cf::TY * Cf::TZ4 + 32, Cf::SMEM, stream()>>>(p.tm_f, p.tm_b, args);
+    timing_end();
+    count_launch();
+    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
+    return B2_OK;
+}
+
+// One sweep of a one-thread-per-point kernel (k_sa_generic, k_visco_generic) over plan p's box: fills the members its
+// argument K shares with the others (strides, box, radius and weights; the caller sets the rest) and launches 64 x 4
+// threads per block on z and y, blocks looping over x. The variant is noted as "<name>_generic", with "+adj" on the
+// adjoint.
+template <class K>
+int launch_nested_generic(void (*kern)(K), K k, const NestedPlan &p, const char *name) {
+    k.sx = p.sx;
+    k.sy = p.sy;
+    k.n0 = p.n[0]; k.n1 = p.n[1]; k.n2 = p.n[2];
+    k.o0 = p.o[0]; k.o1 = p.o[1]; k.o2 = p.o[2];
+    for (int d = 0; d < 3; ++d) {
+        k.r[d] = p.radius[d];
+        for (int i = 0; i < B2_MAX_RADIUS; ++i) k.c[d][i] = p.c[d][i];
+    }
+    dim3 block(64, 4, 1);
+    dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
+    timing_begin();
+    note_sweep_kernel("%s_generic%s", name, p.adjoint ? "+adj" : "");
+    kern<<<grid, block, 0, stream()>>>(k);
     timing_end();
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);

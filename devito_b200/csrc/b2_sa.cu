@@ -12,6 +12,10 @@
 //   sa_tma<R>    : the 2.5-D TMA sweep of the nested operator shared with the viscoacoustic update
 //                  (k_nested_tma<R, SaEpi>, b2_nested.cuh; 3-D grids, R in {2, 4}) on u[t]. Its epilogue SaEpi reads C,
 //                  w and u[t-dir] once with 16-byte loads and writes u[t+dir] with 16-byte stores.
+//
+// The host side is the nested operator's (b2_nested.cuh): nested_plan_init chooses the kernel, points b at the array
+// or at g_sa_scratch[1] and encodes the maps of u and b; sa_plan_init adds C and runs k_sa_coef, and sa_step fills the
+// epilogue or the SaK members of its own before launch_nested_tma / launch_nested_generic.
 #include "b2_sa.cuh"
 #include "b2_sa_point.cuh"
 #include "b2_nested.cuh"
@@ -71,46 +75,22 @@ __global__ void __launch_bounds__(256) k_sa_coef(float *__restrict__ C, float *_
 static ScratchSlot g_sa_scratch[2];
 
 int sa_plan_init(SaPlan &p, int kernel) {
-    if (kernel != 0 && kernel != 1 && kernel != 2) {
-        set_error("b2_sa_forward: unknown kernel %d", kernel);
-        return B2_ERR_INVALID;
-    }
     int rc;
+    if ((rc = nested_plan_init(p, kernel, "b2_sa_forward", g_sa_scratch[1], {p.u, p.w}, p.u, p.tsize))) return rc;
     if ((rc = cached_scratch(g_sa_scratch[0], p.slot_elems, &p.C))) return rc;
-    if (p.b_arr) {
-        p.b = const_cast<float *>(p.b_arr);
-    } else if ((rc = cached_scratch(g_sa_scratch[1], p.slot_elems, &p.b))) {
-        return rc;
-    }
     const size_t n = p.slot_elems;
     const int blocks = (int)std::min<size_t>((n + 255) / 256, 65535);
     k_sa_coef<<<blocks, 256, 0, stream()>>>(p.C, p.b_arr ? nullptr : p.b, p.vp_arr, p.b_arr, p.vp_value, p.b_value,
                                             p.dt * p.dt, n);
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
-    // the TMA sweep: 3-D, R in {2, 4} on every axis, z rows and the box start 16-byte aligned (the conditions of
-    // k_iso_tma: so % 4 == 0 and nz % 4 == 0 make the row pitch a multiple of 4 floats)
-    const int R = p.radius[2];
-    bool ok = p.radius[0] == R && p.radius[1] == R && (R == 2 || R == 4);
-    ok = ok && p.a[2] % 4 == 0 && p.o[2] % 4 == 0 && p.slot_elems % 4 == 0;
-    ok = ok && (uintptr_t)p.u % 16 == 0 && (uintptr_t)p.b % 16 == 0 && (uintptr_t)p.C % 16 == 0;
-    ok = ok && (uintptr_t)p.w % 16 == 0;
-    if (kernel == 2 && !ok) {
-        set_error("b2_sa_forward: TMA kernel forced but the layout does not qualify (3-D, radius 2 or 4, z extent "
-                  "and z start multiples of 4, 16-byte aligned arrays; radius=%d a2=%d o2=%d)", R, p.a[2], p.o[2]);
-        return B2_ERR_INVALID;
-    }
-    p.use_tma = ok && kernel != 1;
-    if (!p.use_tma) return B2_OK;
-    return R == 2 ? nested_maps<2>(p, p.u, p.tsize, p.b, p.tm_u, p.tm_b, "b2_sa_forward")
-                  : nested_maps<4>(p, p.u, p.tsize, p.b, p.tm_u, p.tm_b, "b2_sa_forward");
+    return B2_OK;
 }
 
 int sa_step(const SaPlan &p, int slot0, int slotm, int slot1) {
     if (p.use_tma) {
         const SaEpi e{p.u + (size_t)slotm * p.slot_elems, p.u + (size_t)slot1 * p.slot_elems, p.C, p.w, p.dt};
-        return p.radius[2] == 2 ? launch_nested_tma<2>(p, p.c, p.tm_u, p.tm_b, slot0, e, "sa", p.adjoint)
-                                : launch_nested_tma<4>(p, p.c, p.tm_u, p.tm_b, slot0, e, "sa", p.adjoint);
+        return p.radius[2] == 2 ? launch_nested_tma<2>(p, slot0, e, "sa") : launch_nested_tma<4>(p, slot0, e, "sa");
     }
     SaK k;
     k.u0 = p.u + (size_t)slot0 * p.slot_elems;
@@ -119,24 +99,8 @@ int sa_step(const SaPlan &p, int slot0, int slotm, int slot1) {
     k.b = p.b;
     k.C = p.C;
     k.w = p.w;
-    k.sx = p.sx;
-    k.sy = p.sy;
-    k.n0 = p.n[0]; k.n1 = p.n[1]; k.n2 = p.n[2];
-    k.o0 = p.o[0]; k.o1 = p.o[1]; k.o2 = p.o[2];
-    for (int d = 0; d < 3; ++d) {
-        k.r[d] = p.radius[d];
-        for (int i = 0; i < B2_MAX_RADIUS; ++i) k.c[d][i] = p.c[d][i];
-    }
     k.dt = p.dt;
-    dim3 block(64, 4, 1);
-    dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
-    timing_begin();
-    note_sweep_kernel(p.adjoint ? "sa_generic+adj" : "sa_generic");
-    k_sa_generic<<<grid, block, 0, stream()>>>(k);
-    timing_end();
-    count_launch();
-    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
-    return B2_OK;
+    return launch_nested_generic(k_sa_generic, k, p, "sa");
 }
 
 }  // namespace b2

@@ -17,6 +17,11 @@
 // Algorithmic bytes per point and step (DESIGN §3.3k): forward 44 (p[t], b, p[t-1], r[t], five tables; writes r[t+1],
 // p[t+1]); adjoint 64 (the mix reads p[t], r[t], Kd, Kg, Kt, b and writes r[t-1], s: 32; the sweep reads s, b, p[t],
 // p[t+1], Kd, W, Wm and writes p[t-1]: 32).
+//
+// The host side is the nested operator's (b2_nested.cuh): nested_plan_init chooses the kernel, points b at the array
+// or at g_visco_scratch[VK_NTAB] and encodes the maps of p (or s) and b; visco_plan_init adds s and the tables and runs
+// k_visco_coef, and visco_step fills the epilogue or the ViscoK members of its own before launch_nested_tma /
+// launch_nested_generic.
 #include "b2_visco.cuh"
 #include "b2_nested.cuh"
 #include <algorithm>
@@ -103,8 +108,7 @@ static int visco_step_tma(const ViscoPlan &p, int t0, int t2, int t1) {
     e.r1 = ADJ ? nullptr : at(p.r, t1);
     for (int i = 0; i < VK_NTAB; ++i) e.K[i] = p.K[i];
     const int slot0 = ADJ ? 0 : t0;
-    return p.radius[2] == 2 ? launch_nested_tma<2>(p, p.c, p.tm_f, p.tm_b, slot0, e, "visco", ADJ)
-                            : launch_nested_tma<4>(p, p.c, p.tm_f, p.tm_b, slot0, e, "visco", ADJ);
+    return p.radius[2] == 2 ? launch_nested_tma<2>(p, slot0, e, "visco") : launch_nested_tma<4>(p, slot0, e, "visco");
 }
 
 // the tables of b2_visco_point.cuh over the slot (and bx = b when b is a scalar), evaluated in double
@@ -117,30 +121,15 @@ __global__ void __launch_bounds__(256) k_visco_coef(ViscoCoefK k) {
 static ScratchSlot g_visco_scratch[VK_NTAB + 2];
 
 int visco_plan_init(ViscoPlan &p, int kernel) {
-    if (kernel != 0 && kernel != 1 && kernel != 2) {
-        set_error("b2_visco_forward: unknown kernel %d", kernel);
-        return B2_ERR_INVALID;
-    }
-    // the TMA sweep: 3-D, R in {2, 4} on every axis, z rows and the box start 16-byte aligned (the conditions of
-    // the self-adjoint sweep)
-    const int R = p.radius[2];
-    bool ok = p.radius[0] == R && p.radius[1] == R && (R == 2 || R == 4);
-    ok = ok && p.a[2] % 4 == 0 && p.o[2] % 4 == 0 && p.slot_elems % 4 == 0;
-    ok = ok && (uintptr_t)p.p % 16 == 0 && (uintptr_t)p.r % 16 == 0 && (uintptr_t)p.b_arr % 16 == 0;
-    if (kernel == 2 && !ok) {
-        set_error("b2_visco_forward: TMA kernel forced but the layout does not qualify (3-D, radius 2 or 4, z extent "
-                  "and z start multiples of 4, 16-byte aligned arrays; radius=%d a2=%d o2=%d)", R, p.a[2], p.o[2]);
-        return B2_ERR_INVALID;
-    }
     int rc;
+    // the TMA sweep's ring streams p[t] forward (every slot of p, the slot a coordinate) and the single slot s on the
+    // adjoint, so s comes before the maps
+    if (p.adjoint && (rc = cached_scratch(g_visco_scratch[VK_NTAB + 1], p.slot_elems, &p.s))) return rc;
+    if ((rc = nested_plan_init(p, kernel, "b2_visco_forward", g_visco_scratch[VK_NTAB], {p.p, p.r},
+                               p.adjoint ? p.s : p.p, p.adjoint ? 1 : p.tsize)))
+        return rc;
     for (int i = 0; i < VK_NTAB; ++i)
         if ((rc = cached_scratch(g_visco_scratch[i], p.slot_elems, &p.K[i]))) return rc;
-    if (p.b_arr) {
-        p.b = const_cast<float *>(p.b_arr);
-    } else if ((rc = cached_scratch(g_visco_scratch[VK_NTAB], p.slot_elems, &p.b))) {
-        return rc;
-    }
-    if (p.adjoint && (rc = cached_scratch(g_visco_scratch[VK_NTAB + 1], p.slot_elems, &p.s))) return rc;
     const size_t n = p.slot_elems;
     const int blocks = (int)std::min<size_t>((n + 255) / 256, 65535);
     ViscoCoefK ck;
@@ -153,13 +142,7 @@ int visco_plan_init(ViscoPlan &p, int kernel) {
     k_visco_coef<<<blocks, 256, 0, stream()>>>(ck);
     count_launch();
     B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
-    p.use_tma = ok && kernel != 1;
-    if (!p.use_tma) return B2_OK;
-    // forward: the ring streams p[t] (every slot of p, the slot a coordinate); adjoint: the single slot s
-    const float *f = p.adjoint ? p.s : p.p;
-    const int fslots = p.adjoint ? 1 : p.tsize;
-    return R == 2 ? nested_maps<2>(p, f, fslots, p.b, p.tm_f, p.tm_b, "b2_visco_forward")
-                  : nested_maps<4>(p, f, fslots, p.b, p.tm_f, p.tm_b, "b2_visco_forward");
+    return B2_OK;
 }
 
 static int visco_mix(const ViscoPlan &p, int t0, int t2, int t1) {
@@ -198,24 +181,8 @@ int visco_step(const ViscoPlan &p, int t0, int t2, int t1) {
     k.r1 = p.adjoint ? nullptr : at(p.r, t1);
     k.b = p.b;
     for (int i = 0; i < VK_NTAB; ++i) k.K[i] = p.K[i];
-    k.sx = p.sx;
-    k.sy = p.sy;
-    k.n0 = p.n[0]; k.n1 = p.n[1]; k.n2 = p.n[2];
-    k.o0 = p.o[0]; k.o1 = p.o[1]; k.o2 = p.o[2];
-    for (int d = 0; d < 3; ++d) {
-        k.r[d] = p.radius[d];
-        for (int i = 0; i < B2_MAX_RADIUS; ++i) k.c[d][i] = p.c[d][i];
-    }
     k.adjoint = p.adjoint ? 1 : 0;
-    dim3 block(64, 4, 1);
-    dim3 grid((k.n2 + 63) / 64, (k.n1 + 3) / 4, (unsigned)std::min(k.n0, 65535));
-    timing_begin();
-    note_sweep_kernel(p.adjoint ? "visco_generic+adj" : "visco_generic");
-    k_visco_generic<<<grid, block, 0, stream()>>>(k);
-    timing_end();
-    count_launch();
-    B2_CUDA(cudaGetLastError(), B2_ERR_LAUNCH);
-    return B2_OK;
+    return launch_nested_generic(k_visco_generic, k, p, "visco");
 }
 
 }  // namespace b2

@@ -1727,10 +1727,9 @@ class Operator:
                 raise InvalidArgument(f"the override of `{s.obj.name}` must be {_OVERRIDE_KINDS[s.check]}")
         args['fields'] = [args[m] for m in ('u', 'v') if m in args]
         if grid.distributor.is_parallel:
-            if p['kind'] == 'sa':
-                raise InvalidArgument("the self-adjoint update does not run on a decomposed grid in this version")
-            if p['kind'] == 'visco':
-                raise InvalidArgument("the SLS viscoacoustic update does not run on a decomposed grid in this version")
+            if p['kind'] in ('sa', 'visco'):
+                name = {'sa': "self-adjoint", 'visco': "SLS viscoacoustic"}[p['kind']]
+                raise InvalidArgument(f"the {name} update does not run on a decomposed grid in this version")
             if p['kind'] == 'tti' and grid.dim == 2:
                 raise InvalidArgument("2-D TTI modelling does not run on a decomposed grid in this version")
             if p['kind'] == 'tti' and p.get('adjoint'):
@@ -2022,13 +2021,13 @@ class Operator:
         if p['kind'] == 'linear':
             return float(2 * len(p['taps'])), 4.0 * (len({t for t, _, _ in p['taps']}) + 1)
         R, nd = p['R'], p['grid'].dim
-        if p['kind'] == 'sa':
-            # per axis 2R fluxes of R multiply-adds and a multiply, then R outer multiply-adds; the update 6
-            return float(nd * (2 * R * (2 * R + 1) + 2 * R) + 6), 24.0
-        if p['kind'] == 'visco':
-            # the nested operator as for 'sa'; the epilogue of b2_visco_point.cuh 16 (forward) or the mix 8 and the
-            # update 6 (adjoint); bytes of DESIGN §3.3k
+        if p['kind'] in ('sa', 'visco'):
+            # the nested operator: per axis 2R fluxes of R multiply-adds and a multiply, then R outer multiply-adds
             lap = nd * (2 * R * (2 * R + 1) + 2 * R)
+            if p['kind'] == 'sa':
+                return float(lap + 6), 24.0                 # the update 6
+            # the epilogue of b2_visco_point.cuh 16 (forward) or the mix 8 and the update 6 (adjoint); bytes of
+            # DESIGN §3.3k
             return (float(lap + 14), 64.0) if p.get('adjoint') else (float(lap + 16), 44.0)
         star = 1 + nd * R * 3                       # centre mul + per tap pair: add, multiply-add
         if p['kind'] == 'iso':

@@ -2,14 +2,14 @@
 
 CPU (tests/support/emu_box.cu, nvcc host build): the box of `x_m .. z_M` in the internal 3-dim convention (a 1-D or
 2-D grid gets leading dummy dims of extent 1) against numpy's own view of that box, and the reach rule of the wave
-calls: a box grown by the stencil's reach (iso: radius r, TTI: R, SA: 2R-1) must stay inside the allocation, dim 0, 1,
-2 in turn, where an empty extent means "nothing to do".
+calls: a box grown by the stencil's reach (iso: radius r, TTI: R, SA and SLS: 2R-1) must stay inside the allocation,
+dim 0, 1, 2 in turn, where an empty extent means "nothing to do".
 
-GPU, called through the ABI on tiny 2-D and 3-D grids (host arrays, `dmap` NULL): for b2_iso_forward, b2_tti_forward
-and b2_sa_forward, a box whose reach passes the allocation by one cell is refused (210) with every host array
-byte-identical, the box one cell smaller matches the float64 references (ref64, tti2d_ref, sa_ref), an empty box
-writes nothing, and a sparse radius beyond the halo is refused; errctl stops TTI and SA on an Inf (100) and still
-writes the arrays back; the timers report section0 for TTI, SA and the linear update.
+GPU, called through the ABI on tiny 2-D and 3-D grids (host arrays, `dmap` NULL): for b2_iso_forward, b2_tti_forward,
+b2_sa_forward and b2_visco_forward, a box whose reach passes the allocation by one cell is refused (210) with every
+host array byte-identical, the box one cell smaller matches the float64 references (ref64, tti2d_ref, sa_ref,
+visco_ref), an empty box writes nothing, and a sparse radius beyond the halo is refused; errctl stops TTI, SA and SLS
+on an Inf (100) and still writes the arrays back; the timers report section0 for TTI, SA and the linear update.
 """
 import ctypes
 import os
@@ -22,6 +22,7 @@ import pytest
 import ref64
 import sa_ref
 import tti2d_ref
+import visco_ref
 from helpers import rel_linf
 from oracle import oracle as O
 
@@ -95,7 +96,7 @@ def test_box_layout(emu, nd):
 
 
 # reach of each wave update at space order 8: (name, reach)
-RULES = [('iso', 4), ('tti', 4), ('sa', 2 * 4 - 1), ('iso_r1', 1)]
+RULES = [('iso', 4), ('tti', 4), ('sa', 2 * 4 - 1), ('visco', 2 * 4 - 1), ('iso_r1', 1)]
 
 
 @pytest.mark.parametrize('rule,reach', RULES, ids=[r for r, _ in RULES])
@@ -143,9 +144,10 @@ SO = 4
 K = 4                                   # time steps 1 .. K
 NT = K + 2
 SHAPES = {2: (14, 12), 3: (9, 10, 12)}
-TOL = {'iso': 1e-5, 'tti': 1e-4, 'sa': 1e-5}
-REACH = {'iso': SO // 2, 'tti': SO // 2, 'sa': SO - 1}      # radius SO/2 everywhere; SA's nested stencil 2R-1
-FN = {'iso': 'b2_iso_forward', 'tti': 'b2_tti_forward', 'sa': 'b2_sa_forward'}
+TOL = {'iso': 1e-5, 'tti': 1e-4, 'sa': 1e-5, 'visco': 2e-5}
+REACH = {'iso': SO // 2, 'tti': SO // 2, 'sa': SO - 1, 'visco': SO - 1}   # radius SO/2; the nested stencil 2R-1
+FN = {'iso': 'b2_iso_forward', 'tti': 'b2_tti_forward', 'sa': 'b2_sa_forward', 'visco': 'b2_visco_forward'}
+F0 = 0.01                               # the SLS reference frequency
 
 
 def _L():
@@ -240,6 +242,18 @@ class Call:
         a.b_value, a.vp_value, a.dt = 1.25, 2.0, 0.9
         self.dt = 0.9
 
+    def _visco(self, errctl, born):
+        a = self.a = _L().ViscoArgs()
+        R = SO // 2
+        a.ndim, a.space_order, a.radius = self.nd, SO, R
+        self.c64 = [sa_ref.sa_weights(R, H)] * self.nd
+        a.c = self.weights(self.c64)
+        self.host['r'] = self.noise((3,) + self.alloc, 0.1)
+        self.host['damp'] = 1.0 - self.host['damp']                         # a mask profile in [0.9, 1]
+        a.u, a.r, a.damp = (self.obj(self.host[k]) for k in ('u', 'r', 'damp'))
+        a.b_value, a.vp_value, a.qp_value, a.f0, a.dt = 1.25, 2.0, 30.0, F0, 0.9
+        self.dt = 0.9
+
     def run(self):
         """(return code, message, host arrays before the call); the call releases its staging"""
         L = _L().lib()
@@ -262,6 +276,10 @@ class Call:
         if self.kind == 'sa':
             u, tr = sa_ref.sa_forward(before['u'], SO, self.c64, self.dt, 1, K, 1.25, 2.0, w=before['damp'], **kw)
             return dict(u=u), tr
+        if self.kind == 'visco':
+            u, r, tr = visco_ref.visco_forward(before['u'], before['r'], SO, self.c64, self.dt,
+                                               float(np.float32(F0)), 1, K, 1.25, 2.0, 30.0, damp=before['damp'], **kw)
+            return dict(u=u, r=r), tr
         if self.nd == 3:
             u, v, tr = ref64.tti_forward(before['u'], before['v'], SO, self.w2, self.w1, self.dt, 1, K,
                                          before['damp'], self.params, **kw)
@@ -277,7 +295,7 @@ def _touching(nd, reach):
     return [reach - SO] * nd, [n - 1 + SO - reach for n in SHAPES[nd]]
 
 
-CASES = [(k, nd) for k in ('iso', 'tti', 'sa') for nd in (2, 3)]
+CASES = [(k, nd) for k in ('iso', 'tti', 'sa', 'visco') for nd in (2, 3)]
 IDS = [f'{k}-{nd}d' for k, nd in CASES]
 
 
@@ -350,7 +368,7 @@ def _stopped_on_nan(c, field, written):
 def test_errctl_stops_on_inf_in_u(kind, nd):
     c = Call(kind, nd, [0] * nd, [n - 1 for n in SHAPES[nd]], errctl=1)
     _plant_inf(c, 'u')
-    _stopped_on_nan(c, 'u', ['u'])
+    _stopped_on_nan(c, 'p' if kind == 'visco' else 'u', ['u'])
 
 
 @pytest.mark.gpu
